@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- forward+backward views/sec of the Gaussian-splat rasterizer hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Metric (BASELINE.json): forward+backward views/sec @ 3M Gaussians, 1920x1080, SH degree 3,
 plus achieved HBM GB/s of the dominant kernel vs the measured peak.  One "step" = one view
@@ -13,12 +13,19 @@ Prints ONE JSON line (rank 0).  Keys are documented in DESIGN.md section "Measur
   value        views/s, inputs resident in HBM, CUDA-event timed, max over ranks
   e2e          views/s through the public drop-in API with per-step host->device copies of the
                view's camera + upstream image gradient (pinned) and a device->host loss read
-  roofline     dominant kernel: algorithmic bytes / CUDA-event duration vs MEASURED_PEAKS.json
+  roofline     dominant kernel: algorithmic bytes / CUDA-event duration vs MEASURED_PEAKS.json (else the
+               H100 SXM data sheet's 3.35 TB/s)
   cpu_baseline the CPU oracle (scalar C port of the reference) on a bounded sample
 --impl reference runs the UNMODIFIED reference CUDA build (oracle/_ref) through its own
 GaussianRasterizer on the same tensors and protocol (the reference has no CPU rasterizer; its
 CUDA build is the baseline BASELINE.md section 2 names), falling back to the CPU oracle port
 when oracle/_ref is absent.
+--dump-outputs DIR writes what the last timed step computed (rank 0) as DIR/<name>.npy (float32 / float64), at
+most DUMP_LIMIT bytes in all: radii plus every parameter's gradient at a fixed seeded sample of up to DUMP_SAMPLE
+Gaussians (sample_index.npy), and the image of its last view -- whole (image.npy) when it fits the rest of the
+budget, else at a fixed seeded sample of pixels (image_sample.npy [3, n], pixel_index.npy = y * width + x).  The
+inputs are seeded, so two builds run with the same arguments can be compared output for output.  Only the
+rasterizer workloads (raster, c5) dump; the others reject the flag.
 """
 import argparse
 import json
@@ -36,6 +43,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 METRIC = "forward+backward views/sec @3M Gaussians 1920x1080"
+DUMP_SAMPLE = 131072   # Gaussians whose per-Gaussian outputs --dump-outputs keeps (~34 MB at SH degree 3)
+DUMP_LIMIT = 64_000_000   # bytes --dump-outputs may write in all, .npy headers included
 
 
 def load_scenes():
@@ -74,13 +83,15 @@ def parse():
     ap.add_argument("--exchange", default="auto", choices=["auto", "peer", "nccl"],
                     help="N>1: how the ranks' gradients meet inside the backward.  peer: the peer-memory kernels "
                          "(csrc/sgr_peer.cu: CUDA IPC mappings, flags, TMA loads / stores over NVLink); nccl: all-gather + "
-                         "chunked all-reduce; auto (default): peer on the world sizes it was measured faster on "
+                         "chunked all-reduce; auto (default): peer on the world sizes the design gives to it, not timed on H100 "
                          "(sugar_b200.parallel.PEER_AUTO_WORLDS), else nccl")
     ap.add_argument("--peer", action="store_true", help="same as --exchange peer")
     ap.add_argument("--no-taper", action="store_true",
                     help="N>1, peer exchange: equal chunks instead of halving ones")
     ap.add_argument("--force-exchange", action="store_true",
                     help="diagnostic, N=1: run the exchange path's kernels (factor-mode backward + finalize) without NCCL")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (image, sampled radii and gradients)")
     args = ap.parse_args()
     if args.peer:
         args.exchange = "peer"
@@ -96,16 +107,6 @@ def parse():
 KERNEL_BOUND = {"preprocess": "hbm", "preprocess_backward": "hbm", "scatter": "l2-atomics", "tile_scan": "latency",
                 "tile_sort_smem": "shared-memory", "tile_sort_global": "l2", "blend_forward": "fp32-issue",
                 "blend_backward": "fp32-issue", "field_forward": "hbm", "field_backward": "l2-atomics"}
-
-
-def load_ncu_facts():
-    """Per-kernel facts from the committed ncu capture (profiles/ncu_kernels.json, written by
-    scripts/summarize_ncu.py): DRAM bytes and warp-instructions per launch at the headline workload."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_kernels.json")) as f:
-            return json.load(f)
-    except Exception:
-        return {}
 
 
 def algorithmic_bytes(P, V, R, W, H, M, D, sh_written=True):
@@ -125,7 +126,7 @@ def algorithmic_bytes(P, V, R, W, H, M, D, sh_written=True):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -178,7 +179,7 @@ def load_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s), not measured"
 
 
 def _cpu_sample(job):
@@ -296,6 +297,39 @@ def verify_exchange(torch, dist, mod, parallel, scenes, dev, rank, world, D, sh_
     return out
 
 
+def dump_outputs(out_dir, last, P):
+    """--dump-outputs: radii and the gradients at up to DUMP_SAMPLE seeded Gaussian indices, then the image, whole
+    if it fits what is left of DUMP_LIMIT, else at as many seeded pixels as fit."""
+    import torch
+    header = 128   # bytes of an .npy header for these shapes
+    per_gauss = {("radii" if k == "radii" else "dL_d" + k): v for k, v in last.items() if k != "color" and v is not None}
+    row_bytes = 8 + sum(4 * (v[0].numel() if v.dim() > 1 else 1) for v in per_gauss.values())   # + sample_index
+    n = min(P, DUMP_SAMPLE, int(0.55 * DUMP_LIMIT) // row_bytes)
+    idx = np.arange(P) if n == P else np.sort(np.random.default_rng(0).choice(P, n, replace=False))
+    arrays = {"sample_index": idx.astype(np.float64)}
+    sel = torch.from_numpy(idx).to(last["color"].device)
+    for name, v in per_gauss.items():
+        arrays[name] = v.detach().index_select(0, sel).float().cpu().numpy()
+    image = last["color"].detach().float()
+    room = DUMP_LIMIT - sum(a.nbytes + header for a in arrays.values()) - 2 * header
+    if image.numel() * 4 <= room:
+        arrays["image"] = image.cpu().numpy()
+    else:
+        C, H, W = image.shape
+        k = min(H * W, room // (4 * C + 8))
+        px = np.sort(np.random.default_rng(1).choice(H * W, k, replace=False))
+        arrays["image_sample"] = image.reshape(C, H * W)[:, torch.from_numpy(px).to(image.device)].cpu().numpy()
+        arrays["pixel_index"] = px.astype(np.float64)
+    total = sum(a.nbytes + header for a in arrays.values())
+    if total > DUMP_LIMIT:
+        raise RuntimeError(f"--dump-outputs: {total} bytes over the {DUMP_LIMIT}-byte budget")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    return {"dir": out_dir, "arrays": sorted(arrays), "bytes": int(total), "gaussians_sampled": int(n),
+            "image": "whole" if "image" in arrays else f"{len(arrays['pixel_index'])} seeded pixels"}
+
+
 def main():
     args = parse()
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -305,6 +339,8 @@ def main():
         args.gaussians, args.width, args.height = args.gaussians or 6_000_000, args.width or 3840, args.height or 2160
         args.views_per_step = args.views_per_step or 8
     elif args.workload != "raster":
+        if args.dump_outputs:
+            raise SystemExit(f"--dump-outputs: --workload {args.workload} has no output dump (raster and c5 have)")
         if rank != 0:
             return 0  # single-GPU workloads: rank 0 alone runs them
         import bench_workloads
@@ -333,7 +369,9 @@ def main():
             mod = h.load_ref_module()
             use_ref = True
         else:
-            # no reference CUDA build on this box: the CPU oracle port is the reference arm
+            # no reference CUDA build on this machine: the CPU oracle port is the reference arm
+            if args.dump_outputs:
+                raise SystemExit("--dump-outputs needs a CUDA path; the CPU oracle arm has no timed GPU step")
             cb = cpu_baseline(args)
             print(json.dumps({"metric": METRIC, "value": cb["value"], "unit": "views/s", "n_gpus": 1,
                               "steps": 1, "warmup": 0, "ms_per_step": 1000.0 / cb["value"], "higher_is_better": True,
@@ -401,6 +439,8 @@ def main():
             p.grad = None
         means2D.grad = None
 
+    last = {}   # --dump-outputs: the most recent step's outputs (references; no copy inside the step)
+
     def step_device():
         for view in views:   # this rank's views of the batch: each backward runs its own exchange
             vm, pm, cp, b, g = view["dev"]
@@ -408,6 +448,8 @@ def main():
             color, radii = rast(means3D=params["means3D"], means2D=means2D, opacities=params["opacities"],
                                 shs=params["shs"], scales=params["scales"], rotations=params["rotations"])
             torch.autograd.backward(color, g)
+        if args.dump_outputs:
+            last.update(color=color, radii=radii, means2D=means2D.grad, **{k: p.grad for k, p in params.items()})
         zero_grads()
         return radii
 
@@ -507,6 +549,7 @@ def main():
     t_timed0 = time.perf_counter()
     ms = timed(step_device, args.steps)
     t_timed1 = time.perf_counter()
+    dump = dict(last)
     launches = 0 if use_ref else int(_lib.lib.sgr_launch_count() - launches0)
     prof = {}
     if profile_in_timed:
@@ -575,7 +618,7 @@ def main():
     out["gpu_launches"] = launches
     if use_ref:
         out["impl"] = "reference"
-        out["impl_note"] = "unmodified diff-gaussian-rasterization CUDA sources compiled for sm_100a (oracle/_ref)"
+        out["impl_note"] = "unmodified diff-gaussian-rasterization CUDA sources compiled for sm_90a (oracle/_ref)"
         out["gpu_launches"] = 0
     if rank == 0 and not use_ref:
         # R of this view for the byte model
@@ -589,9 +632,6 @@ def main():
         used_peer = bool((exchange_check or {}).get("peer_memory")) or (args.force_exchange and args.exchange != "nccl")
         alg = algorithmic_bytes(P, V_vis, R, W, H, 16, D, sh_written=(world == 1 or args.no_sh_factors or used_peer))
         peak, peak_src = load_peaks()
-        ncu = load_ncu_facts()
-        sm_clock = (clk.get("sm_mhz") or 1965.0) * 1e6
-        issue_peak = 148 * 4 * sm_clock  # warp-instructions / s the chip can issue at the measured clock
         stages = {}
         for name, (tot, cnt) in prof.items():
             avg_ms = tot / cnt
@@ -604,24 +644,12 @@ def main():
                   "gbs": round(b / (pass_ms * 1e-3) / 1e9, 1) if b else None,
                   "hbm_frac": round(b / (pass_ms * 1e-3) / 1e9 / peak, 4) if b else None,
                   "bound": KERNEL_BOUND.get(name, "latency")}
-            inst = (ncu.get(name) or {}).get("warp_instructions")
-            if inst:
-                st["issue_frac"] = round(inst / (pass_ms * 1e-3) / issue_peak, 4)
             stages[name] = st
         dom = max(stages, key=lambda k: stages[k]["ms"] * stages[k]["launches_per_step"]) if stages else None
         if dom:
-            facts = ncu.get(dom) or {}
             out["roofline"] = {"kernel": dom, "bound": KERNEL_BOUND.get(dom, "hbm"), "achieved": stages[dom]["gbs"],
-                               "peak": peak, "unit": "GB/s",
-                               "frac": stages[dom]["hbm_frac"], "traffic": facts.get("dram_bytes"),
+                               "peak": peak, "unit": "GB/s", "frac": stages[dom]["hbm_frac"],
                                "peak_source": peak_src, "algorithmic_bytes": alg.get(dom)}
-            if facts.get("warp_instructions"):
-                # the blend kernels are FP32-issue bound (~256 pair evaluations per 40 bytes): their roofline
-                # is the issue rate, warp-instructions (ncu smsp__inst_executed.sum) / duration vs SMs x 4 x clock
-                out["roofline"]["issue"] = {
-                    "achieved": round(facts["warp_instructions"] / (stages[dom]["ms_per_view_pass"] * 1e-3) / 1e9, 1),
-                    "peak": round(issue_peak / 1e9, 1), "unit": "G warp-inst/s", "frac": stages[dom].get("issue_frac"),
-                    "warp_instructions": facts["warp_instructions"], "source": facts.get("source")}
             # the HBM-bound stages BASELINE.md holds to >= 60 % of peak
             out["roofline"]["hbm_stages"] = {k: v["hbm_frac"] for k, v in stages.items()
                                              if v["bound"] == "hbm" and v["hbm_frac"] is not None}
@@ -641,6 +669,8 @@ def main():
     if use_ref:
         out["cpu_baseline"] = {"value": out["value"], "unit": "views/s", "cores": 0, "kind": "reference",
                                "sample": "full workload on the GPU: the reference path has no CPU implementation"}
+    if rank == 0 and args.dump_outputs:
+        out["dumped"] = dump_outputs(args.dump_outputs, dump, P)
     if rank == 0:
         print(json.dumps(out))
     if dist is not None:

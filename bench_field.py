@@ -5,7 +5,7 @@
 
 BASELINE.md section 2 "B-cpu-density" / config 1 and 3: fused sugar_b200 kernels vs the reference's op chain
 (restated in oracle/field_oracle.py) run with PyTorch on the same GPU and on the host cores (bounded sample).
-Prints one JSON line.  Not the driver's bench (that is bench.py); numbers are copied to profiles/.
+Prints one JSON line.  The headline benchmark is bench.py.
 """
 import argparse
 import json

@@ -1,5 +1,5 @@
 /*
- * sugar_b200.h -- C ABI of libsugar_b200.so: a Blackwell (sm_100a) differentiable
+ * sugar_b200.h -- C ABI of libsugar_b200.so: a Hopper (sm_90a) differentiable
  * Gaussian-splat rasterizer + SuGaR density/SDF field evaluator.
  *
  * Drop-in boundary.  These entry points are what a binding of the reference's rasterizer

@@ -1,4 +1,4 @@
-"""Compile the UNMODIFIED reference CUDA rasterizer for sm_100a into oracle/_ref/.
+"""Compile the UNMODIFIED reference CUDA rasterizer for sm_90a into oracle/_ref/.
 
 The sources are compiled where they lie under /root/reference (never copied into the repo);
 only build products go to oracle/_ref/ (git-ignored, but shipped to the GPU box by gpurun):
@@ -8,9 +8,9 @@ only build products go to oracle/_ref/ (git-ignored, but shipped to the GPU box 
                                                             own Python wrapper (like pip --target)
 
 Flags follow the reference's setup.py (DGR/setup.py:29: no arch flags, no fast-math) plus
-`-gencode arch=compute_100a,code=sm_100a` and `-include cstdint` (gcc 13 needs it for
+`-gencode arch=compute_90a,code=sm_90a` and `-include cstdint` (gcc 13 needs it for
 rasterizer_impl.h; no source edit).  This is the parity oracle on the GPU and the
-"reference CUDA build on 1xB200" baseline of bench.py --impl reference.
+"reference CUDA build on 1xH100" baseline of bench.py --impl reference.
 """
 import os
 import shutil
@@ -41,7 +41,7 @@ def main() -> int:
         sources=srcs,
         extra_include_paths=[os.path.join(REF, "third_party/glm"), REF],
         extra_cflags=["-O3", "-include", "cstdint"],
-        extra_cuda_cflags=["-gencode", "arch=compute_100a,code=sm_100a", "-include", "cstdint"],
+        extra_cuda_cflags=["-gencode", "arch=compute_90a,code=sm_90a", "-include", "cstdint"],
         build_directory=build_dir,
         with_cuda=True,
         is_python_module=False,

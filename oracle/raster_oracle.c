@@ -26,7 +26,7 @@
  * depth, pixel position, 2-D covariance, radius and tile rectangle is written
  * with explicit fmaf()/plain ops in exactly the fused/unfused pattern that
  * nvcc 12.9 (-fmad=true, the reference's default flags) emits for the reference
- * sources on sm_100a (read off the PTX and SASS of the unmodified sources; the
+ * sources on sm_90a (read off the PTX and SASS of the unmodified sources; the
  * rule is "a*b + c*d + e*f" -> fma(e,f, fma(a,b, c*d)), plus a handful of
  * ptxas-level fusions noted inline).  Compile this file with -ffp-contract=off
  * so that gcc adds no contraction of its own.  expf() here is glibc's; the
@@ -34,7 +34,7 @@
  * gradients are compared with a tolerance, integer/index outputs exactly.
  *
  * Parity pinning: tests/golden/ holds outputs of the UNMODIFIED reference CUDA
- * build (oracle/_ref) run on a B200, and tests/test_oracle_golden.py checks this
+ * build (oracle/_ref) run on the GPU, and tests/test_oracle_golden.py checks this
  * file against them.
  */
 #include <math.h>

@@ -1,5 +1,5 @@
-"""Per-kernel SASS evidence of libsugar_b200.so -> profiles/<tag>_sass_summary.txt
-    python scripts/sass_summary.py r02
+"""Per-kernel SASS evidence of libsugar_b200.so, printed:
+    python scripts/sass_summary.py [tag] > sass_summary.txt
 Counts, per kernel, the mnemonics that prove the hardware paths DESIGN.md claims: UBLKCP (1-D TMA bulk copies,
 both directions), SYNCS (mbarrier transaction waits), LDGSTS (cp.async), REDG...F32x4 / F32x2 (vector
 reductions), ATOMG (returning atomics), MUFU.* (special-function unit), plus registers and static shared memory
@@ -49,8 +49,6 @@ def main(tag):
         reg, stack, sh = usage.get(k, (0, 0, 0))
         hits = "  ".join(f"{n}={c}" for n, c in counts[k].items() if c)
         out.append(f"{name:48s} inst={n_inst[k]:5d} REG={reg:3d} STACK={stack:3d} SHARED={sh:6d}  {hits}")
-    path = os.path.join(ROOT, "profiles", f"{tag}_sass_summary.txt")
-    open(path, "w").write("\n".join(out) + "\n")
     print("\n".join(out))
 
 

@@ -3,7 +3,7 @@
 signatures and return tuples, implemented over the C ABI of libsugar_b200.so.
 
 torch is used only for device memory (caching allocator), the current stream and the device
-guard; all arithmetic happens in the hand-written sm_100a kernels.
+guard; all arithmetic happens in the hand-written sm_90a kernels.
 """
 import contextlib
 import ctypes as C

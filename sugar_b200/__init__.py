@@ -1,4 +1,4 @@
-"""sugar_b200 -- Blackwell (sm_100a) rasterizer + density-field hot path for Anttwo/SuGaR.
+"""sugar_b200 -- Hopper (sm_90a) rasterizer + density-field hot path for Anttwo/SuGaR.
 
     sugar_b200.diff_gaussian_rasterization   drop-in for the reference's rasterizer module
     sugar_b200.field                         fused SuGaR density / SDF field (get_field_values)

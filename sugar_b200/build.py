@@ -1,9 +1,9 @@
-"""Build libsugar_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libsugar_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a.
 
     python sugar_b200/build.py        # or sugar_b200.build.build_library()
 
-The .so is git-ignored but travels to the GPU box with gpurun (built here; nvcc cross-compiles
-without a GPU).  No torch headers are involved: the boundary is plain C (include/sugar_b200.h).
+The .so is git-ignored; __graft_entry__.build() compiles it (nvcc cross-compiles for sm_90a without a
+GPU).  No torch headers are involved: the boundary is plain C (include/sugar_b200.h).
 """
 import os
 import subprocess
@@ -15,7 +15,7 @@ LIB = os.environ.get("SGR_LIB_OUT", os.path.join(HERE, "lib", "libsugar_b200.so"
 SOURCES = ["sgr_api.cu", "sgr_forward.cu", "sgr_backward.cu", "sgr_field.cu", "sgr_normal.cu", "sgr_knn.cu", "sgr_meshbind.cu",
            "sgr_peer.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--shared",
 ]
 

@@ -27,6 +27,14 @@ int cuda_fail(cudaError_t e, const char *what)
     return SGR_ECUDA;
 }
 
+int device_sm_count()
+{
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+        return 132;  // H100 SXM
+    return n;
+}
+
 // ---- launch counter + optional event profiling (not thread-safe: one profiling client at a time)
 static const char *const g_kind_names[K_NUM_KINDS] = {
     "preprocess", "tile_scan", "scatter", "tile_sort_smem", "tile_sort_global", "blend_forward", "blend_backward",
@@ -276,7 +284,7 @@ SGR_API int sgr_debug_blend_stats(unsigned long long *out16, int reset)
     return sgr::read_bwd_stats(out16 + 8, reset);
 }
 #endif
-const char *sgr_version(void) { return "sugar_b200 0.1 (sm_100a)"; }
+const char *sgr_version(void) { return "sugar_b200 0.1 (sm_90a)"; }
 
 size_t sgr_geometry_bytes(int32_t P) { return GeomState::bytes((size_t)(P < 0 ? 0 : P)); }
 size_t sgr_binning_bytes(int64_t capacity) { return BinState::bytes((size_t)(capacity < 0 ? 0 : capacity)); }

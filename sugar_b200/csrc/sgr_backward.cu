@@ -1,4 +1,4 @@
-// sgr_backward.cu -- backward path of the B200 rasterizer.
+// sgr_backward.cu -- backward path of the H100 rasterizer.
 //
 // Replaces (reference: gaussian_splatting/submodules/diff-gaussian-rasterization/cuda_rasterizer/)
 //   renderCUDA (backward)     backward.cu:399-557  -> blend_backward_kernel
@@ -662,7 +662,8 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
             if (a.cov_pre) bytes += PB_T * 24;
             // peer mode: the other views' factor blocks of these 64 Gaussians, one bulk copy per view straight out of
             // its owner GPU's memory (TMA over NVLink): the factors' all-gather is fused into this kernel's staging.
-            // (A separate, later-waited barrier for them measured slower: 0.308 vs 0.257 ms for 1.6 M Gaussians.)
+            // One barrier for everything: a separate, later-waited barrier for the pulled blocks adds a second wait
+            // to every CTA of a latency-bound pass.
             const int pulled = MULTI ? min(a.nviews - 1, PB_VB) : 0;
             bytes += (uint32_t)pulled * PB_T * 12;
             mbar_expect_tx(&s_bar, bytes);

@@ -1,4 +1,4 @@
-// sgr_forward.cu -- forward path of the B200 rasterizer.
+// sgr_forward.cu -- forward path of the H100 rasterizer.
 //
 // Replaces (reference: gaussian_splatting/submodules/diff-gaussian-rasterization/cuda_rasterizer/)
 //   preprocessCUDA            forward.cu:155-256      -> preprocess_kernel   (+ per-tile counting)
@@ -1140,7 +1140,8 @@ static int launch_binning_and_blend(const ViewConsts &v, int P, const GeomState 
                                                                img.counters, capacity, ids_packed(P) ? 1 : 0, bin.inst_a));
     sgr::prof_begin(K_SORT_SMEM, st);  // one timing bracket around the three size classes ...
     sgr::note_launches(2);             // ... but three launches
-    const int small_grid = T < 296 ? T : 296;  // 2 CTAs per SM, grid-stride over tiles
+    const int slots = 2 * device_sm_count();
+    const int small_grid = T < slots ? T : slots;  // 2 CTAs per SM, grid-stride over tiles
     tile_sort_merge_kernel<512, 0><<<T, 512 / SORT_VT, 512 * 8, st>>>(img.tile_start, img.counters, capacity, bin.inst_a,
                                                                       bin.plist, T);
 #ifdef SGR_SORT_MERGE_ONLY

@@ -1,4 +1,4 @@
-// sgr_internal.cuh -- shared declarations of libsugar_b200 (sm_100a only).
+// sgr_internal.cuh -- shared declarations of libsugar_b200 (sm_90a only).
 //
 // Layout of the three opaque round-trip buffers (the reference's GeometryState / BinningState /
 // ImageState, rasterizer_impl.h:30-63, are opaque to Python so the layout is ours):
@@ -110,6 +110,7 @@ struct ViewConsts {
 
 void set_error(const char *fmt, ...);
 int cuda_fail(cudaError_t e, const char *what);
+int device_sm_count();  // SMs of the current device (grid sizes of the grid-stride kernels)
 
 // Kernel bookkeeping: every launch of one of OUR kernels goes through SGR_LAUNCH so that
 // sgr_launch_count() is a measured number and, when profiling is switched on, each launch is

@@ -1,4 +1,4 @@
-// sgr_knn.cu -- exact K-nearest-neighbour search on a uniform grid (sm_100a).
+// sgr_knn.cu -- exact K-nearest-neighbour search on a uniform grid (sm_90a).
 //
 // Replaces pytorch3d.ops.knn_points as SuGaR uses it (pytorch3d 0.7.4 is not part of the reference
 // tree; call sites: sugar_scene/sugar_model.py:1013-1030 `reset_neighbors` = knn_points(points,
@@ -358,7 +358,7 @@ int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int
     uint32_t *bsums = (uint32_t *)p; p += align_up((nblocks + 1) * 4);
     float4 *sorted = (float4 *)p;
     SGR_LAUNCH(K_KNN, st, knn_bbox_init_kernel<<<1, 32, 0, st>>>(bb));
-    SGR_LAUNCH(K_KNN, st, knn_bbox_kernel<<<148 * 4, 256, 0, st>>>(P, points, bb));
+    SGR_LAUNCH(K_KNN, st, knn_bbox_kernel<<<device_sm_count() * 4, 256, 0, st>>>(P, points, bb));
     SGR_LAUNCH(K_KNN, st, knn_grid_setup_kernel<<<1, 32, 0, st>>>(bb, n, P, grid));
     SGR_CUDA(cudaMemsetAsync(cursor, 0, ncell * 4, st));  // cursor doubles as the count array first
     SGR_LAUNCH(K_KNN, st, knn_count_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, grid, cell_of, cursor));

@@ -326,7 +326,7 @@ int sgr_peer_reduce_records_synced(const void *const *rec_tab, void *const *sum_
     static const size_t cap = [] {
         const char *e = getenv("SGR_PEER_REDUCE_BLOCKS");
         const long v = e ? atol(e) : 0;
-        return (size_t)(v > 0 ? v : 148 * 2);
+        return (size_t)(v > 0 ? v : device_sm_count() * 2);
     }();
     if (blocks > cap) blocks = cap;
     if (blocks == 0) blocks = 1;  // the handshake still runs

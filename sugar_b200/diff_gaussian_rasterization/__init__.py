@@ -1,4 +1,4 @@
-"""Drop-in `diff_gaussian_rasterization` module backed by libsugar_b200 (sm_100a).
+"""Drop-in `diff_gaussian_rasterization` module backed by libsugar_b200 (sm_90a).
 
 Public surface identical to the module SuGaR imports (`from diff_gaussian_rasterization import
 GaussianRasterizationSettings, GaussianRasterizer`, sugar_scene/sugar_model.py:10; reference

@@ -36,7 +36,7 @@ each other's exchange buffers with CUDA IPC once; a backward is then ONE C call,
                                                TMA-stores its records into the staging array of the rank that owns them
     side                                       [chunk 0 signalled] reduce owned slice, post sums to every rank ─ split ─ ...
 
-Over NCCL (`peer=False`, and wherever "auto" has not measured the peer exchange faster; DESIGN.md section 5b):
+Over NCCL (`peer=False`, and on the world sizes "auto" does not give to the peer exchange; DESIGN.md section 5b):
 
     blend pass ─► hook BLEND_DONE ─► per-Gaussian pass, chunk 0 ─► hook ─► chunk 1 ─► hook ─► ... ─► finalize
                      │ all-gather of the SH factors                │ all-reduce of chunk 0's records
@@ -91,7 +91,7 @@ def reduce_grad(t: torch.Tensor, scale: float = 1.0, group=None) -> torch.Tensor
 
 
 _SLOT_BLEND, _SLOT_CHUNK0, _SLOT_REDUCED0, _PEER_MAX_CHUNKS = 0, 1, 17, 16   # flag slots (csrc/sgr_peer.cu)
-PEER_AUTO_WORLDS = (2,)   # measured: 2 GPUs 2.96 ms / step (e2e 661 views/s) vs 3.00 (630) over NCCL; see profiles/r02_scaling.md
+PEER_AUTO_WORLDS = (2,)   # beyond two ranks the peer pass waits on several remote factor blocks per CTA (DESIGN.md 5b)
 
 
 def _peer_auto_worlds():
@@ -206,8 +206,8 @@ class ViewParallel:
     force       run the record / finalize path even with a single rank (tests; no collectives are issued)
     side_stream (NCCL exchange) finalize range c on a second (high-priority) stream as soon as its collective is done,
                 concurrently with the per-Gaussian pass of the ranges behind it, instead of after the whole pass
-    peer        "auto" (default): the peer-memory exchange on the world sizes it measured faster on (PEER_AUTO_WORLDS,
-                override SGR_PEER_WORLDS), NCCL elsewhere or if the ranks cannot map each other's memory; True / False
+    peer        "auto" (default): the peer-memory exchange on the world sizes in PEER_AUTO_WORLDS (a design
+                choice, not timed on H100; override SGR_PEER_WORLDS), NCCL elsewhere or if the ranks cannot map each other's memory; True / False
     peer_timeout_s  a flag wait of the peer exchange traps after this long (a lost rank must not hang the others)
     taper       peer exchange: chunk c+1 is half the size of chunk c (the exposed tail is the last chunk's reduce + split)
     """
@@ -239,7 +239,7 @@ class ViewParallel:
     def uses_peer_memory(self, M: int, has_cov_precomp: bool) -> bool:
         """Peer mode serves the common case: SH colours exchanged as factors, covariances computed in the op.
         peer=True: always (raises if the buffers cannot be mapped); False: never; "auto" (default): on the world sizes
-        it has been measured faster than the NCCL exchange on (PEER_AUTO_WORLDS; override: SGR_PEER_WORLDS="2,4,8"),
+        the design gives to it (PEER_AUTO_WORLDS, not timed on H100; override: SGR_PEER_WORLDS="2,4,8"),
         falling back to NCCL if the ranks cannot map each other's memory."""
         if not self.peer or not M or not self.sh_factors or has_cov_precomp or self.chunks > _PEER_MAX_CHUNKS:
             return False
@@ -265,7 +265,7 @@ class ViewParallel:
         dev = means3D.device
         factor = bool(M) and self.sh_factors
         nchunks = max(1, self.chunks)
-        taper = 0   # equal chunks here: halving ones measured slower with NCCL (2 GPUs: 3.09 vs 3.00 ms per step)
+        taper = 0   # equal chunks here: the halving taper is for the peer exchange's exposed tail (not timed on H100)
         if getattr(self, "_ranges_key", None) != (P, nchunks, taper):
             self._ranges_key = (P, nchunks, taper)
             self._ranges = [self._range(lib, check, P, nchunks, c, taper) for c in range(nchunks)]

@@ -3,7 +3,7 @@
 Must run on a GPU box:   python tests/golden/make_golden.py gpurun_out/golden
 Inputs are NOT stored: they are regenerated from the seed by sugar_b200.scenes.make_scene
 (numpy PCG64, platform independent).  Outputs are what the reference's own kernels produced on
-a B200: every array of its GeometryState / BinningState / ImageState plus image and gradients.
+the GPU: every array of its GeometryState / BinningState / ImageState plus image and gradients.
 The committed .npz files under tests/golden/ pin the CPU oracle (tests/test_oracle_golden.py).
 """
 import os

@@ -1,5 +1,7 @@
 """Shared test plumbing: run the same seeded scene through (a) the sugar_b200 CUDA path,
-(b) the CPU oracle, (c) the unmodified reference CUDA build in oracle/_ref (when present)."""
+(b) the CPU oracle, (c) the unmodified reference CUDA build in oracle/_ref (when present), whose results
+the GPU tests read from tests/golden/refbuild_*.npz (tests/golden/make_refbuild_golden.py)."""
+import hashlib
 import importlib
 import os
 import sys
@@ -8,6 +10,68 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_DIR = os.path.join(ROOT, "oracle", "_ref")
+GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
+
+# what a golden keeps of a gradient tensor: its shape, |g|_inf, N_STRIDED evenly spaced entries and the N_TOP
+# largest -- or the whole tensor, for cases whose gradients hold at most WHOLE_MAX entries in all
+N_STRIDED, N_TOP, WHOLE_MAX = 256, 32, 40_000
+
+
+def _np(x):
+    return x.detach().cpu().numpy() if hasattr(x, "detach") else np.asarray(x)
+
+
+def digest(x):
+    """SHA-256 of an array's values (not of its dtype or shape): integers as int64, floats by their fp32 bits.
+    Two arrays with equal digests are bit-identical, which is what the reference comparisons require."""
+    a = _np(x).reshape(-1)
+    a = a.astype(np.float32).view(np.uint32).astype(np.int64) if a.dtype.kind == "f" else a.astype(np.int64)
+    return np.frombuffer(hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest(), np.uint8)
+
+
+def strided_idx(n):
+    return np.unique(np.arange(N_STRIDED, dtype=np.int64) * n // N_STRIDED) if n else np.zeros(0, np.int64)
+
+
+def grad_summary(prefix, g, whole=False):
+    """{prefix_*: ...} of one gradient for a golden file (g: torch tensor on any device)."""
+    import torch
+    f = g.detach().reshape(-1).float()
+    k = min(N_TOP, f.numel())
+    top = torch.topk(f.abs(), k).indices.cpu().numpy().astype(np.int64) if k else np.zeros(0, np.int64)
+    a = f.cpu().numpy()
+    d = {prefix + "_shape": np.asarray(g.shape, np.int64), prefix + "_inf": np.float64(np.abs(a).max() if a.size else 0.0),
+         prefix + "_top_idx": top, prefix + "_top": a[top], prefix + "_strided": a[strided_idx(a.size)]}
+    if whole:
+        d[prefix + "_whole"] = a
+    return d
+
+
+def golden_rel_err(g, gold, prefix):
+    """rel_err of a gradient against the reference's: over the whole tensor where the golden keeps it, else over the
+    entries it keeps (grad_summary).  The shapes must match."""
+    a = _np(g)
+    assert tuple(a.shape) == tuple(gold[prefix + "_shape"]), f"{prefix}: shape {a.shape} vs {gold[prefix + '_shape']}"
+    a = a.astype(np.float64).reshape(-1)
+    if prefix + "_whole" in gold:
+        return rel_err(a, gold[prefix + "_whole"])
+    d = max(np.abs(a[gold[prefix + "_top_idx"]] - gold[prefix + "_top"]).max(initial=0.0),
+            np.abs(a[strided_idx(a.size)] - gold[prefix + "_strided"]).max(initial=0.0))
+    return d / max(float(gold[prefix + "_inf"]), 1e-30)
+
+
+def load_golden(name):
+    """tests/golden/refbuild_<name>.npz as a dict (what the reference build computed on the same inputs)."""
+    with np.load(os.path.join(GOLDEN_DIR, f"refbuild_{name}.npz")) as z:
+        return {k: z[k] for k in z.files}
+
+
+def assert_digests(gold, got):
+    """Every digest_<field> of `gold` must match the array got[field]."""
+    for k in gold:
+        if k.startswith("digest_"):
+            field = k[len("digest_"):]
+            assert np.array_equal(digest(got[field]), gold[k]), f"{field} not bit-identical to the reference build"
 
 
 def scene_kwargs(sc, use_sh=True, use_cov_precomp=False, sh_degree=3, cov3D=None):

@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
 def test_sizes_and_errors_without_gpu():
     from sugar_b200 import _lib
     L = _lib.lib
-    assert b"sm_100a" in L.sgr_version()
+    assert b"sm_90a" in L.sgr_version()
     assert L.sgr_geometry_bytes(1000) >= 1000 * 60
     assert L.sgr_binning_bytes(0) > 0
     assert L.sgr_image_bytes(1920, 1080) >= 1920 * 1080 * 8

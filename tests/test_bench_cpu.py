@@ -13,7 +13,7 @@ def test_algorithmic_bytes_model_headline():
     b = bench.algorithmic_bytes(P, V, R, W, H, 16, 3)
     assert set(b) == {"preprocess", "tile_scan", "scatter", "tile_sort_smem", "tile_sort_global", "blend_forward",
                       "blend_backward", "preprocess_backward"}
-    # the numbers profiles/README.md quotes (GB/s = bytes / ms) come from exactly these
+    # the GB/s bench.py reports (bytes / ms) come from exactly these
     assert b["blend_backward"] == R * 40 + W * H * 20 + V * 72 == 678_756_768
     assert b["preprocess"] == P * (44 + 192) + P * 12 + V * 56 + R * 4
     assert b["preprocess_backward"] == V * (80 + 192) + P * (92 + 192)

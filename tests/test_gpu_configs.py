@@ -1,5 +1,6 @@
 """Element-wise parity with the UNMODIFIED reference CUDA build (oracle/_ref) at every rasterizer
-configuration BASELINE.json names, through the public module on the same tensors in the same process:
+configuration BASELINE.json names, through the public module on the same seeded tensors; the reference's
+results are read from tests/golden/refbuild_config_*.npz (tests/golden/make_refbuild_golden.py):
 
     C2        100k Gaussians,   800x800,  SH degree 2
     C3          1M Gaussians, 1920x1080,  SH degree 3      (also tests/test_gpu_parity.py::test_full_size_properties)
@@ -8,7 +9,7 @@ configuration BASELINE.json names, through the public module on the same tensors
     C5          6M Gaussians, 3840x2160,  SH degree 3      (one view of the 8-view batch)
 
 Bars: num_rendered, radii, n_contrib equal; image and final_T bit-identical; every gradient
-|a-b|_inf / |b|_inf <= 1e-4 (BASELINE.json).  Mesh-bound Gaussians (a 1e-6 axis) are the documented
+|a-b|_inf / |b|_inf <= 1e-4 (BASELINE.json) over the entries the golden keeps.  Mesh-bound Gaussians (a 1e-6 axis) are the documented
 exception for dL_dscales / dL_drotations: there the reference's own per-Gaussian chain amplifies the fp32
 summation-order noise of the blend accumulators by ~1e3, so those two tensors are held to 5x the larger
 of (the reference's own run-to-run difference, the chain's measured sensitivity to 1e-6 accumulator noise
@@ -39,34 +40,23 @@ CONFIGS = [
 
 @pytest.mark.parametrize("cfg", CONFIGS, ids=[c[0] for c in CONFIGS])
 def test_baseline_config_matches_reference_build(cfg):
-    import torch
-    if not h.have_ref():
-        pytest.skip("oracle/_ref not built")
     name, P, W, H, deg, mesh = cfg
     from sugar_b200 import _C, diff_gaussian_rasterization as ours, scenes
-    ref = h.load_ref_module()
+    gold = h.load_golden("config_" + name)
     sc = scenes.make_scene(P, W, H, seed=0, mesh_bound=mesh)
     dL = scenes.upstream_grad(W, H)
     bg = (0.0, 0.0, 0.0)
     a = h.run_module(ours, sc, bg, dL, use_sh=True, sh_degree=deg)
-    b = h.run_module(ref, sc, bg, dL, use_sh=True, sh_degree=deg)
-    assert a["num_rendered"] == b["num_rendered"]
-    assert torch.equal(a["radii"], b["radii"]), "radii differ"
-    assert torch.equal(a["color"].view(torch.int32), b["color"].view(torch.int32)), "image not bit-exact"
+    assert a["num_rendered"] == int(gold["num_rendered"])
     st = _C.inspect_state(P, W, H, a["num_rendered"], a["geom"], a["binning"], a["img"])
-    rs = h.decode_ref_state(b, P, W, H)
-    assert torch.equal(st["n_contrib"], rs["n_contrib"]), "n_contrib differs"
-    assert torch.equal(st["final_T"].view(torch.int32), rs["final_T"].view(torch.int32)), "final_T not bit-exact"
-    assert torch.equal(st["point_list"], rs["point_list"]), "sorted Gaussian ids differ"
-    assert torch.equal(st["keys"], rs["keys"]), "sorted 64-bit keys differ"
-    assert torch.equal(st["ranges"], rs["ranges"]), "tile ranges differ"
-    del st, rs
-    assert set(a["grads"]) == set(b["grads"])
-    errs = {k: h.rel_err(a["grads"][k].cpu().numpy(), b["grads"][k].cpu().numpy()) for k in b["grads"]}
+    h.assert_digests(gold, dict(radii=a["radii"], color=a["color"], n_contrib=st["n_contrib"], final_T=st["final_T"],
+                                point_list=st["point_list"], keys=st["keys"], ranges=st["ranges"]))
+    del st
+    assert {k[len("grad_"):-len("_inf")] for k in gold if k.endswith("_inf")} == set(a["grads"])
+    errs = {k: h.golden_rel_err(a["grads"][k], gold, "grad_" + k) for k in a["grads"]}
     bad = {k: e for k, e in errs.items() if e > GRAD_RTOL}
     if bad and mesh:
-        b2 = h.run_module(ref, sc, bg, dL, use_sh=True, sh_degree=deg)
-        noise = {k: h.rel_err(b2["grads"][k].cpu().numpy(), b["grads"][k].cpu().numpy()) for k in bad}
+        noise = {k: float(gold["noise_" + k]) for k in bad}
         small = scenes.make_scene(P // 64, W // 8, H // 8, seed=0, mesh_bound=True)
         sens = h.grad_sensitivity(small, bg, scenes.upstream_grad(W // 8, H // 8), use_sh=True, sh_degree=deg)
         bad = {k: e for k, e in bad.items()

@@ -1,7 +1,7 @@
 """Two real ranks on one box (only where at least two GPUs are visible; the single-GPU box skips it): every rank renders
 its own view and the gradients summed inside the backward -- over peer memory and over NCCL, SH factors on and off,
 1 / 4 / 7 chunks -- must equal the locally computed gradients summed with dist.all_reduce.  Runs
-scripts/check_view_parallel.py under torchrun, exactly as the multi-GPU sessions behind profiles/r02_scaling.md did."""
+scripts/check_view_parallel.py under torchrun."""
 import json
 import os
 import socket

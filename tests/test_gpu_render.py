@@ -1,6 +1,7 @@
 """SuGaR.render_image_gaussian_rasterizer as the trainers call it (SURVEY a12): the mirror in sugar_b200/render.py
 against the arguments the reference's own wrapper produced (tests/golden/render_wrapper.npz, made by running
-sugar_model.py:2085-2294 with a recording rasterizer) rasterized by the UNMODIFIED reference CUDA build."""
+sugar_model.py:2085-2294 with a recording rasterizer) rasterized by the UNMODIFIED reference CUDA build (its image and
+radii: tests/golden/refbuild_render.npz, tests/golden/make_refbuild_golden.py)."""
 import os
 
 import numpy as np
@@ -27,16 +28,8 @@ def test_render_wrapper_matches_reference_wrapper_plus_reference_rasterizer():
     assert float((out["radii"] > 0).float().mean()) > 0.5
     # in-kernel SH vs the python colour path: same polynomial, different evaluation order
     assert float((out["image"] - img_py).abs().max()) <= 1e-5
-    if not h.have_ref():
-        pytest.skip("oracle/_ref not built")
-    ref = h.load_ref_module()
-    st = ref.GaussianRasterizationSettings(
-        image_height=H, image_width=W, tanfovx=float(g["tanfov"][0]), tanfovy=float(g["tanfov"][1]), bg=t("bg"),
-        scale_modifier=1.0, viewmatrix=t("viewmatrix"), projmatrix=t("projmatrix"), sh_degree=int(g["sh_degree"]),
-        campos=t("campos"), prefiltered=False, debug=False)
-    m3 = t("means3D")
-    img_ref, radii_ref = ref.GaussianRasterizer(st)(means3D=m3, means2D=torch.zeros_like(m3), opacities=t("opacities"),
-                                                    colors_precomp=t("colors_precomp"), scales=t("scales"),
-                                                    rotations=t("rotations"))
+    ref = h.load_golden("render")
+    img_ref = torch.from_numpy(ref["image"]).cuda()
+    radii_ref = torch.from_numpy(ref["radii"]).cuda()
     assert float((img_py - img_ref.permute(1, 2, 0)).abs().max()) <= 2e-5
     assert float((radii_ref == out["radii"]).float().mean()) > 0.995

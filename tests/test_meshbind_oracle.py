@@ -40,7 +40,7 @@ def _host_lib(tmp_path_factory):
     out = str(tmp_path_factory.mktemp("meshbind") / "libmeshbind_host.so")
     src = os.path.join(ROOT, "sugar_b200", "csrc", "sgr_meshbind.cu")
     subprocess.check_call([nvcc if os.path.exists(nvcc) else "nvcc", "-O1", "-std=c++17", "-DSGR_MESHBIND_HOST_TEST",
-                           "-gencode", "arch=compute_100a,code=sm_100a", "--shared", "-Xcompiler", "-fPIC", src, "-o", out],
+                           "-gencode", "arch=compute_90a,code=sm_90a", "--shared", "-Xcompiler", "-fPIC", src, "-o", out],
                           stderr=subprocess.DEVNULL)
     return C.CDLL(out)
 
