@@ -291,9 +291,12 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
             }
             // Conservative cull threshold: alpha = min(.99, o*exp(power)) < 1/255 is certain when
             // power < tau = ln(1/(255 o)) - 1e-4 (margin >> ulp error of expf/logf; DESIGN.md).
+            // "Always skipped" is exactly the blend's own rejection of the largest alpha, o < 1/255: at
+            // o == 1/255 (where o * 255 rounds to 1) a pixel with power == 0 has alpha == 1/255 and is drawn,
+            // and tau = -1e-4 keeps it.
             float tau;
-            if (opacity * 255.0f > 1.0f) tau = -logf(opacity * 255.0f) - 1e-4f;
-            else if (opacity == opacity) tau = __int_as_float(0x7f800000);  // never reaches 1/255: always skipped
+            if (opacity < 1.0f / 255.0f) tau = __int_as_float(0x7f800000);  // never reaches 1/255: always skipped
+            else if (opacity == opacity) tau = -logf(opacity * 255.0f) - 1e-4f;
             else tau = -__int_as_float(0x7f800000);                          // NaN opacity: take the exact path
             float4 *rec = a.geom.rec + (size_t)idx * 3;
             rec[0] = make_float4(px, py, con_a, con_b);

@@ -89,6 +89,48 @@ def scene_kwargs(sc, use_sh=True, use_cov_precomp=False, sh_degree=3, cov3D=None
     return kw
 
 
+ALPHA_MIN = np.float32(1) / np.float32(255)   # the blend's threshold 1.0f / 255.0f: the one o with o * 255 == 1 in fp32
+EDGE_OPACITIES = [0.3, ALPHA_MIN, np.nextafter(ALPHA_MIN, np.float32(0)), np.nextafter(ALPHA_MIN, np.float32(1)), 0.05,
+                  ALPHA_MIN, 0.7, np.nextafter(ALPHA_MIN, np.float32(0)), ALPHA_MIN]
+
+
+def opacity_edge_scene():
+    """Gaussians on the optical axis of an identity camera, 33x33 pixels: every mean projects to pixel (16, 16) exactly,
+    where power == 0 and alpha == min(0.99, opacity).  Opacities 1/255 (drawn there: alpha < 1/255 is false), one ulp
+    below it (never drawn), one ulp above, and ordinary values, front to back in EDGE_OPACITIES order; the farthest is
+    1/255, so it decides n_contrib at the centre."""
+    from sugar_b200 import scenes
+    P = len(EDGE_OPACITIES)
+    sc = scenes.make_scene(P, 33, 33, seed=255, camera="identity", frac_behind=0.0)
+    m = np.zeros((P, 3), np.float32)
+    m[:, 2] = 2.0 + 0.5 * np.arange(P)
+    return sc._replace(means3D=m, opacities=np.asarray(EDGE_OPACITIES, np.float32).reshape(P, 1))
+
+
+def sh_basis(d, deg):
+    """Real SH basis [P,16] in float64 for unit directions d [P,3], in the reference's order and sign convention
+    (forward.cu:20-71 / backward.cu:20-139); zero beyond degree `deg`."""
+    C0, C1 = 0.28209479177387814, 0.4886025119029199
+    C2 = (1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396)
+    C3 = (-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658,
+          1.445305721320277, -0.5900435899266435)
+    x, y, z = d[:, 0], d[:, 1], d[:, 2]
+    b = np.zeros((d.shape[0], 16))
+    b[:, 0] = C0
+    if deg > 0:
+        b[:, 1], b[:, 2], b[:, 3] = -C1 * y, C1 * z, -C1 * x
+    if deg > 1:
+        xx, yy, zz, xy, yz, xz = x * x, y * y, z * z, x * y, y * z, x * z
+        b[:, 4], b[:, 5], b[:, 6] = C2[0] * xy, C2[1] * yz, C2[2] * (2 * zz - xx - yy)
+        b[:, 7], b[:, 8] = C2[3] * xz, C2[4] * (xx - yy)
+    if deg > 2:
+        b[:, 9], b[:, 10] = C3[0] * y * (3 * xx - yy), C3[1] * xy * z
+        b[:, 11], b[:, 12] = C3[2] * y * (4 * zz - xx - yy), C3[3] * z * (2 * zz - 3 * xx - 3 * yy)
+        b[:, 13], b[:, 14] = C3[4] * x * (4 * zz - xx - yy), C3[5] * z * (xx - yy)
+        b[:, 15] = C3[6] * x * (xx - 3 * yy)
+    return b
+
+
 def run_oracle(sc, bg, dL=None, **opts):
     from oracle import raster_oracle as ro
     kw = scene_kwargs(sc, **opts)

@@ -32,6 +32,21 @@ def _render_loss(mod, t, sc, dL, deg, ps, bg=(0.1, 0.2, 0.3), colors=None):
                                                      (2, 3, False, True)])
 @pytest.mark.parametrize("peer", [True, False])
 def test_forced_exchange_matches_plain_backward(deg, chunks, factors, side, peer):
+    check_forced_exchange(16, deg, chunks, factors, side, peer)
+
+
+# M = 1 / 4 / 9 stored SH coefficients: the generic finalize kernel (M = 16 has its own), and in peer mode the
+# per-Gaussian pass with rows that are not 48 floats; deg < sqrt(M) - 1 leaves trailing coefficients that must be zero
+@pytest.mark.parametrize("M,deg,chunks,factors,side", [
+    (9, 2, 3, True, False), (9, 2, 4, True, True), (9, 1, 2, False, True), (4, 1, 4, True, False), (4, 1, 3, True, True),
+    (4, 0, 2, False, False), (1, 0, 1, True, True), (1, 0, 3, True, False)])
+@pytest.mark.parametrize("peer", [True, False])
+def test_forced_exchange_with_fewer_stored_sh_coefficients(M, deg, chunks, factors, side, peer):
+    check_forced_exchange(M, deg, chunks, factors, side, peer)
+
+
+def check_forced_exchange(M, deg, chunks, factors, side, peer):
+    """ViewParallel(force=True) with [P, M, 3] SH coefficients: scale x the plain backward's gradients."""
     import torch
     from sugar_b200 import diff_gaussian_rasterization as mod
     from sugar_b200 import parallel, scenes
@@ -39,6 +54,7 @@ def test_forced_exchange_matches_plain_backward(deg, chunks, factors, side, peer
     sc = scenes.make_scene(P, W, H, seed=31 + deg, camera="posed")
     dL = torch.from_numpy(scenes.upstream_grad(W, H, seed=5)).cuda()
     t = h.to_torch(sc)
+    t["shs"] = t["shs"][:, :M].contiguous()
     leaf = lambda x: x.clone().requires_grad_(True)
     names = ("means3D", "opacities", "shs", "scales", "rotations")
     ps_a = {k: leaf(t[k]) for k in names}
@@ -59,8 +75,10 @@ def test_forced_exchange_matches_plain_backward(deg, chunks, factors, side, peer
         assert _err(ps_b[k].grad, 0.5 * ps_a[k].grad) <= 1e-4, k   # fp32 atomics: run-to-run order differs
     assert _err(m2b.grad, m2a.grad) <= 1e-4                        # per-view statistic: neither summed nor scaled
     used = (deg + 1) ** 2
-    if used < 16:
+    assert ps_b["shs"].grad.shape == (P, M, 3)
+    if used < M:
         assert float(ps_b["shs"].grad[:, used:].abs().max()) == 0.0
+        assert float(ps_a["shs"].grad[:, used:].abs().max()) == 0.0
 
 
 def test_exchange_with_precomputed_colours_and_activations_in_front():
@@ -124,11 +142,21 @@ def test_two_backwards_per_step_accumulate():
 
 
 def test_sh_factors_of_three_views_rebuild_the_summed_dsh():
+    check_sh_factors_rebuild(16, 3)
+
+
+def test_sh_factors_rebuild_the_summed_dsh_with_nine_stored_coefficients():
+    """M = 9 stored coefficients, degree 1: the generic kernel, and coefficients 4..8 must come back zero."""
+    check_sh_factors_rebuild(9, 1)
+
+
+def check_sh_factors_rebuild(M, deg):
     """sgr_sh_grad_from_factors on the gathered factors of several views == the sum of the views' dL_dsh; the
-    factor of a view is the dL_dcolors the backward returns with SH colours (clamp-masked dL/dRGB)."""
+    factor of a view is the dL_dcolors the backward returns with SH colours (clamp-masked dL/dRGB).  Also against
+    sum_v basis(normalize(mean - campos_v)) (x) factor_v evaluated in float64."""
     import torch
     from sugar_b200 import _C, parallel, scenes
-    P, W, H, deg = 6000, 160, 96, 3
+    P, W, H = 6000, 160, 96
     base = scenes.make_scene(P, W, H, seed=34, camera="posed")
     views = [base, scenes.with_camera_offset(base, 0.15, (0.3, -0.1, 0.2)),
              scenes.with_camera_offset(base, -0.2, (-0.4, 0.2, 0.5))]
@@ -136,6 +164,7 @@ def test_sh_factors_of_three_views_rebuild_the_summed_dsh():
     E = torch.Tensor([])
     for v, sc in enumerate(views):
         t = h.to_torch(sc)
+        t["shs"] = t["shs"][:, :M].contiguous()
         dL = torch.from_numpy(scenes.upstream_grad(W, H, seed=5 + v)).cuda()
         bg = torch.zeros(3, device="cuda")
         R, color, radii, geom, binning, img = _C.rasterize_gaussians(
@@ -147,12 +176,30 @@ def test_sh_factors_of_three_views_rebuild_the_summed_dsh():
         factors.append(g[1].clone())
         campos.append(t["campos"].clone())
         want = g[5].double() if want is None else want + g[5].double()
-    got = parallel.sh_grad_from_factors(torch.from_numpy(base.means3D).cuda(), torch.stack(campos).contiguous(),
-                                        torch.stack(factors).contiguous(), 16, deg)
+    means = torch.from_numpy(base.means3D).cuda()
+    got = parallel.sh_grad_from_factors(means, torch.stack(campos).contiguous(), torch.stack(factors).contiguous(), M, deg)
+    assert got.shape == (P, M, 3)
     assert _err(got, want) <= 1e-4
+    exact = 0.0
+    for f, cp in zip(factors, campos):
+        d = base.means3D.astype(np.float64) - cp.cpu().numpy().astype(np.float64).reshape(1, 3)
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+        exact = exact + h.sh_basis(d, deg)[:, :M, None] * f.cpu().numpy().astype(np.float64)[:, None, :]
+    assert h.rel_err(got.cpu().numpy(), exact) <= 1e-5
+    used = (deg + 1) ** 2
+    if used < M:
+        assert float(got[:, used:].abs().max()) == 0.0 and float(want[:, used:].abs().max()) == 0.0
 
 
 def test_peer_exchange_with_three_emulated_ranks():
+    check_peer_exchange_with_three_emulated_ranks(16, 3)
+
+
+def test_peer_exchange_with_three_emulated_ranks_and_nine_stored_coefficients():
+    check_peer_exchange_with_three_emulated_ranks(9, 2)
+
+
+def check_peer_exchange_with_three_emulated_ranks(M, deg):
     """The peer-memory exchange (csrc/sgr_peer.cu) as rank 0 of THREE, on one GPU: ranks 1 and 2 are static stand-ins --
     their factor blocks and record arrays are filled from plain backwards of their views, their flag words are preset,
     and this process reduces their record slices as well.  Everything the real multi-rank run executes runs here: the
@@ -162,15 +209,20 @@ def test_peer_exchange_with_three_emulated_ranks():
     import torch
     from sugar_b200 import _C, _lib, diff_gaussian_rasterization as mod
     from sugar_b200 import parallel, scenes
-    P, W, H, deg, scale = 6001, 160, 96, 3, 0.25
+    P, W, H, scale = 6001, 160, 96, 0.25
     base = scenes.make_scene(P, W, H, seed=41, camera="posed")
     views = [base, scenes.with_camera_offset(base, 0.15, (0.3, -0.1, 0.2)),
              scenes.with_camera_offset(base, -0.2, (-0.4, 0.2, 0.5))]
     names = ("means3D", "opacities", "shs", "scales", "rotations")
     E = torch.Tensor([])
     plain, factors, records = [], [], []
-    for v, sc in enumerate(views):
+
+    def to_torch(sc):
         t = h.to_torch(sc)
+        t["shs"] = t["shs"][:, :M].contiguous()
+        return t
+    for v, sc in enumerate(views):
+        t = to_torch(sc)
         dL = torch.from_numpy(scenes.upstream_grad(W, H, seed=5 + v)).cuda()
         bg = torch.zeros(3, device="cuda")
         R, color, radii, geom, binning, img = _C.rasterize_gaussians(
@@ -205,7 +257,7 @@ def test_peer_exchange_with_three_emulated_ranks():
         "shape": (64, 64), "typestr": "<i4", "data": (st.base, False), "version": 2}})(), device="cuda")
     flags[:63, 1:3] = 1 << 30   # ranks 1 and 2 have "already signalled" every slot of every step (row 63: CTA counters)
     vp._emulated = (1, 2)
-    t0, sc0 = h.to_torch(views[0]), views[0]
+    t0, sc0 = to_torch(views[0]), views[0]
     dL0 = torch.from_numpy(scenes.upstream_grad(W, H, seed=5)).cuda()
     for step in range(2):       # both factor-block parities
         ps = {k: t0[k].clone().requires_grad_(True) for k in names}

@@ -41,11 +41,20 @@ CASES = [
     ("coplanar", 20000, 160, 96, "identity", False, 0, False, (0.0, 0.0, 0.0)),
     # two thin depth shells: very skewed per-tile depth histogram (bucket sort falls back to merge)
     ("two_shells", 60000, 128, 96, "identity", False, 0, False, (0.0, 0.0, 0.0)),
+    # splats of opacity 1/255 and one ulp either side of it, drawn or not at the one pixel where power == 0
+    # (helpers.opacity_edge_scene)
+    ("opacity_edge", 9, 33, 33, "identity", False, 0, False, (0.25, 0.5, 1.0)),
 ]
+# the oracle comparison also runs at the C2 size of BASELINE.json (tests/test_gpu_configs.py, the same scene)
+ORACLE_CASES = CASES + [("c2_100k_800x800_sh2", 100_000, 800, 800, "identity", True, 2, False, (0.0, 0.0, 0.0))]
 
 
 def _scene(name, P, W, H, camera):
     from sugar_b200 import scenes
+    if name == "opacity_edge":
+        return h.opacity_edge_scene()
+    if name.startswith("c2_"):
+        return scenes.make_scene(P, W, H, seed=0)
     kw = {}
     if name == "mesh_bound":
         kw["mesh_bound"] = True
@@ -122,8 +131,25 @@ def test_matches_reference_build(case):
     assert not bad, "; ".join(bad)
 
 
-@pytest.mark.parametrize("case", CASES[:5], ids=[c[0] for c in CASES[:5]])
+ORACLE_GRAD_RTOL = 5e-4
+GRAD_NAMES = dict(means3D="dL_dmeans3D", means2D="dL_dmeans2D", opacities="dL_dopacity", shs="dL_dsh",
+                  colors_precomp="dL_dcolors", scales="dL_dscales", rotations="dL_drotations",
+                  cov3D_precomp="dL_dcov3D")
+
+
+def tile_classes(fw, gid):
+    """The per-tile sort classes (instances per tile: <= 512 merge, <= 2048 bucket, <= 8192 merge, above: global
+    radix) of the tiles Gaussian `gid` is binned to, from an oracle forward."""
+    tiles = (fw["keys"] >> np.uint64(32)).astype(np.int64)[fw["point_list"] == gid]
+    n = (fw["ranges"][:, 1].astype(np.int64) - fw["ranges"][:, 0])[tiles]
+    cls = lambda c: "<=512" if c <= 512 else "<=2048" if c <= 2048 else "<=8192" if c <= 8192 else ">8192"
+    return sorted({cls(int(c)) for c in n}, key=len)
+
+
+@pytest.mark.parametrize("case", ORACLE_CASES, ids=[c[0] for c in ORACLE_CASES])
 def test_matches_cpu_oracle(case):
+    """Every output against the CPU oracle, every gradient tensor whole (the reference-build goldens keep a sample of
+    the larger ones).  A gradient over the bar names the tile-size classes of its worst Gaussian."""
     name, P, W, H, camera, use_sh, deg, covpre, bg = case
     from sugar_b200 import diff_gaussian_rasterization as ours, scenes
     from sugar_b200 import _C
@@ -154,11 +180,96 @@ def test_matches_cpu_oracle(case):
     img = a["color"].cpu().numpy()
     d = np.abs(img - fw["color"])
     assert np.quantile(d, 0.999) < 2e-6 and d.max() < 5e-3, (float(np.quantile(d, 0.999)), float(d.max()))
-    names = dict(means3D="dL_dmeans3D", means2D="dL_dmeans2D", opacities="dL_dopacity", shs="dL_dsh",
-                 colors_precomp="dL_dcolors", scales="dL_dscales", rotations="dL_drotations", cov3D_precomp="dL_dcov3D")
-    for k, g in a["grads"].items():
-        err = h.rel_err(g.cpu().numpy().reshape(bw[names[k]].shape), bw[names[k]])
-        assert err <= 5e-4, f"grad {k}: rel err vs oracle {err:.3e}"
+    bad, sens = [], None
+    for k, g in sorted(a["grads"].items()):
+        want = bw[GRAD_NAMES[k]]
+        got = g.cpu().numpy().reshape(want.shape)
+        err = h.rel_err(got, want)
+        bar = ORACLE_GRAD_RTOL
+        if err > bar and name == "mesh_bound" and k in ("scales", "rotations"):
+            # the 1e-6 axis: held to 5x the chain's sensitivity to 1e-6 accumulator noise (module docstring)
+            sens = sens or h.grad_sensitivity(sc, bg, dL, **opts)
+            bar = max(bar, 5.0 * sens.get(k, 0.0))
+        if err > bar:
+            d = np.abs(got.astype(np.float64) - want).reshape(P, -1).max(axis=1)
+            worst = int(np.argmax(d))
+            bad.append(f"grad {k}: rel err vs oracle {err:.3e} > {bar:.1e}; worst Gaussian {worst} "
+                       f"(|d| {d[worst]:.2e}) in tiles of size class {tile_classes(fw, worst)}")
+    assert not bad, "; ".join(bad)
+
+
+def edge_outputs(bg):
+    """Forward state, image and gradients of helpers.opacity_edge_scene through ours, as numpy arrays."""
+    from sugar_b200 import _C, diff_gaussian_rasterization as ours, scenes
+    sc = h.opacity_edge_scene()
+    P, W, H = sc.means3D.shape[0], sc.width, sc.height
+    a0 = h.run_module(ours, sc, bg, None, use_sh=False)
+    st = _C.inspect_state(P, W, H, a0["num_rendered"], a0["geom"], a0["binning"], a0["img"])
+    a = h.run_module(ours, sc, bg, scenes.upstream_grad(W, H), use_sh=False)
+    out = {k: v.cpu().numpy() for k, v in st.items()}
+    out.update(num_rendered=np.int64(a0["num_rendered"]), radii=a0["radii"].cpu().numpy(), color=a0["color"].cpu().numpy(),
+               color_bw=a["color"].cpu().numpy(), **{"grad_" + k: v.cpu().numpy() for k, v in a["grads"].items()})
+    return out
+
+
+def _edge_outputs_unpacked(bg):
+    """edge_outputs with the instance lists in the unpacked-id format (read once per process: a subprocess)."""
+    import os
+    import subprocess
+    import sys
+    import tempfile
+    code = ("import sys, numpy as np; sys.path[:0] = [%r, %r]; import test_gpu_parity as t; "
+            "np.savez(sys.argv[1], **t.edge_outputs(%r))" % (h.ROOT, os.path.join(h.ROOT, "tests"), tuple(bg)))
+    with tempfile.TemporaryDirectory() as d:
+        out = os.path.join(d, "u.npz")
+        subprocess.run([sys.executable, "-c", code, out], check=True, env=dict(os.environ, SGR_FORCE_UNPACKED_IDS="1"),
+                       timeout=600)
+        with np.load(out) as z:
+            return {k: z[k] for k in z.files}
+
+
+@pytest.mark.parametrize("unpacked", [False, True], ids=["packed_ids", "unpacked_ids"])
+@pytest.mark.parametrize("bg", [(0.0, 0.0, 0.0), (0.25, 0.5, 1.0)], ids=["bg0", "bg"])
+def test_opacity_at_the_alpha_threshold_matches_cpu_oracle(bg, unpacked):
+    """A splat of opacity exactly 1/255 is drawn where power == 0 (alpha == 1/255 passes `alpha < 1/255`), one of the
+    next float below is not: the cull threshold, the footprint masks and both blend kernels must agree with that.
+    At the centre pixel (power == 0, exp(0) == 1 on both sides) n_contrib, final_T and the image are bit-identical to
+    the CPU oracle; elsewhere the oracle tolerances apply.  Gradients whole."""
+    sc = h.opacity_edge_scene()
+    P, W, H = sc.means3D.shape[0], sc.width, sc.height
+    from sugar_b200 import scenes
+    fw, bw = h.run_oracle(sc, np.asarray(bg, np.float32), scenes.upstream_grad(W, H), use_sh=False)
+    o = _edge_outputs_unpacked(bg) if unpacked else edge_outputs(bg)
+    c = (W - 1) // 2
+    assert int(fw["n_contrib"][c, c]) == P   # the oracle draws the farthest splat, of opacity 1/255 (test_oracle_properties)
+    assert int(o["num_rendered"]) == fw["num_rendered"]
+    assert np.array_equal(o["radii"], fw["radii"])
+    assert np.array_equal(o["means2D"].view(np.uint32), fw["means2D"].view(np.uint32))
+    assert np.array_equal(o["conic_opacity"].view(np.uint32), fw["conic_opacity"].view(np.uint32))
+    assert np.array_equal(o["keys"].view(np.uint64), fw["keys"])
+    assert np.array_equal(o["point_list"].view(np.uint32), fw["point_list"])
+    assert np.array_equal(o["ranges"].view(np.uint32), fw["ranges"])
+    nc = o["n_contrib"].view(np.uint32)
+    assert int(nc[c, c]) == P, f"centre pixel: n_contrib {int(nc[c, c])}, the oracle's {P}"
+    assert o["final_T"][c, c].view(np.uint32) == fw["final_T"][c, c].view(np.uint32)
+    for img in (o["color"], o["color_bw"]):
+        assert np.array_equal(img[:, c, c].view(np.uint32), fw["color"][:, c, c].view(np.uint32))
+        d = np.abs(img - fw["color"])
+        assert np.quantile(d, 0.999) < 2e-6 and d.max() < 5e-3, (float(np.quantile(d, 0.999)), float(d.max()))
+    assert int((nc != fw["n_contrib"]).sum()) <= 2
+    if not unpacked:
+        # every drawn splat's footprint mask holds the centre pixel's block (tile (1, 1), block 0)
+        tile = (o["keys"].view(np.uint64) >> np.uint64(32)).astype(np.int64)
+        ctr = tile == (c // 16) * ((W + 15) // 16) + c // 16
+        drawn = sc.opacities.reshape(-1)[o["point_list"][ctr]] >= h.ALPHA_MIN
+        assert np.all(o["footprint"][ctr][drawn] & 1), o["footprint"][ctr]
+    for k in ("means3D", "means2D", "opacities", "colors_precomp", "scales", "rotations"):
+        want = bw[GRAD_NAMES[k]]
+        err = h.rel_err(o["grad_" + k].reshape(want.shape), want)
+        assert err <= ORACLE_GRAD_RTOL, f"grad {k}: rel err vs oracle {err:.3e}"
+    # the two splats one ulp below 1/255 contribute nowhere: zero gradient for their opacity and colour
+    below = sc.opacities.reshape(-1) < h.ALPHA_MIN
+    assert not o["grad_opacities"][below].any() and not o["grad_colors_precomp"][below].any()
 
 
 def test_mark_visible_and_empty():

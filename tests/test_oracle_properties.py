@@ -70,6 +70,34 @@ def test_culled_gaussians_have_zero_radius_and_zero_gradients():
         assert not np.any(bw[k][culled]), k
 
 
+def test_a_splat_of_opacity_one_255th_is_drawn_where_power_is_zero():
+    """alpha = min(0.99, o exp(power)) is skipped when alpha < 1/255 (forward.cu:344).  At the pixel a mean projects
+    to exactly, power == 0 and alpha == o, so o == 1/255 is drawn and the next float below it is not.  Restated here:
+    the centre pixel's n_contrib, final_T and colour follow from the opacities alone, blended in fp32 front to back."""
+    from sugar_b200 import scenes
+    sc = h.opacity_edge_scene()
+    P, W, H = sc.means3D.shape[0], sc.width, sc.height
+    bg = np.array([0.25, 0.5, 1.0], np.float32)
+    fw, _ = h.run_oracle(sc, bg, scenes.upstream_grad(W, H), use_sh=False)
+    c = (W - 1) // 2
+    assert np.all(fw["means2D"] == np.float32(c)) and np.all(fw["radii"] > 0)
+    o = sc.opacities.reshape(-1)
+    drawn = o >= h.ALPHA_MIN
+    assert drawn.sum() == P - 2 and drawn[-1]
+    T, C = np.float32(1), np.zeros(3, np.float32)
+    for i in np.flatnonzero(drawn):      # means sorted by depth == index order
+        a = np.float32(min(np.float32(0.99), o[i]))
+        C = (C + T * (a * sc.colors_precomp[i])).astype(np.float32)
+        T = np.float32(T * (np.float32(1) - a))
+    assert int(fw["n_contrib"][c, c]) == P        # the farthest splat (1/255) is the last contributor
+    assert abs(float(fw["final_T"][c, c]) - float(T)) <= 1e-7
+    assert np.abs(fw["color"][:, c, c] - (C + T * bg)).max() <= 1e-6
+    # the splats one ulp below 1/255 add nothing anywhere: the image equals the one with their opacity at zero
+    fw1, _ = h.run_oracle(sc._replace(opacities=np.where(drawn[:, None], sc.opacities, 0).astype(np.float32)), bg,
+                          use_sh=False)
+    assert np.array_equal(fw1["n_contrib"], fw["n_contrib"]) and np.array_equal(fw1["color"], fw["color"])
+
+
 def test_linear_properties_checker_on_the_oracle():
     """helpers.check_linear_properties (the checker the GPU suite runs at the headline size) on the CPU oracle."""
     sc = _scene(P=1200, W=80, H=48, seed=17)
@@ -80,29 +108,6 @@ def test_linear_properties_checker_on_the_oracle():
                                                             "dL_dscales", "dL_drotations")}
         return fw["color"], fw["radii"], grads
     h.check_linear_properties(run, sc.width, sc.height, tol_img=1e-6, tol_grad=2e-5)
-
-
-def _sh_basis(d, deg):
-    """Real SH basis values in the reference's order and sign convention (forward.cu:20-71 / backward.cu:20-139)."""
-    C0, C1 = 0.28209479177387814, 0.4886025119029199
-    C2 = (1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396)
-    C3 = (-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658,
-          1.445305721320277, -0.5900435899266435)
-    x, y, z = d[:, 0], d[:, 1], d[:, 2]
-    b = np.zeros((d.shape[0], 16))
-    b[:, 0] = C0
-    if deg > 0:
-        b[:, 1], b[:, 2], b[:, 3] = -C1 * y, C1 * z, -C1 * x
-    if deg > 1:
-        xx, yy, zz, xy, yz, xz = x * x, y * y, z * z, x * y, y * z, x * z
-        b[:, 4], b[:, 5], b[:, 6] = C2[0] * xy, C2[1] * yz, C2[2] * (2 * zz - xx - yy)
-        b[:, 7], b[:, 8] = C2[3] * xz, C2[4] * (xx - yy)
-    if deg > 2:
-        b[:, 9], b[:, 10] = C3[0] * y * (3 * xx - yy), C3[1] * xy * z
-        b[:, 11], b[:, 12] = C3[2] * y * (4 * zz - xx - yy), C3[3] * z * (2 * zz - 3 * xx - 3 * yy)
-        b[:, 13], b[:, 14] = C3[4] * x * (4 * zz - xx - yy), C3[5] * z * (xx - yy)
-        b[:, 15] = C3[6] * x * (xx - 3 * yy)
-    return b
 
 
 def test_a_views_sh_gradient_is_a_rank_one_product_of_its_colour_gradient():
@@ -124,7 +129,7 @@ def test_a_views_sh_gradient_is_a_rank_one_product_of_its_colour_gradient():
             factor[~vis] = 0.0
             d = sc.means3D.astype(np.float64) - np.asarray(sc.campos, np.float64).reshape(1, 3)
             d /= np.linalg.norm(d, axis=1, keepdims=True)
-            want = _sh_basis(d, deg)[:, :, None] * factor[:, None, :]
+            want = h.sh_basis(d, deg)[:, :, None] * factor[:, None, :]
             got = bw["dL_dsh"].astype(np.float64)
             assert vis.sum() > 100
             assert np.abs(got - want).max() <= 2e-6 * max(np.abs(want).max(), 1e-30), deg
