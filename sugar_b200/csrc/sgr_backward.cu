@@ -439,14 +439,17 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
 
 // ------------------------------------------------------------------------------------------------
 // per-Gaussian backward (cov2D inverse, projection, SH, scale/rotation), one fused pass.
-// HBM-bound: every input array is staged into shared memory with coalesced transfers (1-D bulk
-// copies through the TMA engine for the contiguous arrays, 16-byte cp.async into padded rows for
-// the SH block), each thread works on its own Gaussian out of shared memory, the SH gradient
-// overwrites the SH row in place, and all outputs leave through coalesced stores.
+// HBM-bound: every input array is staged into shared memory by 1-D bulk copies through the TMA
+// engine, each thread works on its own Gaussian out of shared memory, and all outputs leave through
+// coalesced stores.  The SH coefficients are not an input: the view-direction term of dL/dmean3D
+// comes from the forward's Jacobian rows (36 B per Gaussian instead of the 192 B row), and the SH
+// gradient is built in a shared-memory row block on its way out.
 // ------------------------------------------------------------------------------------------------
 struct PreBwdArgs {
     int p0, p1;  // Gaussian range of this launch (one chunk of the per-Gaussian pass); p0 % PB_T == 0
+    // shs / sh_rest: only whether SH colours are present (their contents are never read)
     const float *means, *scales, *rots, *shs, *cov_pre;
+    const float *sh_jac;  // [P][9] the forward's dRGB/d(dir) rows (GeomState::sh_jac)
     ViewConsts v;
     const int32_t *radii;
     const float *gacc;  // [P][8] blend accumulators
@@ -456,9 +459,8 @@ struct PreBwdArgs {
     // 44-byte record instead of the four arrays (the view-parallel step all-reduces these records chunk by chunk)
     float *rec11;
     int in_bulk_ok, out_bulk_ok, sh_stride, sh_vec;
-    // raw-parameter mode (SgrGaussians.activations): scales / rots are the model's raw parameters, shs its DC
-    // array and sh_rest the others; dopacity / dscales / drots / dsh / dsh_rest are gradients of the RAW parameters
-    const float *sh_rest;
+    // raw-parameter mode (SgrGaussians.activations): scales / rots are the model's raw parameters; dopacity / dscales /
+    // drots / dsh / dsh_rest are gradients of the RAW parameters, dsh of the DC array and dsh_rest of the others
     const float4 *rec;  // splat records of the forward: rec[3i+1].z = the activated opacity
     float *dsh_rest;
     // view-parallel peer mode (csrc/sgr_peer.cu): dsh rows leave as the sum over ALL views' SH gradients.  view_tab is a
@@ -489,25 +491,20 @@ struct f3 {
     float x, y, z;
 };
 
-// SH backward (backward.cu:20-139) on one shared-memory row [M][3], in place: row k is read once
-// (t_k = <sh_k, dL/dRGB> feeds the view-direction gradient) and then overwritten by dL/dsh_k.
-// `dc` is coefficient 0's row of three, `rest` coefficient 1's (one combined row: rest = dc + 3; raw-parameter
-// mode: two arrays).
+// dL/dsh of one view (backward.cu:20-139: dL/dsh_k = basis_k(dir) dL/dRGB) into one shared-memory row [M][3].
+// Write-only: the view-direction term, the only use the reference makes of the coefficients, comes from the
+// forward's Jacobian rows (sh_dir_grad).  `dc` is coefficient 0's row of three, `rest` coefficient 1's (one combined
+// row: rest = dc + 3; raw-parameter mode: two arrays).
 template <bool OTHERS = false>
-__device__ __forceinline__ void sh_backward_inplace(int deg, int M, float *dc, float *rest, f3 dir_orig, f3 dRGB,
-                                                    f3 &dmean, float out_scale = 1.0f, const float *oacc = nullptr)
+__device__ __forceinline__ void sh_grad_row(int deg, int M, float *dc, float *rest, f3 dir_orig, f3 dRGB,
+                                            float out_scale = 1.0f, const float *oacc = nullptr)
 {
     const f3 dS = {dRGB.x * out_scale, dRGB.y * out_scale, dRGB.z * out_scale};  // x 1.0f is exact
     const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
     const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
-    float ddx = 0.f, ddy = 0.f, ddz = 0.f;
-#define SHB(k, w, cx, cy, cz)                                                          \
+#define SHB(k, w)                                                                      \
     {                                                                                  \
         float *q_ = (k) == 0 ? dc : rest + ((k) - 1) * 3;                              \
-        const float t_ = q_[0] * dRGB.x + q_[1] * dRGB.y + q_[2] * dRGB.z;             \
-        ddx += (cx) * t_;                                                              \
-        ddy += (cy) * t_;                                                              \
-        ddz += (cz) * t_;                                                              \
         const float w_ = (w);                                                          \
         if (OTHERS) { /* the other views' SH gradients of this Gaussian (registers) join the row here */ \
             q_[0] = fmaf(w_, dS.x, oacc[(k) * 3]);                                     \
@@ -519,42 +516,48 @@ __device__ __forceinline__ void sh_backward_inplace(int deg, int M, float *dc, f
             q_[2] = w_ * dS.z;                                                         \
         }                                                                              \
     }
-    SHB(0, SH_C0, 0.f, 0.f, 0.f);
+    SHB(0, SH_C0);
     if (deg > 0) {
-        SHB(1, -SH_C1 * y, 0.f, -SH_C1, 0.f);
-        SHB(2, SH_C1 * z, 0.f, 0.f, SH_C1);
-        SHB(3, -SH_C1 * x, -SH_C1, 0.f, 0.f);
+        SHB(1, -SH_C1 * y);
+        SHB(2, SH_C1 * z);
+        SHB(3, -SH_C1 * x);
         if (deg > 1) {
             const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-            SHB(4, b_SH_C2[0] * xy, b_SH_C2[0] * y, b_SH_C2[0] * x, 0.f);
-            SHB(5, b_SH_C2[1] * yz, 0.f, b_SH_C2[1] * z, b_SH_C2[1] * y);
-            SHB(6, b_SH_C2[2] * (2.f * zz - xx - yy), b_SH_C2[2] * 2.f * -x, b_SH_C2[2] * 2.f * -y, b_SH_C2[2] * 2.f * 2.f * z);
-            SHB(7, b_SH_C2[3] * xz, b_SH_C2[3] * z, 0.f, b_SH_C2[3] * x);
-            SHB(8, b_SH_C2[4] * (xx - yy), b_SH_C2[4] * 2.f * x, b_SH_C2[4] * 2.f * -y, 0.f);
+            SHB(4, b_SH_C2[0] * xy);
+            SHB(5, b_SH_C2[1] * yz);
+            SHB(6, b_SH_C2[2] * (2.f * zz - xx - yy));
+            SHB(7, b_SH_C2[3] * xz);
+            SHB(8, b_SH_C2[4] * (xx - yy));
             if (deg > 2) {
-                SHB(9, b_SH_C3[0] * y * (3.f * xx - yy), b_SH_C3[0] * 3.f * 2.f * xy, b_SH_C3[0] * 3.f * (xx - yy), 0.f);
-                SHB(10, b_SH_C3[1] * xy * z, b_SH_C3[1] * yz, b_SH_C3[1] * xz, b_SH_C3[1] * xy);
-                SHB(11, b_SH_C3[2] * y * (4.f * zz - xx - yy), b_SH_C3[2] * -2.f * xy,
-                    b_SH_C3[2] * (-3.f * yy + 4.f * zz - xx), b_SH_C3[2] * 4.f * 2.f * yz);
-                SHB(12, b_SH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy), b_SH_C3[3] * -3.f * 2.f * xz,
-                    b_SH_C3[3] * -3.f * 2.f * yz, b_SH_C3[3] * 3.f * (2.f * zz - xx - yy));
-                SHB(13, b_SH_C3[4] * x * (4.f * zz - xx - yy), b_SH_C3[4] * (-3.f * xx + 4.f * zz - yy),
-                    b_SH_C3[4] * -2.f * xy, b_SH_C3[4] * 4.f * 2.f * xz);
-                SHB(14, b_SH_C3[5] * z * (xx - yy), b_SH_C3[5] * 2.f * xz, b_SH_C3[5] * -2.f * yz, b_SH_C3[5] * (xx - yy));
-                SHB(15, b_SH_C3[6] * x * (xx - 3.f * yy), b_SH_C3[6] * 3.f * (xx - yy), b_SH_C3[6] * -3.f * 2.f * xy, 0.f);
+                SHB(9, b_SH_C3[0] * y * (3.f * xx - yy));
+                SHB(10, b_SH_C3[1] * xy * z);
+                SHB(11, b_SH_C3[2] * y * (4.f * zz - xx - yy));
+                SHB(12, b_SH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy));
+                SHB(13, b_SH_C3[4] * x * (4.f * zz - xx - yy));
+                SHB(14, b_SH_C3[5] * z * (xx - yy));
+                SHB(15, b_SH_C3[6] * x * (xx - 3.f * yy));
             }
         }
     }
 #undef SHB
     // rows above the active degree stay zero (the reference returns zero-filled dL_dsh)
     for (int k = (deg + 1) * (deg + 1) * 3 - 3; k < (M - 1) * 3; k++) rest[k] = 0.f;
-    // dnormvdv (auxiliary.h:107-117)
-    const f3 o = dir_orig;
+}
+
+// The view-direction term of dL/dmean3D (backward.cu:127-133): dL/ddir = (<dRGBdx, dL/dRGB>, <dRGBdy, ..>,
+// <dRGBdz, ..>) from the Jacobian row `jac` the forward stored, then dnormvdv (auxiliary.h:107-117).
+__device__ __forceinline__ f3 sh_dir_grad(const float *jac, f3 dRGB)
+{
+    return {jac[0] * dRGB.x + jac[1] * dRGB.y + jac[2] * dRGB.z, jac[3] * dRGB.x + jac[4] * dRGB.y + jac[5] * dRGB.z,
+            jac[6] * dRGB.x + jac[7] * dRGB.y + jac[8] * dRGB.z};
+}
+__device__ __forceinline__ void add_dnormvdv(f3 o, f3 ddir, f3 &dmean)
+{
     const float sum2 = o.x * o.x + o.y * o.y + o.z * o.z;
     const float invsum32 = 1.0f / sqrtf(sum2 * sum2 * sum2);
-    dmean.x += ((+sum2 - o.x * o.x) * ddx - o.y * o.x * ddy - o.z * o.x * ddz) * invsum32;
-    dmean.y += (-o.x * o.y * ddx + (sum2 - o.y * o.y) * ddy - o.z * o.y * ddz) * invsum32;
-    dmean.z += (-o.x * o.z * ddx - o.y * o.z * ddy + (sum2 - o.z * o.z) * ddz) * invsum32;
+    dmean.x += ((+sum2 - o.x * o.x) * ddir.x - o.y * o.x * ddir.y - o.z * o.x * ddir.z) * invsum32;
+    dmean.y += (-o.x * o.y * ddir.x + (sum2 - o.y * o.y) * ddir.y - o.z * o.y * ddir.z) * invsum32;
+    dmean.z += (-o.x * o.z * ddir.x - o.y * o.z * ddir.y + (sum2 - o.z * o.z) * ddir.z) * invsum32;
 }
 
 // Another view's SH gradient of one Gaussian, accumulated in registers: acc[3k + c] += basis_k(normalize(dir)) * g_c
@@ -616,8 +619,10 @@ constexpr int PB_O_OPA = PB_O_R11;
 constexpr int PB_O_M3D = PB_O_OPA + PB_T;
 constexpr int PB_O_SCL = PB_O_M3D + PB_T * 3;
 constexpr int PB_O_ROT = PB_O_SCL + PB_T * 3;  // multiple of 4 floats
-constexpr int PB_SHDC = PB_O_R11 + PB_T * 11;  // raw mode: the DC coefficients / their gradient, PB_T*3
-constexpr int PB_SH = PB_SHDC + PB_T * 3 + (PB_T & 3 ? 4 - (PB_T & 3) : 0);  // PB_T * sh_stride
+constexpr int PB_SHDC = PB_O_R11 + PB_T * 11;  // raw mode: the gradient of the DC coefficients, PB_T*3
+// the SH block, PB_T rows of sh_stride floats (raw mode: of 3(M-1)) and at least PB_T*9: it first receives the CTA's
+// Jacobian rows (PB_T*9, read into registers before the first dL/dsh row is written), then the dL/dsh rows
+constexpr int PB_SH = PB_SHDC + PB_T * 3 + (PB_T & 3 ? 4 - (PB_T & 3) : 0);
 static_assert(PB_T % 4 == 0, "every region starts on a 16-byte boundary");
 static_assert(PB_ROTS % 4 == 0 && PB_O_ROT % 4 == 0 && PB_SH % 4 == 0, "16-byte alignment of float4 regions");
 
@@ -656,8 +661,7 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
             mbar_init(&s_bar, 1);
             mbar_fence_init();
             uint32_t bytes = PB_T * 32 + PB_T * 12;
-            if (a.shs) bytes += PB_T * 12;  // dL/dRGB is only an input of the SH backward
-            if (RAW && a.shs) bytes += PB_T * 12 + PB_T * (uint32_t)(a.v.M - 1) * 12;
+            if (a.shs) bytes += PB_T * 12 + PB_T * 36;  // dL/dRGB and the Jacobian rows: inputs of the SH backward only
             if (a.scales) bytes += PB_T * 12 + PB_T * 16;
             if (a.cov_pre) bytes += PB_T * 24;
             // peer mode: the other views' factor blocks of these 64 Gaussians, one bulk copy per view straight out of
@@ -671,13 +675,11 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
                 const int v = u + (u >= a.my_view ? 1 : 0);
                 bulk_g2s(sm + a.pf_off + u * PB_T * 3, a.view_tab[v] + (size_t)base * 3, PB_T * 12, &s_bar);
             }
-            if (RAW && a.shs) {
-                bulk_g2s(sm + PB_SHDC, a.shs + (size_t)base * 3, PB_T * 12, &s_bar);
-                if (a.v.M > 1)
-                    bulk_g2s(sm + PB_SH, a.sh_rest + (size_t)base * (a.v.M - 1) * 3, PB_T * (uint32_t)(a.v.M - 1) * 12, &s_bar);
-            }
             bulk_g2s(sm + PB_GACC, a.gacc + (size_t)base * 8, PB_T * 32, &s_bar);
-            if (a.shs) bulk_g2s(sm + PB_DCOL, a.dcol + (size_t)base * 3, PB_T * 12, &s_bar);
+            if (a.shs) {
+                bulk_g2s(sm + PB_DCOL, a.dcol + (size_t)base * 3, PB_T * 12, &s_bar);
+                bulk_g2s(sm + PB_SH, a.sh_jac + (size_t)base * 9, PB_T * 36, &s_bar);
+            }
             bulk_g2s(sm + PB_MEANS, a.means + (size_t)base * 3, PB_T * 12, &s_bar);
             if (a.scales) {
                 bulk_g2s(sm + PB_SCALES, a.scales + (size_t)base * 3, PB_T * 12, &s_bar);
@@ -687,17 +689,16 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
         }
     } else {
         pb_stage(sm + PB_GACC, a.gacc + (size_t)base * 8, n * 8);
-        if (a.shs) pb_stage(sm + PB_DCOL, a.dcol + (size_t)base * 3, n * 3);
+        if (a.shs) {
+            pb_stage(sm + PB_DCOL, a.dcol + (size_t)base * 3, n * 3);
+            pb_stage(sm + PB_SH, a.sh_jac + (size_t)base * 9, n * 9);
+        }
         pb_stage(sm + PB_MEANS, a.means + (size_t)base * 3, n * 3);
         if (a.scales) {
             pb_stage(sm + PB_SCALES, a.scales + (size_t)base * 3, n * 3);
             pb_stage(sm + PB_ROTS, a.rots + (size_t)base * 4, n * 4);
         }
         if (a.cov_pre) pb_stage(sm + PB_COV, a.cov_pre + (size_t)base * 6, n * 6);
-        if (RAW && a.shs) {
-            pb_stage(sm + PB_SHDC, a.shs + (size_t)base * 3, n * 3);
-            pb_stage(sm + PB_SH, a.sh_rest + (size_t)base * (M - 1) * 3, n * (M - 1) * 3);
-        }
         if (MULTI) {
             const int pulled = min(a.nviews - 1, PB_VB);
             for (int u = 0; u < pulled; u++) {
@@ -708,39 +709,18 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
     }
     float *s_sh = sm + PB_SH;
     const int row_f = RAW ? (M - 1) * 3 : M * 3;  // floats per row of the SH block in shared memory
-    if (!RAW && a.shs) {
-        const float *src = a.shs + (size_t)base * row_f;
-        if (a.sh_vec) {
-            const int row_v = row_f >> 2, total = n * row_v;
-            int r = tid / row_v, c = tid - r * row_v;
-            const int dr = PB_T / row_v, dc = PB_T - dr * row_v;
-            for (int k = tid; k < total; k += PB_T) {
-                // (skipping the rows of culled Gaussians saves 8 % of this kernel's DRAM bytes but the per-chunk
-                // radius test costs more than that: 0.384 vs 0.333 ms at the headline size, round 2)
-                cp_async16(s_sh + r * a.sh_stride + c * 4, src + (size_t)k * 4);
-                r += dr;
-                c += dc;
-                if (c >= row_v) {
-                    c -= row_v;
-                    r++;
-                }
-            }
-        } else {
-            const int total = n * row_f;
-            for (int k = tid; k < total; k += PB_T) {
-                const int r = k / row_f, c = k - r * row_f;
-                cp_async4(s_sh + r * a.sh_stride + c, src + k);
-            }
-        }
-        cp_async_commit();
-    }
     int radius = 0;
     if (tid < n) radius = a.radii[i];
     const int others = MULTI ? a.nviews - 1 : 0;
     __syncthreads();
     if (a.in_bulk_ok && full) mbar_wait(&s_bar, 0);
-    if (!RAW && a.shs) {
-        cp_async_wait<0>();
+    // dL/ddir from this Gaussian's Jacobian row, before the SH block is reused for the dL/dsh rows
+    f3 ddir = {0.f, 0.f, 0.f};
+    if (a.shs) {
+        if (tid < n && radius > 0) {
+            const f3 dRGB = {sm[PB_DCOL + tid * 3], sm[PB_DCOL + tid * 3 + 1], sm[PB_DCOL + tid * 3 + 2]};
+            ddir = sh_dir_grad(s_sh + tid * 9, dRGB);  // stride 9: conflict-free
+        }
         __syncthreads();
     }
 
@@ -918,12 +898,15 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
             dmean.y += (proj[4] * m_w - proj[7] * mul1) * dmx + (proj[5] * m_w - proj[7] * mul2) * dmy;
             dmean.z += (proj[8] * m_w - proj[11] * mul1) * dmx + (proj[9] * m_w - proj[11] * mul2) * dmy;
             if (a.shs) {
-                // accumulated dL/dRGB, already masked where the forward clamped the colour
-                const f3 dRGB = {sm[PB_DCOL + tid * 3], sm[PB_DCOL + tid * 3 + 1], sm[PB_DCOL + tid * 3 + 2]};
                 const float *cp = a.v.campos;
-                sh_backward_inplace<MULTI>(a.v.D, M, RAW ? sm + PB_SHDC + tid * 3 : row, RAW ? row : row + 3,
-                                           {mx - cp[0], my - cp[1], mz - cp[2]}, dRGB, dmean,
-                                           MULTI ? a.dsh_scale : 1.0f, oacc);
+                const f3 dir_orig = {mx - cp[0], my - cp[1], mz - cp[2]};
+                add_dnormvdv(dir_orig, ddir, dmean);
+                if (a.dsh) {
+                    // accumulated dL/dRGB, already masked where the forward clamped the colour
+                    const f3 dRGB = {sm[PB_DCOL + tid * 3], sm[PB_DCOL + tid * 3 + 1], sm[PB_DCOL + tid * 3 + 2]};
+                    sh_grad_row<MULTI>(a.v.D, M, RAW ? sm + PB_SHDC + tid * 3 : row, RAW ? row : row + 3, dir_orig, dRGB,
+                                       MULTI ? a.dsh_scale : 1.0f, oacc);
+                }
             }
             o_m3d[0] = dmean.x;
             o_m3d[1] = dmean.y;
@@ -1425,6 +1408,7 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     a.rots = g->rotations;
     a.shs = g->shs;
     a.cov_pre = g->cov3D_precomp;
+    a.sh_jac = geom.sh_jac;
     a.v.viewmatrix = view->viewmatrix;
     a.v.projmatrix = view->projmatrix;
     a.v.campos = view->campos;
@@ -1471,7 +1455,6 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
             return SGR_EINVAL;
         }
     }
-    a.sh_rest = g->sh_rest;
     a.rec = geom.rec;
     a.dsh_rest = plan ? plan->dL_dsh_rest : nullptr;
     if (raw && g->shs && dL_dsh && g->M > 1 && !a.dsh_rest) {
@@ -1479,9 +1462,9 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
         return SGR_EINVAL;
     }
     auto al16 = [](const void *p) { return ((uintptr_t)p & 15u) == 0; };
+    // (the SH arrays are not read; sh_jac is 256-byte aligned by GeomState::carve)
     a.in_bulk_ok = al16(gacc) && al16(dL_dcolors) && al16(g->means3D) && (!g->scales || al16(g->scales)) &&
-                   (!g->rotations || al16(g->rotations)) && (!g->cov3D_precomp || al16(g->cov3D_precomp)) &&
-                   (!raw || !g->shs || (al16(g->shs) && (g->M == 1 || al16(g->sh_rest))));
+                   (!g->rotations || al16(g->rotations)) && (!g->cov3D_precomp || al16(g->cov3D_precomp));
     a.out_bulk_ok = al16(dL_dmeans2D) && al16(dL_dcov3D) &&
                     (rec11 ? al16(rec11) : (al16(dL_dopacity) && al16(dL_dmeans3D) && al16(dL_dscales) && al16(dL_drotations)));
     if (raw && g->shs && dL_dsh) a.out_bulk_ok = a.out_bulk_ok && al16(dL_dsh) && (g->M == 1 || al16(a.dsh_rest));
@@ -1492,7 +1475,7 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     a.sh_vec = 0;
     if (g->shs && !raw) {
         const int row_f = g->M * 3;
-        if ((row_f % 4) == 0 && al16(g->shs) && al16(dL_dsh)) {
+        if ((row_f % 4) == 0 && al16(dL_dsh)) {  // rows leave as 16-byte stores
             int s4 = row_f / 4;
             if ((s4 & 1) == 0) s4 += 1;
             a.sh_stride = s4 * 4;
@@ -1501,7 +1484,10 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
             a.sh_stride = (row_f & 1) ? row_f : row_f + 1;
         }
     }
-    a.pf_off = PB_SH + PB_T * (raw ? (g->M > 0 ? (g->M - 1) * 3 : 0) : a.sh_stride);
+    // the SH block: dL/dsh rows, and before them the Jacobian rows (9 floats per Gaussian, M = 1 has shorter rows)
+    int sh_block = raw ? (g->M > 0 ? (g->M - 1) * 3 : 0) : a.sh_stride;
+    if (g->shs && sh_block < 9) sh_block = 9;
+    a.pf_off = PB_SH + PB_T * sh_block;
     const int pulled = a.view_tab ? (a.nviews - 1 < PB_VB ? a.nviews - 1 : PB_VB) : 0;
     const size_t dyn = (size_t)(a.pf_off + pulled * PB_T * 3) * sizeof(float) + 16;
     // the per-Gaussian pass, in `num_chunks` Gaussian ranges (multiples of the CTA size) so that a caller

@@ -94,6 +94,40 @@ __device__ __forceinline__ float sh_channel(int deg, const float *dc, const floa
     return res;
 }
 
+// dRGB/d(dir) for one channel: the three sums dRGBdx, dRGBdy, dRGBdz of backward.cu:36-128 (same terms, same
+// grouping), from the coefficients sh_channel has just read.  `rest` points at coefficient 1 of the channel.
+// The backward's view-direction term of dL/dmean3D is their dot product with dL/dRGB, so it needs these nine
+// numbers per Gaussian instead of the whole SH row.
+__device__ __forceinline__ void sh_channel_jacobian(int deg, const float *rest, float x, float y, float z, float &jx,
+                                                    float &jy, float &jz)
+{
+#define SHK(k) rest[((k) - 1) * 3]
+    jx = -SH_C1 * SHK(3);
+    jy = -SH_C1 * SHK(1);
+    jz = SH_C1 * SHK(2);
+    if (deg > 1) {
+        const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+        jx += c_SH_C2[0] * y * SHK(4) + c_SH_C2[2] * 2.f * -x * SHK(6) + c_SH_C2[3] * z * SHK(7) +
+              c_SH_C2[4] * 2.f * x * SHK(8);
+        jy += c_SH_C2[0] * x * SHK(4) + c_SH_C2[1] * z * SHK(5) + c_SH_C2[2] * 2.f * -y * SHK(6) +
+              c_SH_C2[4] * 2.f * -y * SHK(8);
+        jz += c_SH_C2[1] * y * SHK(5) + c_SH_C2[2] * 2.f * 2.f * z * SHK(6) + c_SH_C2[3] * x * SHK(7);
+        if (deg > 2) {
+            jx += c_SH_C3[0] * SHK(9) * 3.f * 2.f * xy + c_SH_C3[1] * SHK(10) * yz + c_SH_C3[2] * SHK(11) * -2.f * xy +
+                  c_SH_C3[3] * SHK(12) * -3.f * 2.f * xz + c_SH_C3[4] * SHK(13) * (-3.f * xx + 4.f * zz - yy) +
+                  c_SH_C3[5] * SHK(14) * 2.f * xz + c_SH_C3[6] * SHK(15) * 3.f * (xx - yy);
+            jy += c_SH_C3[0] * SHK(9) * 3.f * (xx - yy) + c_SH_C3[1] * SHK(10) * xz +
+                  c_SH_C3[2] * SHK(11) * (-3.f * yy + 4.f * zz - xx) + c_SH_C3[3] * SHK(12) * -3.f * 2.f * yz +
+                  c_SH_C3[4] * SHK(13) * -2.f * xy + c_SH_C3[5] * SHK(14) * -2.f * yz +
+                  c_SH_C3[6] * SHK(15) * -3.f * 2.f * xy;
+            jz += c_SH_C3[1] * SHK(10) * xy + c_SH_C3[2] * SHK(11) * 4.f * 2.f * yz +
+                  c_SH_C3[3] * SHK(12) * 3.f * (2.f * zz - xx - yy) + c_SH_C3[4] * SHK(13) * 4.f * 2.f * xz +
+                  c_SH_C3[5] * SHK(14) * (xx - yy);
+        }
+    }
+#undef SHK
+}
+
 // Cooperative, coalesced copy of n floats into shared memory (fallback when bulk copy is not legal).
 __device__ __forceinline__ void stage_plain(float *dst, const float *__restrict__ src, int n)
 {
@@ -110,11 +144,14 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
 {
     extern __shared__ __align__(16) float s_sh[];  // PRE_T rows x sh_stride floats (only with SH)
     __shared__ __align__(16) float s_means[PRE_T * 3];
-    __shared__ __align__(16) float s_scales[PRE_T * 3];   // or colors_precomp when scales absent? no: separate below
     __shared__ __align__(16) float4 s_rots[PRE_T];
     __shared__ __align__(16) float s_opac[PRE_T];
     __shared__ __align__(16) float s_col[PRE_T * 3];
-    __shared__ __align__(16) float s_cov[PRE_T * 6];
+    // scales (3 floats) and cov3D_precomp (6) of the CTA's Gaussians; once every thread is past the geometry phase the
+    // same 36 bytes per Gaussian hold its SH Jacobian row on the way out (a separate array would cost the kernel one
+    // of its six CTAs per SM)
+    __shared__ __align__(16) float s_geo[PRE_T * 9];
+    float *const s_scales = s_geo, *const s_cov = s_geo + PRE_T * 3, *const s_jac = s_geo;
     __shared__ __align__(8) uint64_t s_bar;
 
     const int tid = threadIdx.x;
@@ -252,16 +289,21 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
             }
         }
     }
-    if (!RAW && a.shs && a.sh_stride) {
-        if (SGR_PRE_LATE_SH) {
-            s_live[tid] = visible ? 1 : 0;
-            __syncthreads();
-            stage_sh_rows(s_live);
+    if (a.shs) {
+        if (!RAW && a.sh_stride) {
+            if (SGR_PRE_LATE_SH) {
+                s_live[tid] = visible ? 1 : 0;
+                __syncthreads();
+                stage_sh_rows(s_live);
+            }
+            cp_async_wait<0>();
         }
-        cp_async_wait<0>();
-        __syncthreads();
+        __syncthreads();  // SH rows landed; no thread reads s_scales / s_cov any more, s_jac may overwrite them
     }
     if (tid < n) {
+        float jac[9];  // (dRGBdx, dRGBdy, dRGBdz) as RGB triples; zero for culled Gaussians and degree 0
+#pragma unroll
+        for (int k = 0; k < 9; k++) jac[k] = 0.f;
         if (visible) {
             float r, g, b;
             uint32_t clamp_bits = 0;
@@ -283,6 +325,10 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
                 r = sh_channel(a.v.D, dc + 0, rest + 0, x, y, z);
                 g = sh_channel(a.v.D, dc + 1, rest + 1, x, y, z);
                 b = sh_channel(a.v.D, dc + 2, rest + 2, x, y, z);
+                if (a.v.D > 0) {
+#pragma unroll
+                    for (int c = 0; c < 3; c++) sh_channel_jacobian(a.v.D, rest + c, x, y, z, jac[c], jac[3 + c], jac[6 + c]);
+                }
                 // clamped <=> result + 0.5 < 0 (forward.cu:63-70)
                 clamp_bits = (r < -0.5f ? 1u : 0u) | (g < -0.5f ? 2u : 0u) | (b < -0.5f ? 4u : 0u);
                 r = (clamp_bits & 1u) ? 0.0f : __fadd_rn(r, 0.5f);
@@ -310,6 +356,21 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
         } else {
             a.geom.rect[idx] = make_ushort4(0, 0, 0, 0);
             a.radii[idx] = 0;
+        }
+        if (a.shs) {
+#pragma unroll
+            for (int k = 0; k < 9; k++) s_jac[tid * 9 + k] = jac[k];  // stride 9: conflict-free
+        }
+    }
+    // the CTA's Jacobian rows are one contiguous block of sh_jac: coalesced 16-byte stores, evict-first (only the
+    // backward reads them, long after this pass; a single bulk store per CTA measured the same)
+    if (a.shs) {
+        __syncthreads();
+        float *dst = a.geom.sh_jac + (size_t)base * 9;
+        if (full) {
+            for (int k = tid; k < PRE_T * 9 / 4; k += PRE_T) __stcs((float4 *)dst + k, ((const float4 *)s_jac)[k]);
+        } else {
+            for (int k = tid; k < n * 9; k += PRE_T) __stcs(dst + k, s_jac[k]);
         }
     }
 

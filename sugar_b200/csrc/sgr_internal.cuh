@@ -7,12 +7,15 @@
 //   rec    float4[3P]  48 B splat rec  final_T  f32[HW]                      inst_a  u64[C] depth|idx
 //   rect   ushort4[P]   8 B tile rect  n_contrib u32[HW]                     inst_b  u64[C] sort pong
 //   depth  f32[P]       4 B            tile_count u32[T]  tile_start u32[T+1] (plist is laid out FIRST)
-//                                      tile_cursor u32[T] tile_order u32[T] counters u32[16]
+//   sh_jac f32[9P]     36 B            tile_cursor u32[T] tile_order u32[T] counters u32[16]
 //
 // Splat record (what the blend kernels gather, 48 B = 1.5 sectors instead of the reference's
 // three separate gathers xy / conic_opacity / rgb = 3-4 sectors):
 //   rec[0] = (x, y, conic_a, conic_b)   rec[1] = (conic_c, tau, opacity, r)   rec[2] = (g, b, clamp bits, id)
 // tau = conservative power threshold below which alpha < 1/255 is certain (see blend kernels).
+// sh_jac = the SH colour's derivatives by the normalised view direction, three RGB triples per Gaussian
+// (dRGBdx, dRGBdy, dRGBdz of backward.cu:36-128): the backward's view-direction term of dL/dmean3D needs only
+// these, so it never reads the SH coefficients.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -30,14 +33,19 @@ struct GeomState {
     float4 *rec;
     ushort4 *rect;
     float *depth;
-    static size_t bytes(size_t P) { return align_up(P * 48) + align_up(P * 8) + align_up(P * 4) + SGR_ALIGN; }
+    float *sh_jac;  // [P][9] (dRGB/dx, dRGB/dy, dRGB/dz) of the SH colour; zero rows for culled Gaussians
+    static size_t bytes(size_t P)
+    {
+        return align_up(P * 48) + align_up(P * 8) + align_up(P * 4) + align_up(P * 36) + SGR_ALIGN;
+    }
     static GeomState carve(void *base, size_t P)
     {
         char *p = (char *)align_up((size_t)base);
         GeomState s;
         s.rec = (float4 *)p; p += align_up(P * 48);
         s.rect = (ushort4 *)p; p += align_up(P * 8);
-        s.depth = (float *)p;
+        s.depth = (float *)p; p += align_up(P * 4);
+        s.sh_jac = (float *)p;
         return s;
     }
 };
