@@ -7,7 +7,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("SGR_LIB_PATH", os.path.join(_HERE, "lib", "libsugar_b200.so"))  # override: A/B builds
+LIB_PATH = os.environ.get("SGR_LIB_PATH", os.path.join(_HERE, "lib", "libsugar_b200.so"))  # override: the stats build (scripts/blend_stats.py)
 
 
 class SgrError(RuntimeError):

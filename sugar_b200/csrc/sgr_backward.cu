@@ -19,21 +19,11 @@
 
 namespace sgr {
 
-// Record pipeline of the backward blend.  SGR_BWD_PIPE3 = 1 (default): SGR_BWD_NS stages of SGR_BWD_B records with
-// full / empty mbarriers -- a warp waits only for the loader warps' data, never for its sibling warps, so the
-// tile's eight warps may drift NS - 2 batches apart and the statistical imbalance between the blocks of one batch
-// (the busiest block of a 128-record batch does 1.32x the mean) is averaged over more records: 1.029 -> 0.973 ms
-// at the headline size against SGR_BWD_PIPE3 = 0 (two stages of 128 records, two CTA barriers per batch).
-#ifndef SGR_BWD_PIPE3
-#define SGR_BWD_PIPE3 1
-#endif
-#ifndef SGR_BWD_NS
-#define SGR_BWD_NS 3
-#endif
-#ifndef SGR_BWD_B
-#define SGR_BWD_B (SGR_BWD_PIPE3 ? 96 : 128)
-#endif
-constexpr int BWD_B = SGR_BWD_B;  // Gaussians per shared-memory batch (loader threads: the first BWD_B of the CTA)
+// Record pipeline of the backward blend: BWD_NS stages of BWD_B records with full / empty mbarriers.  A warp waits
+// only for the loader warps' data, never for its sibling warps, so the tile's eight warps may drift BWD_NS - 2 batches
+// apart and the statistical imbalance between the blocks of one batch is averaged over more records.
+constexpr int BWD_B = 96;   // Gaussians per shared-memory batch (loader threads: the first BWD_B of the CTA)
+constexpr int BWD_NS = 3;   // record stages
 constexpr int BWD_NW = 8;   // warps per CTA (16x16 pixels)
 
 // Blend accumulators (zeroed by a memset before the blend pass):
@@ -92,11 +82,10 @@ constexpr int CH_PITCH = CH + 1;   // float2 elements per pixel row: odd pitch =
 // (57.2 KB per CTA in total with three record stages: four CTAs per SM fit, with 64 registers per thread)
 constexpr uint32_t CB_META = 32 * CH_PITCH * 8, CB_DP = CB_META + CH * 32, CB_BYTES = CB_DP + 32 * 16;
 // CTA shared-memory map (dynamic): the record stages, their membership words, the mbarriers, chunk scratch
-constexpr uint32_t BWD_NS = SGR_BWD_PIPE3 ? SGR_BWD_NS : 2;  // record stages
 constexpr uint32_t SM_A = 0, SM_B = SM_A + BWD_NS * BWD_B * 16, SM_C = SM_B + BWD_NS * BWD_B * 16,
                    SM_MEMBER = SM_C + BWD_NS * BWD_B * 16,
-                   SM_BAR = SM_MEMBER + (SGR_BWD_PIPE3 ? BWD_NS : 1) * BWD_NW * (BWD_B / 32) * 4,  // PIPE3: full[3], empty[3]
-                   SM_LAST = SM_BAR + (SGR_BWD_PIPE3 ? 2 * BWD_NS * 8 : 0), SM_CHUNK = SM_LAST + 16,
+                   SM_BAR = SM_MEMBER + BWD_NS * BWD_NW * (BWD_B / 32) * 4,  // full[BWD_NS], empty[BWD_NS]
+                   SM_LAST = SM_BAR + 2 * BWD_NS * 8, SM_CHUNK = SM_LAST + 16,
                    BWD_SMEM_BYTES = SM_CHUNK + BWD_NW * CB_BYTES;
 static_assert(SM_BAR % 8 == 0 && BWD_B % 32 == 0, "mbarriers are 8-byte aligned; a batch is whole membership words");
 static_assert(4 * (BWD_SMEM_BYTES + 1024) <= 228 * 1024, "four CTAs of the backward blend must fit one SM's shared memory");
@@ -239,25 +228,13 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
     int nfill = 0;
     const float blk_x0 = (float)bx0, blk_y0 = (float)by0;
 
-    // record pipeline (threads 0..BWD_B-1 own one slot of every batch): issue() starts the async
-    // copies of one splat record into buffer `buf`; list words are fetched one batch further ahead
+    // record pipeline (threads 0..BWD_B-1 own one slot of every batch)
     const bool loader = tid < BWD_B;
     auto fetch = [&](int b0) -> uint32_t {
         // back to front; dead instances (packed list, empty footprint) are dropped here: 0xffffffff
         if (!(loader && b0 + tid < n)) return 0xffffffffu;
         const uint32_t w = plist[lo + (uint32_t)(n - 1 - (b0 + tid))];
         return (packed && (w & 0xffu) == 0u) ? 0xffffffffu : w;
-    };
-    auto issue = [&](uint32_t w, int buf) {
-        if (w != 0xffffffffu) {
-            const uint32_t id = packed ? (w >> 8) : w;
-            const float4 *r = rec + (size_t)id * 3;
-            const uint32_t e = buf * BWD_B + tid;
-            cp_async16_a(sm + SM_A + e * 16, r);
-            cp_async16_a(sm + SM_B + e * 16, r + 1);
-            cp_async16_a(sm + SM_C + e * 16, r + 2);
-        }
-        cp_async_commit();
     };
     // membership words of the batch in stage `st` from the loader threads' masks
     auto publish_members = [&](uint32_t mask, uint32_t(*set)[BWD_B / 32]) {
@@ -267,22 +244,20 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
             if (lane == 0) set[blk][wid] = word;
         }
     };
-#if SGR_BWD_PIPE3
-    constexpr int NS = (int)BWD_NS;
-    uint64_t *bars = (uint64_t *)(s_raw + SM_BAR);  // full[0..NS) then empty[0..NS)
+    uint64_t *bars = (uint64_t *)(s_raw + SM_BAR);  // full[0..BWD_NS) then empty[0..BWD_NS)
     if (tid == 0) {
-        for (int st = 0; st < NS; st++) {
-            mbar_init(&bars[st], 2 * BWD_B);      // per loader thread: one async arrive (copies landed) + one plain
-            mbar_init(&bars[NS + st], BWD_NW);    // one arrive per warp when it is done with the stage
+        for (int st = 0; st < BWD_NS; st++) {
+            mbar_init(&bars[st], 2 * BWD_B);         // per loader thread: one async arrive (copies landed) + one plain
+            mbar_init(&bars[BWD_NS + st], BWD_NW);  // one arrive per warp when it is done with the stage
         }
         mbar_fence_init();
     }
     __syncthreads();
     const int nb = (n + BWD_B - 1) / BWD_B;
-    // loader warps: fill stage b % NS with batch b (waits until every warp has released the stage's previous batch)
+    // loader warps: fill stage b % BWD_NS with batch b (waits until every warp has released the stage's previous batch)
     auto produce = [&](int b) {
-        const int st = b % NS;
-        if (b >= NS) mbar_wait(&bars[NS + st], (uint32_t)((b / NS - 1) & 1));
+        const int st = b % BWD_NS;
+        if (b >= BWD_NS) mbar_wait(&bars[BWD_NS + st], (uint32_t)((b / BWD_NS - 1) & 1));
         const uint32_t w = fetch(b * BWD_B);
         uint32_t mask = 0;
         if (w != 0xffffffffu) {
@@ -308,41 +283,12 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
     };
     if (loader) produce(0);
     for (int b = 0; b < nb; b++) {
-        const int b0 = b * BWD_B, buf = b % NS;
+        const int b0 = b * BWD_B, buf = b % BWD_NS;
         const uint32_t sa = sm + SM_A + buf * (BWD_B * 16), sb = sm + SM_B + buf * (BWD_B * 16),
                        sc = sm + SM_C + buf * (BWD_B * 16);
         if (loader && b + 1 < nb) produce(b + 1);
-        mbar_wait(&bars[buf], (uint32_t)((b / NS) & 1));  // batch b has landed and its membership words are visible
+        mbar_wait(&bars[buf], (uint32_t)((b / BWD_NS) & 1));  // batch b has landed and its membership words are visible
         const uint32_t(*member)[BWD_B / 32] = s_member + buf * BWD_NW;
-#else
-    uint32_t w_cur = fetch(0);
-    issue(w_cur, 0);
-    uint32_t w_next = fetch(BWD_B);
-
-    for (int b0 = 0, buf = 0; b0 < n; b0 += BWD_B, buf ^= 1) {
-        const uint32_t sa = sm + SM_A + buf * (BWD_B * 16), sb = sm + SM_B + buf * (BWD_B * 16),
-                       sc = sm + SM_C + buf * (BWD_B * 16);
-        cp_async_wait<0>();
-        __syncthreads();  // batch b0 has landed in `buf`; every warp is done with the other buffer
-        if (loader) {
-            uint32_t mask = 0;
-            if (w_cur != 0xffffffffu) {
-                if (packed) {
-                    mask = w_cur & 0xffu;
-                } else {
-                    const float4 r0 = lds128(sa + tid * 16), r1 = lds128(sb + tid * 16);
-                    mask = block_mask_of_record(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, tx0, ty0);
-                }
-            }
-            publish_members(mask, s_member);
-            // next batch's records start moving now; they are not needed before the next barrier
-            issue(w_next, buf ^ 1);
-            w_cur = w_next;
-            w_next = fetch(b0 + 2 * BWD_B);
-        }
-        __syncthreads();
-        const uint32_t(*member)[BWD_B / 32] = s_member;
-#endif
         const int m = min(BWD_B, n - b0);
 #ifdef SGR_BLEND_STATS
         if (tid == 0) BWD_STAT(6, m);
@@ -429,10 +375,8 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
                 }
             }
         }
-#if SGR_BWD_PIPE3
         __syncwarp();
-        if (lane == 0) mbar_arrive(&bars[NS + buf]);  // this warp no longer reads the stage
-#endif
+        if (lane == 0) mbar_arrive(&bars[BWD_NS + buf]);  // this warp no longer reads the stage
     }
     if (nfill) chunk_flush(cb, nfill, blk_x0, blk_y0, 0.5f * W, 0.5f * H, gacc, dcol);
 }
@@ -599,11 +543,9 @@ __device__ __forceinline__ void sh_accumulate(int deg, float *acc, f3 dir_orig, 
 #undef SHA
 }
 
-#ifndef SGR_PB_T
-#define SGR_PB_T 64
-#endif
 constexpr int PB_VB = 7;  // other views whose factors a thread fetches at the top of the kernel (8 ranks: all of them)
-constexpr int PB_T = SGR_PB_T;
+constexpr int PB_T = 64;
+static_assert(PB_T == 64, "the peer record exchange (sgr_peer.cu) works in blocks of 64 records");
 // dynamic shared memory carve-up (floats): inputs, outputs, then the SH block
 constexpr int PB_GACC = 0;                     // PB_T*8
 constexpr int PB_DCOL = PB_GACC + PB_T * 8;    // PB_T*3
@@ -1055,10 +997,7 @@ __device__ __forceinline__ const float *view_block(const float *base, size_t str
 }
 
 constexpr int SF_T = 256;  // 64 Gaussians per CTA, four threads each
-#ifndef SGR_SF_VB
-#define SGR_SF_VB 4
-#endif
-constexpr int SF_VB = SGR_SF_VB;  // views whose factors a thread fetches before it uses any
+constexpr int SF_VB = 4;  // views whose factors a thread fetches before it uses any
 
 // Four threads per Gaussian: thread q owns SH coefficients 4q .. 4q+3, i.e. 48 contiguous bytes of the row
 // (three 16-byte stores; the four threads of a Gaussian cover its 192-byte row, a warp 1.5 KB without gaps), and
@@ -1450,8 +1389,8 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
         a.my_view = plan->peer_rank;
         a.dsh_scale = plan->peer_dsh_scale;
         a.stage_tab = (float *const *)plan->peer_record_stages;
-        if (a.stage_tab && (!rec11 || PB_T != 64)) {
-            set_error("peer_record_stages needs reduce_records (the local staging array) and 64-thread CTAs");
+        if (a.stage_tab && !rec11) {
+            set_error("peer_record_stages needs reduce_records (the local staging array)");
             return SGR_EINVAL;
         }
     }
@@ -1468,9 +1407,6 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     a.out_bulk_ok = al16(dL_dmeans2D) && al16(dL_dcov3D) &&
                     (rec11 ? al16(rec11) : (al16(dL_dopacity) && al16(dL_dmeans3D) && al16(dL_dscales) && al16(dL_drotations)));
     if (raw && g->shs && dL_dsh) a.out_bulk_ok = a.out_bulk_ok && al16(dL_dsh) && (g->M == 1 || al16(a.dsh_rest));
-#ifdef SGR_PB_NO_BULK_STORE
-    a.out_bulk_ok = 0;
-#endif
     a.sh_stride = 0;
     a.sh_vec = 0;
     if (g->shs && !raw) {

@@ -4,14 +4,16 @@
 //   preprocessCUDA            forward.cu:155-256      -> preprocess_kernel   (+ per-tile counting)
 //   InclusiveSum + D2H sync   rasterizer_impl.cu:277-281 -> tile_scan_kernel (over TILES, not Gaussians)
 //   duplicateWithKeys         rasterizer_impl.cu:70-111  -> scatter_kernel   (atomic cursor per tile)
-//   cub SortPairs (6 passes)  rasterizer_impl.cu:303-308 -> tile_sort_kernel (per-tile LSD radix in smem)
+//   cub SortPairs (6 passes)  rasterizer_impl.cu:303-308 -> tile_sort_{bucket,merge}_kernel (per tile, in smem),
+//                                                          tile_sort_global_kernel (tiles above SORT_CAP)
 //   identifyTileRanges        rasterizer_impl.cu:116-138 -> (ranges fall out of the tile scan)
 //   renderCUDA                forward.cu:261-374      -> blend_forward_kernel
 //
 // Binning design: the 64-bit key (tile<<32 | depth) is sorted MSD-first.  The tile digit is a
 // counting sort (per-tile counts by L2 atomics in preprocess, exclusive scan over tiles, atomic
-// cursor scatter), the remaining (depth, gaussian-id) order is an 8-bit LSD radix sort done
-// entirely in one CTA's shared memory per tile.  Instances move through HBM once (8 B write,
+// cursor scatter), the remaining (depth, gaussian-id) order is sorted by one CTA per tile in its
+// shared memory (bucket or merge sort by size class; tiles of more than SORT_CAP instances take an
+// 8-bit LSD radix sort through global memory).  Instances move through HBM once (8 B write,
 // 8 B read, 4 B write) instead of ~150 B for six global radix passes, and the sorted order is
 // exactly the reference's: by tile, then depth bits, then Gaussian index (the reference's
 // stable sort keeps emission order = index order among equal keys).
@@ -28,10 +30,7 @@ namespace sgr {
 // ------------------------------------------------------------------------------------------------
 // preprocess
 // ------------------------------------------------------------------------------------------------
-#ifndef SGR_PRE_T
-#define SGR_PRE_T 128
-#endif
-constexpr int PRE_T = SGR_PRE_T;
+constexpr int PRE_T = 128;
 
 struct PreArgs {
     int P;
@@ -200,10 +199,7 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
         }
     }
     // ---- SH rows: coalesced cp.async into bank-conflict-free padded rows -----------------------
-    // (sh_stride == 0 selects the direct path: each surviving thread reads its own row from global)
-    // SGR_PRE_LATE_SH (A/B knob): issue the row copies only after the cull, for the surviving rows; saves the
-    // bytes of culled Gaussians' coefficients at the price of exposing the copy latency behind the geometry phase.
-    auto stage_sh_rows = [&](const unsigned char *row_live) {
+    if (!RAW && a.shs) {
         const int row_f = a.v.M * 3;
         const float *src = a.shs + (size_t)base * row_f;
         if (a.sh_vec) {
@@ -211,7 +207,7 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
             int r = tid / row_v, c = tid - r * row_v;  // (row, 16-byte column) advanced without divisions
             const int dr = PRE_T / row_v, dc = PRE_T - dr * row_v;
             for (int i = tid; i < total; i += PRE_T) {
-                if (!row_live || row_live[r]) cp_async16(s_sh + r * a.sh_stride + c * 4, src + (size_t)i * 4);
+                cp_async16(s_sh + r * a.sh_stride + c * 4, src + (size_t)i * 4);
                 r += dr;
                 c += dc;
                 if (c >= row_v) {
@@ -223,16 +219,11 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
             const int total = n * row_f;
             for (int i = tid; i < total; i += PRE_T) {
                 const int r = i / row_f, c = i - r * row_f;
-                if (!row_live || row_live[r]) cp_async4(s_sh + r * a.sh_stride + c, src + i);
+                cp_async4(s_sh + r * a.sh_stride + c, src + i);
             }
         }
         cp_async_commit();
-    };
-#ifndef SGR_PRE_LATE_SH
-#define SGR_PRE_LATE_SH 0
-#endif
-    __shared__ unsigned char s_live[PRE_T];
-    if (!SGR_PRE_LATE_SH && !RAW && a.shs && a.sh_stride) stage_sh_rows(nullptr);
+    }
     __syncthreads();  // barrier init visible / plain staging complete
     if (a.bulk_ok && full) mbar_wait(&s_bar, 0);
 
@@ -290,14 +281,7 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
         }
     }
     if (a.shs) {
-        if (!RAW && a.sh_stride) {
-            if (SGR_PRE_LATE_SH) {
-                s_live[tid] = visible ? 1 : 0;
-                __syncthreads();
-                stage_sh_rows(s_live);
-            }
-            cp_async_wait<0>();
-        }
+        if (!RAW) cp_async_wait<0>();
         __syncthreads();  // SH rows landed; no thread reads s_scales / s_cov any more, s_jac may overwrite them
     }
     if (tid < n) {
@@ -319,7 +303,7 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
                     dc = s_col + tid * 3;
                     rest = s_sh + tid * (a.v.M - 1) * 3;
                 } else {
-                    dc = a.sh_stride ? s_sh + tid * a.sh_stride : a.shs + (size_t)idx * a.v.M * 3;
+                    dc = s_sh + tid * a.sh_stride;
                     rest = dc + 3;
                 }
                 r = sh_channel(a.v.D, dc + 0, rest + 0, x, y, z);
@@ -494,10 +478,6 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(const uint32_t *__restr
 // arithmetic it does while they are in flight is free: this is where the exact footprint mask of every
 // instance (sgr_internal.cuh, block_mask) is computed -- once, for both blend kernels.
 // ------------------------------------------------------------------------------------------------
-#ifndef SGR_SCATTER_SMALL
-#define SGR_SCATTER_SMALL 6
-#endif
-
 __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushort4 *__restrict__ rect,
                                                       const float *__restrict__ depth, const float4 *__restrict__ rec,
                                                       uint32_t *__restrict__ cursor,
@@ -525,7 +505,7 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushor
     // Rects of up to SMALL tiles are walked by their own thread: masks first (pure arithmetic), then all
     // the slot claims back to back (the returning atomics are in flight together), then the stores.
     // Larger rects are walked cooperatively by the whole warp, one tile per lane.
-    constexpr int SMALL = SGR_SCATTER_SMALL;
+    constexpr int SMALL = 6;
     static_assert(SMALL <= 8, "masks of a small rect are packed into one 64-bit register");
     const int rw = (int)rc.z - (int)rc.x, rcnt = (rc.z > rc.x && rc.w > rc.y) ? rw * ((int)rc.w - (int)rc.y) : 0;
     const uint32_t low_id = packed ? ((uint32_t)idx << 8) : (uint32_t)idx;
@@ -608,21 +588,20 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushor
 }
 
 // ------------------------------------------------------------------------------------------------
-// per-tile sort of (depth|id) words: LSD radix, 8-bit digits, warp-private histograms,
-// match_any ranking (stable), constant bytes skipped.  SMEM variant keeps both ping-pong buffers
-// in shared memory; the GLOBAL variant (tiles with more than SORT_CAP instances) ping-pongs
-// between inst_a and inst_b in L2/HBM with the same code.
+// per-tile sort of the tiles with more than SORT_CAP instances: LSD radix on the (depth|id) words,
+// 8-bit digits, warp-private histograms, match_any ranking (stable), constant bytes skipped; the
+// words ping-pong between inst_a and inst_b in L2/HBM.
 // ------------------------------------------------------------------------------------------------
-constexpr int SORT_CAP = 8192;  // largest shared-memory (bitonic) class; above it: global radix
+constexpr int SORT_CAP = 8192;  // largest shared-memory (merge sort) class; above it: global radix
+constexpr int GSORT_T = 1024;
 
-template <int THREADS, bool GLOBAL>
-__global__ void __launch_bounds__(THREADS) tile_sort_kernel(const uint32_t *__restrict__ tile_start,
-                                                            const uint32_t *__restrict__ counters, uint64_t capacity,
-                                                            uint64_t *__restrict__ inst_a, uint64_t *__restrict__ inst_b,
-                                                            uint32_t *__restrict__ plist, int num_tiles)
+__global__ void __launch_bounds__(GSORT_T) tile_sort_global_kernel(const uint32_t *__restrict__ tile_start,
+                                                                   const uint32_t *__restrict__ counters,
+                                                                   uint64_t capacity, uint64_t *__restrict__ inst_a,
+                                                                   uint64_t *__restrict__ inst_b,
+                                                                   uint32_t *__restrict__ plist, int num_tiles)
 {
-    constexpr int NW = THREADS / 32;
-    extern __shared__ __align__(16) uint64_t s_keys[];  // SMEM variant: 2 * SORT_CAP
+    constexpr int NW = GSORT_T / 32;
     __shared__ uint32_t s_hist[NW][256];
     __shared__ uint32_t s_diff[2];
     __shared__ uint32_t s_wsum[32];
@@ -632,27 +611,18 @@ __global__ void __launch_bounds__(THREADS) tile_sort_kernel(const uint32_t *__re
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const uint32_t lo = tile_start[tile];
     const int n = (int)(tile_start[tile + 1] - lo);
-    if (GLOBAL ? (n <= SORT_CAP) : (n > SORT_CAP || n == 0)) continue;
+    if (n <= SORT_CAP) continue;
 
-    uint64_t *src, *dst;
-    if (GLOBAL) {
-        src = inst_a + lo;
-        dst = inst_b + lo;
-    } else {
-        src = s_keys;
-        dst = s_keys + SORT_CAP;
-    }
+    uint64_t *src = inst_a + lo, *dst = inst_b + lo;
 
-    // load (SMEM) + find which key bytes vary inside this tile
+    // find which key bytes vary inside this tile
     if (tid < 2) s_diff[tid] = 0;
     __syncthreads();
     {
         const uint64_t k0 = inst_a[lo];
         uint32_t dlo = 0, dhi = 0;
-        for (int i = tid; i < n; i += THREADS) {
-            const uint64_t k = inst_a[lo + i];
-            if (!GLOBAL) src[i] = k;
-            const uint64_t x = k ^ k0;
+        for (int i = tid; i < n; i += GSORT_T) {
+            const uint64_t x = inst_a[lo + i] ^ k0;
             dlo |= (uint32_t)x;
             dhi |= (uint32_t)(x >> 32);
         }
@@ -672,7 +642,7 @@ __global__ void __launch_bounds__(THREADS) tile_sort_kernel(const uint32_t *__re
 
     for (int shift = 0; shift < 64; shift += 8) {
         if (((diff >> shift) & 0xffull) == 0) continue;
-        for (int i = tid; i < NW * 256; i += THREADS) (&s_hist[0][0])[i] = 0;
+        for (int i = tid; i < NW * 256; i += GSORT_T) (&s_hist[0][0])[i] = 0;
         __syncthreads();
         // pass 1: warp-private digit histogram
         for (int i = w_lo + lane; i - lane < w_hi; i += 32) {
@@ -732,7 +702,7 @@ __global__ void __launch_bounds__(THREADS) tile_sort_kernel(const uint32_t *__re
         src = dst;
         dst = t;
     }
-    for (int i = tid; i < n; i += THREADS) plist[lo + i] = (uint32_t)src[i];
+    for (int i = tid; i < n; i += GSORT_T) plist[lo + i] = (uint32_t)src[i];
     __syncthreads();
     }
 }
@@ -746,10 +716,7 @@ __global__ void __launch_bounds__(THREADS) tile_sort_kernel(const uint32_t *__re
 // Size classes (LOWER, CAP]: each class is its own launch over all tiles with early exit, so the
 // shared-memory footprint (and occupancy) matches the tile population.
 // ------------------------------------------------------------------------------------------------
-#ifndef SGR_SORT_VT
-#define SGR_SORT_VT 8
-#endif
-constexpr int SORT_VT = SGR_SORT_VT;  // words per thread in the per-tile merge sort
+constexpr int SORT_VT = 8;  // words per thread in the per-tile merge sort
 
 __device__ __forceinline__ void cswap(uint64_t &a, uint64_t &b)
 {
@@ -757,8 +724,6 @@ __device__ __forceinline__ void cswap(uint64_t &a, uint64_t &b)
     a = lo;
     b = hi;
 }
-
-#define SGR_NET16 cswap(r[0], r[1]); cswap(r[2], r[3]); cswap(r[4], r[5]); cswap(r[6], r[7]); cswap(r[8], r[9]); cswap(r[10], r[11]); cswap(r[12], r[13]); cswap(r[14], r[15]); cswap(r[0], r[2]); cswap(r[1], r[3]); cswap(r[4], r[6]); cswap(r[5], r[7]); cswap(r[8], r[10]); cswap(r[9], r[11]); cswap(r[12], r[14]); cswap(r[13], r[15]); cswap(r[1], r[2]); cswap(r[5], r[6]); cswap(r[9], r[10]); cswap(r[13], r[14]); cswap(r[0], r[4]); cswap(r[1], r[5]); cswap(r[2], r[6]); cswap(r[3], r[7]); cswap(r[8], r[12]); cswap(r[9], r[13]); cswap(r[10], r[14]); cswap(r[11], r[15]); cswap(r[2], r[4]); cswap(r[3], r[5]); cswap(r[10], r[12]); cswap(r[11], r[13]); cswap(r[1], r[2]); cswap(r[3], r[4]); cswap(r[5], r[6]); cswap(r[9], r[10]); cswap(r[11], r[12]); cswap(r[13], r[14]); cswap(r[0], r[8]); cswap(r[1], r[9]); cswap(r[2], r[10]); cswap(r[3], r[11]); cswap(r[4], r[12]); cswap(r[5], r[13]); cswap(r[6], r[14]); cswap(r[7], r[15]); cswap(r[4], r[8]); cswap(r[5], r[9]); cswap(r[6], r[10]); cswap(r[7], r[11]); cswap(r[2], r[4]); cswap(r[3], r[5]); cswap(r[6], r[8]); cswap(r[7], r[9]); cswap(r[10], r[12]); cswap(r[11], r[13]); cswap(r[1], r[2]); cswap(r[3], r[4]); cswap(r[5], r[6]); cswap(r[7], r[8]); cswap(r[9], r[10]); cswap(r[11], r[12]); cswap(r[13], r[14]);
 
 // In-place merge sort of s_keys[0..n) by the NT threads of the CTA (all must call).  s_keys must
 // have room for ceil(n/VT)*VT words; n <= NT*VT.
@@ -776,16 +741,12 @@ __device__ __forceinline__ void block_merge_sort(uint64_t *s_keys, const int n)
             const int i = tid * VT + k;
             r[k] = i < n ? s_keys[i] : ~0ull;
         }
-        // Batcher odd-even merge sort network on the VT registers (19 comparators for 8, 63 for 16)
-        static_assert(VT == 8 || VT == 16, "sorting network written out for 8 or 16 words per thread");
-        if constexpr (VT == 8) {
-            cswap(r[0], r[1]); cswap(r[2], r[3]); cswap(r[4], r[5]); cswap(r[6], r[7]); cswap(r[0], r[2]);
-            cswap(r[1], r[3]); cswap(r[4], r[6]); cswap(r[5], r[7]); cswap(r[1], r[2]); cswap(r[5], r[6]);
-            cswap(r[0], r[4]); cswap(r[1], r[5]); cswap(r[2], r[6]); cswap(r[3], r[7]); cswap(r[2], r[4]);
-            cswap(r[3], r[5]); cswap(r[1], r[2]); cswap(r[3], r[4]); cswap(r[5], r[6]);
-        } else {
-            SGR_NET16
-        }
+        // Batcher odd-even merge sort network on the VT registers (19 comparators)
+        static_assert(VT == 8, "sorting network written out for 8 words per thread");
+        cswap(r[0], r[1]); cswap(r[2], r[3]); cswap(r[4], r[5]); cswap(r[6], r[7]); cswap(r[0], r[2]);
+        cswap(r[1], r[3]); cswap(r[4], r[6]); cswap(r[5], r[7]); cswap(r[1], r[2]); cswap(r[5], r[6]);
+        cswap(r[0], r[4]); cswap(r[1], r[5]); cswap(r[2], r[6]); cswap(r[3], r[7]); cswap(r[2], r[4]);
+        cswap(r[3], r[5]); cswap(r[1], r[2]); cswap(r[3], r[4]); cswap(r[5], r[6]);
     }
     __syncthreads();  // every thread has read its window before anyone overwrites it
     if (tid < nact) {
@@ -981,9 +942,6 @@ __global__ void __launch_bounds__(BK_T) tile_sort_bucket_kernel(const uint32_t *
 // Tiles are taken heaviest first (tile_order).
 // ------------------------------------------------------------------------------------------------
 constexpr int BLEND_T = 256;
-#ifndef SGR_FWD_MIN_BLOCKS
-#define SGR_FWD_MIN_BLOCKS 1   // A/B knob: resident CTAs/SM the register allocation must allow
-#endif
 
 // -DSGR_BLEND_STATS: count what the blend loops do (scripts/blend_stats.py); never in the shipped build
 #ifdef SGR_BLEND_STATS
@@ -991,8 +949,10 @@ __device__ unsigned long long g_fwd_stats[8];
 #define FWD_STAT(k, v) atomicAdd(&g_fwd_stats[k], (unsigned long long)(v))
 #endif
 
+// The minimum of one resident CTA per SM is not redundant: without it nvcc allocates fewer registers (40 instead of 51
+// for the unpacked list format) and generates different code.
 template <bool packed>
-__global__ void __launch_bounds__(BLEND_T, SGR_FWD_MIN_BLOCKS) blend_forward_kernel(const uint32_t *__restrict__ tile_order,
+__global__ void __launch_bounds__(BLEND_T, 1) blend_forward_kernel(const uint32_t *__restrict__ tile_order,
                                                                 const uint32_t *__restrict__ tile_start,
                                                                 const uint32_t *__restrict__ plist,
                                                                 const float4 *__restrict__ rec,
@@ -1208,18 +1168,13 @@ static int launch_binning_and_blend(const ViewConsts &v, int P, const GeomState 
     const int small_grid = T < slots ? T : slots;  // 2 CTAs per SM, grid-stride over tiles
     tile_sort_merge_kernel<512, 0><<<T, 512 / SORT_VT, 512 * 8, st>>>(img.tile_start, img.counters, capacity, bin.inst_a,
                                                                       bin.plist, T);
-#ifdef SGR_SORT_MERGE_ONLY
-    tile_sort_merge_kernel<2048, 512><<<T, 2048 / SORT_VT, 2048 * 8, st>>>(img.tile_start, img.counters, capacity,
-                                                                           bin.inst_a, bin.plist, T);
-#else
     tile_sort_bucket_kernel<<<T, BK_T, 0, st>>>(img.tile_start, img.counters, capacity, bin.inst_a, bin.plist, T, 512);
-#endif
     tile_sort_merge_kernel<8192, 2048><<<small_grid, 8192 / SORT_VT, 8192 * 8, st>>>(img.tile_start, img.counters,
                                                                                      capacity, bin.inst_a, bin.plist, T);
     sgr::prof_end(st);
     SGR_LAUNCH(K_SORT_GLOBAL, st,
-               tile_sort_kernel<1024, true><<<small_grid, 1024, 0, st>>>(img.tile_start, img.counters, capacity,
-                                                                        bin.inst_a, bin.inst_b, bin.plist, T));
+               tile_sort_global_kernel<<<small_grid, GSORT_T, 0, st>>>(img.tile_start, img.counters, capacity,
+                                                                       bin.inst_a, bin.inst_b, bin.plist, T));
     SGR_LAUNCH(K_BLEND_FWD, st,
                if (ids_packed(P))
                    blend_forward_kernel<true><<<T, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec,
@@ -1307,11 +1262,6 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
             a.sh_stride = (row_f & 1) ? row_f : row_f + 1;
         }
         dyn = (size_t)PRE_T * a.sh_stride * sizeof(float);
-#ifdef SGR_PRE_DIRECT_SH
-        a.sh_stride = 0;
-        a.sh_vec = 0;
-        dyn = 0;
-#endif
     }
     a.geom = geom;
     a.radii = radii;

@@ -22,7 +22,6 @@
 // waits for its peers once per backward (BLEND); a wait that outlives its timeout traps (the context dies with an error
 // instead of hanging the box).
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "sgr_internal.cuh"
@@ -321,13 +320,9 @@ int sgr_peer_reduce_records_synced(const void *const *rec_tab, void *const *sum_
     if (q1 == q0 && !flag_tab) return SGR_OK;  // nothing owned and nobody to tell
     cudaStream_t st = (cudaStream_t)stream;
     const int T = 256;
-    // 2 CTAs of 256 threads per SM by default, grid-stride over the slice
+    // at most 2 CTAs of 256 threads per SM, grid-stride over the slice
     size_t blocks = (q1 - q0 + T - 1) / T;
-    static const size_t cap = [] {
-        const char *e = getenv("SGR_PEER_REDUCE_BLOCKS");
-        const long v = e ? atol(e) : 0;
-        return (size_t)(v > 0 ? v : device_sm_count() * 2);
-    }();
+    const size_t cap = (size_t)device_sm_count() * 2;
     if (blocks > cap) blocks = cap;
     if (blocks == 0) blocks = 1;  // the handshake still runs
     PeerSync sy;

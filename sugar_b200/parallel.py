@@ -99,10 +99,6 @@ def _peer_auto_worlds():
     return tuple(int(x) for x in e.split(",") if x.strip()) if e else PEER_AUTO_WORLDS
 
 
-_PEER_SERIAL = os.environ.get("SGR_PEER_SERIAL", "0") == "1"                 # diagnostics (scripts/timeline_peer.py)
-_PEER_LOCAL_FACTORS = os.environ.get("SGR_PEER_LOCAL_FACTORS", "0") == "1"
-
-
 class _DevMem:
     """A raw device range as seen by torch.as_tensor (the CUDA array interface)."""
 
@@ -168,8 +164,6 @@ class _PeerState:
             tab = lambda name: i64([b + off[name] for b in bases])
             self.flag_tab, self.S_tab = tab("flags"), tab("S")
             self.F_tab = [tab("F0"), tab("F1")]
-            if _PEER_LOCAL_FACTORS:   # diagnostic (WRONG gradients): every "peer" factor block is this rank's own
-                self.F_tab = [i64([self.base + off[k]] * world) for k in ("F0", "F1")]
             # records: rank j's staging array number `rank` receives what this rank's per-Gaussian pass computes for the
             # blocks j owns; this rank's own arrays 0 .. world-1 receive every rank's records of the blocks IT owns
             self.stage_tab = i64([b + off["STAGE"] + rank * rb for b in bases])
@@ -381,8 +375,6 @@ class ViewParallel:
         seq, par = st.seq, st.seq & 1
         main = torch.cuda.current_stream(dev)
         B, Csig, ev = st.streams(dev)
-        if _PEER_SERIAL:     # diagnostic: everything on the caller's stream (isolated kernel durations)
-            B, Csig = main, None
         F = st.F_local[par]
         F[3 * P:3 * P + 3].copy_(campos.reshape(3))     # the camera position rides behind the factors
         args = list(args)
@@ -397,7 +389,7 @@ class ViewParallel:
         plan = plan_type(stage_hook_type(0), None, nchunks, st.R_ptr, None, st.flag_tab.data_ptr(), world, rank,
                          _SLOT_BLEND, _SLOT_CHUNK0, seq, st.F_tab[par].data_ptr(), st.flags_ptr, self.scale,
                          self.peer_timeout_s, taper, st.stage_tab.data_ptr(),
-                         Csig.cuda_stream if Csig is not None else None, B.cuda_stream, st.rec_tab.data_ptr(),
+                         Csig.cuda_stream, B.cuda_stream, st.rec_tab.data_ptr(),
                          st.S_tab.data_ptr(), st.S_ptr, _SLOT_REDUCED0, emulate)
         # ... and on the side stream, also enqueued by the C call, chunk by chunk underneath the per-Gaussian pass of the
         # later chunks: [wait(CHUNK c, every rank) -> sum the slice this rank owns over the staging arrays (local loads)
@@ -405,8 +397,7 @@ class ViewParallel:
         # the next chunk's reduce: wait(REDUCED c) -> split S into the four gradient arrays (x scale)
         check(lib.sgr_rasterize_backward_staged(*args, C.byref(plan)))
         main.wait_stream(B)
-        if Csig is not None:
-            main.wait_stream(Csig)
+        main.wait_stream(Csig)
         self.stats["backwards"] += 1
 
     def close(self):
