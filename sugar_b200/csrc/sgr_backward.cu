@@ -22,8 +22,11 @@ namespace sgr {
 // Record pipeline of the backward blend: BWD_NS stages of BWD_B records with full / empty mbarriers.  A warp waits
 // only for the loader warps' data, never for its sibling warps, so the tile's eight warps may drift BWD_NS - 2 batches
 // apart and the statistical imbalance between the blocks of one batch is averaged over more records.
-constexpr int BWD_B = 96;   // Gaussians per shared-memory batch (loader threads: the first BWD_B of the CTA)
-constexpr int BWD_NS = 3;   // record stages
+// 64-record batches in four stages (55.6 KB per CTA) rather than 96 in three (57.2 KB): the warps may drift 128
+// records apart instead of 96, so fewer of them wait on a slower sibling's stage release; measured on the headline
+// step (H100 SXM, 400 W): 0.98-0.99 ms against 1.01-1.02 ms, and 1.01 ms for 32 records in eight stages.
+constexpr int BWD_B = 64;   // Gaussians per shared-memory batch (loader threads: the first BWD_B of the CTA)
+constexpr int BWD_NS = 4;   // record stages
 constexpr int BWD_NW = 8;   // warps per CTA (16x16 pixels)
 
 // Blend accumulators (zeroed by a memset before the blend pass):
@@ -44,13 +47,16 @@ __device__ __forceinline__ void red_add_v2(float *addr, float a, float b)
 // blend backward.  One CTA per 16x16 tile, one thread per pixel, one warp per 8x4 pixel block (the
 // forward's geometry); the tile's list is walked back to front over its first max(n_contrib)
 // positions only, a batch of BWD_B records at a time, with the footprint masks deciding which warp
-// visits which splat (sgr_internal.cuh).  Splat records move through a three-stage cp.async (LDGSTS) pipeline
+// visits which splat (sgr_internal.cuh).  Splat records move through a four-stage cp.async (LDGSTS) pipeline
 // with full / empty mbarriers: the copies of batch b+1 are in flight while batch b is processed, and no warp
 // ever waits for a sibling warp, only for data.
 //
 // Reduction.  The 9 per-pair values are NOT reduced across the warp with shuffles.  Phase 1 (lane =
 // pixel) parks S = dL/dG * G and the colour weight alpha*T of every contributing splat in a per-warp
-// [pixel][slot] shared-memory tile; after CH splats the warp turns around (phase 2, lane = slot x half
+// [pixel][slot] shared-memory tile, and lane `slot` keeps the splat's batch slot in a register.  The
+// splat's metadata (centre, conic, opacity, clamp bits, id) is copied out of the record stage by 16 lanes at
+// once, when the chunk is flushed or before the warp releases the stage, not by every lane on every visit.
+// After CH splats the warp turns around (phase 2, lane = slot x half
 // block): each lane walks the 16 pixels of its half, accumulates RAW moments of S about the half's
 // centre -- the pixel offsets are compile-time constants, so a pixel costs 3 FMAs for the moments and 3
 // for the colours -- shifts them to the splat's centre once, combines the two halves with one xor-16
@@ -78,8 +84,11 @@ constexpr int CH = 16;             // splats per chunk
 constexpr int CH_PITCH = CH + 1;   // float2 elements per pixel row: odd pitch = conflict-free transpose
 // per-warp chunk scratch (bytes from its base): pair[32][CH_PITCH] float2 | meta[CH] x 32 B | dp[32] float4
 //   meta: (x, y, conic a, conic b) (conic c, opacity, clamp bits, id) -- what phase 2 needs of a parked splat
+//         (copied from the record stage by stash_meta)
 //   dp:   (dL/dpixel r g b, -T_final <bg, dL/dpixel>) of the block's pixels
-// (57.2 KB per CTA in total with three record stages: four CTAs per SM fit, with 64 registers per thread)
+// (55.6 KB per CTA in total with four record stages of 64: four CTAs per SM fit, with 64 registers per thread; three
+// CTAs with 80 registers measured 1.13 ms against 1.05 ms on the headline step, H100 SXM at 400 W, with the earlier
+// three stages of 96)
 constexpr uint32_t CB_META = 32 * CH_PITCH * 8, CB_DP = CB_META + CH * 32, CB_BYTES = CB_DP + 32 * 16;
 // CTA shared-memory map (dynamic): the record stages, their membership words, the mbarriers, chunk scratch
 constexpr uint32_t SM_A = 0, SM_B = SM_A + BWD_NS * BWD_B * 16, SM_C = SM_B + BWD_NS * BWD_B * 16,
@@ -281,6 +290,20 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
         publish_members(mask, s_member + st * BWD_NW);
         mbar_arrive(&bars[st]);
     };
+    // Chunk slots [0, nfill) hold parked pairs; the metadata of slots [0, nmeta) is already in the chunk's meta rows.
+    // A slot parked from the current stage only records its batch slot (lane `slot`'s pj); its metadata is copied
+    // out of the stage by stash_meta, once per flush and once before the stage is released.
+    int nmeta = 0, pj = 0;
+    auto stash_meta = [&](uint32_t sa, uint32_t sb, uint32_t sc, int to) {
+        if ((int)lane >= nmeta && (int)lane < to) {
+            const float4 A = lds128(sa + pj * 16), B = lds128(sb + pj * 16);
+            const float2 Cm = lds64(sc + pj * 16 + 8);  // (clamp bits, id)
+            const uint32_t ma = cb + CB_META + lane * 32;
+            sts128(ma, A.x, A.y, A.z, A.w);
+            sts128(ma + 16, B.x, B.z, Cm.x, Cm.y);
+        }
+        nmeta = to;
+    };
     if (loader) produce(0);
     for (int b = 0; b < nb; b++) {
         const int b0 = b * BWD_B, buf = b % BWD_NS;
@@ -329,52 +352,49 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
                 if (!__any_sync(0xffffffffu, valid)) continue;
                 // S = dL/dG * G and the colour weight alpha*T of this pair; zero for lanes without one.
                 // (A candidate warp almost always keeps a contributing lane, so there is no second vote:
-                // an all-zero slot is harmless.)
-                float S = 0.f, dchannel = 0.f;
-                if (valid) {
-                    float G = ex2_approx(power * 1.4426950408889634f);
-                    float alpha = fminf(0.99f, B.z * G);
-                    if (fabsf(alpha - 1.0f / 255.0f) < 4.0e-8f) {  // on the threshold: decide as the forward did
-                        G = expf(power);
-                        alpha = fminf(0.99f, __fmul_rn(B.z, G));
-                    }
-                    if (!(alpha < 1.0f / 255.0f)) {
-                        const float2 Cc = lds64(sc + j * 16);
-                        const float4 dp = lds128(cb + CB_DP + lane * 16);
-                        const float om = 1.0f - alpha;  // in [0.01, 1): a bare MUFU.RCP suffices
-                        float inv;
-                        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(om));
-                        T = T * inv;
-                        dchannel = alpha * T;
-                        // acc holds the colour blended behind this splat (backward.cu:493-499 keeps
-                        // last_alpha / last_color and folds them in one iteration later; same
-                        // operations on the same values, evaluated eagerly below)
-                        float dL_dalpha = (B.w - acc0) * dp.x;
-                        dL_dalpha = fmaf(Cc.x - acc1, dp.y, dL_dalpha);
-                        dL_dalpha = fmaf(Cc.y - acc2, dp.z, dL_dalpha);
-                        dL_dalpha *= T;
-                        dL_dalpha = fmaf(dp.w, inv, dL_dalpha);
-                        S = B.z * dL_dalpha * G;
-                        acc0 = fmaf(alpha, B.w, om * acc0);
-                        acc1 = fmaf(alpha, Cc.x, om * acc1);
-                        acc2 = fmaf(alpha, Cc.y, om * acc2);
-                    }
+                // an all-zero slot is harmless.)  Every lane evaluates the pair and only a contributing lane keeps
+                // it: the warp issues these instructions anyway, and without the two divergent branches it saves
+                // their convergence barriers.
+                float G = ex2_approx(power * 1.4426950408889634f);
+                float alpha = fminf(0.99f, B.z * G);
+                if (valid && fabsf(alpha - 1.0f / 255.0f) < 4.0e-8f) {  // on the threshold: decide as the forward did
+                    G = expf(power);
+                    alpha = fminf(0.99f, __fmul_rn(B.z, G));
                 }
-                // park: every lane its pair; the record + id by all lanes alike (same address, same
-                // value: one wavefront, no branch)
+                const bool hit = valid && !(alpha < 1.0f / 255.0f);
+                const float2 Cc = lds64(sc + j * 16);
+                const float4 dp = lds128(cb + CB_DP + lane * 16);
+                const float om = 1.0f - alpha;  // in [0.01, 1) where kept: a bare MUFU.RCP suffices
+                float inv;
+                asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(om));
+                const float Tn = T * inv;
+                // acc holds the colour blended behind this splat (backward.cu:493-499 keeps last_alpha /
+                // last_color and folds them in one iteration later; same operations on the same values,
+                // evaluated eagerly below)
+                float dL_dalpha = (B.w - acc0) * dp.x;
+                dL_dalpha = fmaf(Cc.x - acc1, dp.y, dL_dalpha);
+                dL_dalpha = fmaf(Cc.y - acc2, dp.z, dL_dalpha);
+                dL_dalpha *= Tn;
+                dL_dalpha = fmaf(dp.w, inv, dL_dalpha);
+                const float S = hit ? B.z * dL_dalpha * G : 0.f;
+                const float dchannel = hit ? alpha * Tn : 0.f;
+                if (hit) {
+                    acc0 = fmaf(alpha, B.w, om * acc0);
+                    acc1 = fmaf(alpha, Cc.x, om * acc1);
+                    acc2 = fmaf(alpha, Cc.y, om * acc2);
+                    T = Tn;
+                }
+                // park: every lane its pair, lane `nfill` the batch slot (the metadata follows in stash_meta)
                 sts64(cb + (lane * CH_PITCH + nfill) * 8, S, dchannel);
-                const uint32_t ma = cb + CB_META + nfill * 32;
-                sts128(ma, A.x, A.y, A.z, A.w);
-                {
-                    const float2 Cm = lds64(sc + j * 16 + 8);  // (clamp bits, id)
-                    sts128(ma + 16, B.x, B.z, Cm.x, Cm.y);
-                }
+                if ((int)lane == nfill) pj = j;
                 if (++nfill == CH) {
+                    stash_meta(sa, sb, sc, CH);
                     chunk_flush(cb, CH, blk_x0, blk_y0, 0.5f * W, 0.5f * H, gacc, dcol);
-                    nfill = 0;
+                    nfill = nmeta = 0;
                 }
             }
         }
+        stash_meta(sa, sb, sc, nfill);  // the parked slots' metadata leaves the stage before it is released
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars[BWD_NS + buf]);  // this warp no longer reads the stage
     }
