@@ -936,7 +936,7 @@ __global__ void __launch_bounds__(BK_T) tile_sort_bucket_kernel(const uint32_t *
 // (block w = band * 2 + half, sgr_internal.cuh).  The records of a batch of the tile's list are
 // gathered once into shared memory -- only those whose footprint mask is not empty: a third of the
 // instances are dead in their tile -- and each warp walks only the splats whose mask has its block's
-// bit (ffs over a per-block membership word).  power / alpha / T / C follow the reference's rounding
+// bit (clz over a bit-reversed per-block membership word).  power / alpha / T / C follow the reference's rounding
 // exactly (forward.cu:261-374), so final_T, n_contrib and the image are bit-identical to the
 // reference; the masks and the `power < tau` test only skip pairs the exact alpha test would reject.
 // Tiles are taken heaviest first (tile_order).
@@ -949,10 +949,19 @@ __device__ unsigned long long g_fwd_stats[8];
 #define FWD_STAT(k, v) atomicAdd(&g_fwd_stats[k], (unsigned long long)(v))
 #endif
 
-// The minimum of one resident CTA per SM is not redundant: without it nvcc allocates fewer registers (40 instead of 51
-// for the unpacked list format) and generates different code.
+// (1 << n) - 1 for n = 0..31 in one instruction (BMSK); nvcc makes a shift of a materialised -1 and a LOP3 of it
+__device__ __forceinline__ uint32_t low_mask(uint32_t n)
+{
+    uint32_t r;
+    asm("bmsk.clamp.b32 %0, 0, %1;" : "=r"(r) : "r"(n));
+    return r;
+}
+
+// No minimum CTA count in the launch bounds: with a minimum of 1 nvcc gives the packed format 38 registers (6 CTAs per
+// SM) instead of 32 (8 CTAs), and the unpacked one 53 instead of 48.  The extra CTAs outweigh the one instruction per
+// visit the 32-register code spends (DESIGN.md §3).
 template <bool packed>
-__global__ void __launch_bounds__(BLEND_T, 1) blend_forward_kernel(const uint32_t *__restrict__ tile_order,
+__global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *__restrict__ tile_order,
                                                                 const uint32_t *__restrict__ tile_start,
                                                                 const uint32_t *__restrict__ plist,
                                                                 const float4 *__restrict__ rec,
@@ -962,9 +971,12 @@ __global__ void __launch_bounds__(BLEND_T, 1) blend_forward_kernel(const uint32_
                                                                 uint32_t *__restrict__ n_contrib,
                                                                 float *__restrict__ out_color)
 {
-    __shared__ float4 s_a[BLEND_T];  // x, y, conic a, conic b
-    __shared__ float4 s_b[BLEND_T];  // conic c, tau, opacity, r
-    __shared__ float2 s_c[BLEND_T];  // g, b
+    // A batch slot is 48 contiguous bytes: (x, y, conic a, conic b), (conic c, tau, opacity, r), (g, b, -): one IMAD
+    // gives the slot's address and the loads take immediate offsets.  Every lane of a warp reads the same slot, so
+    // the loads are broadcasts and the 48-byte stride costs no bank conflicts.
+    __shared__ __align__(16) float4 s_rec[BLEND_T * 3];
+    // s_member[w][k]: slots 32k..32k+31 whose footprint mask has block w, bit-reversed (slot 32k + i is bit 31 - i)
+    // so that the walk finds the next member with one clz
     __shared__ uint32_t s_member[8][BLEND_T / 32];
     if ((uint64_t)counters[0] > capacity) return;
     const int tile = (int)tile_order[blockIdx.x];
@@ -979,7 +991,8 @@ __global__ void __launch_bounds__(BLEND_T, 1) blend_forward_kernel(const uint32_
     uint32_t done = inside ? 0u : 1u;  // 32-bit flag: a bool makes nvcc shuffle bytes (PRMT) in the hot loop
     float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f;
     uint32_t last = 0;
-    const uint32_t sa = smem_addr_pinned(s_a), sb = smem_addr_pinned(s_b), sc = smem_addr_pinned(s_c);
+    const uint32_t srec = smem_addr_pinned(s_rec);
+    const uint32_t smem_put = smem_addr_pinned(&s_member[0][wid]), smem_get = smem_addr_pinned(&s_member[wid][0]);
     for (uint32_t b0 = lo; b0 < hi; b0 += BLEND_T) {
         if (__syncthreads_count(done != 0u) == BLEND_T) break;
         uint32_t mask = 0;
@@ -994,15 +1007,16 @@ __global__ void __launch_bounds__(BLEND_T, 1) blend_forward_kernel(const uint32_
                 const float4 *r = rec + (size_t)id * 3;
                 const float4 r0 = __ldg(r), r1 = __ldg(r + 1), r2 = __ldg(r + 2);
                 if (!packed) mask = block_mask_of_record(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, tx0, ty0);
-                s_a[tid] = r0;
-                s_b[tid] = r1;
-                s_c[tid] = make_float2(r2.x, r2.y);
+                const uint32_t p = srec + (uint32_t)tid * 48u;
+                sts128(p, r0.x, r0.y, r0.z, r0.w);
+                sts128(p + 16, r1.x, r1.y, r1.z, r1.w);
+                sts64(p + 32, r2.x, r2.y);
             }
         }
 #pragma unroll
         for (int blk = 0; blk < 8; blk++) {
-            const uint32_t word = __ballot_sync(0xffffffffu, (mask >> blk) & 1u);
-            if (lane == 0) s_member[blk][wid] = word;
+            const uint32_t word = __ballot_sync(0xffffffffu, mask & (1u << blk));
+            if (lane == 0) sts32(smem_put + blk * (BLEND_T / 32) * 4, __brev(word));
         }
         __syncthreads();
         const uint32_t base_pos = b0 - lo;
@@ -1012,15 +1026,21 @@ __global__ void __launch_bounds__(BLEND_T, 1) blend_forward_kernel(const uint32_
         if (!__all_sync(0xffffffffu, done != 0u)) {
 #pragma unroll 1
             for (int k = 0; k < BLEND_T / 32; k++) {
-                uint32_t mw = s_member[wid][k];
+                // every lane reads the same word: the OR over the warp is that word, but in a uniform register, so
+                // ptxas knows the walk's branches are warp-uniform (no WARPSYNC in front of the votes) and runs the
+                // walk's integer work on the uniform datapath
+                uint32_t mw = __reduce_or_sync(0xffffffffu, lds32(smem_get + k * 4));
+                const uint32_t wrec = srec + (uint32_t)k * (32u * 48u) + 31u * 48u;  // slot 32k + 31
+                const uint32_t wlast = base_pos + (uint32_t)(k << 5) + 32u;       // n_contrib of slot 32k + 31
 #pragma unroll 1
                 while (mw) {
-                    const int j = (k << 5) + __ffs(mw) - 1;
-                    mw &= mw - 1;
+                    const uint32_t msb = 31 - __clz(mw);  // slot 32k + 31 - msb: the word's first member
+                    mw &= low_mask(msb);
+                    const uint32_t p = wrec - msb * 48u;
 #ifdef SGR_BLEND_STATS
                     {
-                        const float4 A = lds128(sa + j * 16);
-                        const float4 B = lds128(sb + j * 16);
+                        const float4 A = lds128(p);
+                        const float4 B = lds128(p + 16);
                         const float power = splat_power(__fsub_rn(A.x, pxf), __fsub_rn(A.y, pyf), A.z, A.w, B.x);
                         const bool cand = !done && !(power > 0.0f || power < B.y);
                         const bool hit = cand && !(fminf(0.99f, __fmul_rn(B.z, expf(power))) < 1.0f / 255.0f);
@@ -1036,25 +1056,28 @@ __global__ void __launch_bounds__(BLEND_T, 1) blend_forward_kernel(const uint32_
                         }
                     }
 #endif
-                    if (done) continue;
-                    const float4 A = lds128(sa + j * 16);
-                    const float4 B = lds128(sb + j * 16);
+                    const float4 A = lds128(p);
+                    const float4 B = lds128(p + 16);
                     const float dx = __fsub_rn(A.x, pxf), dy = __fsub_rn(A.y, pyf);
                     const float power = splat_power(dx, dy, A.z, A.w, B.x);
-                    if (power > 0.0f || power < B.y) continue;
+                    const bool cand = (done == 0u) & !(power > 0.0f || power < B.y);
+                    if (!__any_sync(0xffffffffu, cand)) continue;
+                    // Every lane of a warp with a candidate evaluates the tail; selects (not products with 0) keep
+                    // what a lane that does not contribute had, signed zeros and NaNs included.
+                    const float2 Cc = lds64(p + 32);
                     const float alpha = fminf(0.99f, __fmul_rn(B.z, expf(power)));
-                    if (alpha < 1.0f / 255.0f) continue;
                     const float test_T = __fmul_rn(T, __fsub_rn(1.0f, alpha));
-                    if (test_T < 0.0001f) {
-                        done = 1u;
-                        continue;
-                    }
-                    const float2 Cc = lds64(sc + j * 8);
-                    C0 = __fmaf_rn(T, __fmul_rn(alpha, B.w), C0);
-                    C1 = __fmaf_rn(T, __fmul_rn(alpha, Cc.x), C1);
-                    C2 = __fmaf_rn(T, __fmul_rn(alpha, Cc.y), C2);
-                    T = test_T;
-                    last = base_pos + (uint32_t)j + 1u;
+                    const bool hit = cand && !(alpha < 1.0f / 255.0f);
+                    const bool contrib = hit && !(test_T < 0.0001f);
+                    done = (hit && test_T < 0.0001f) ? 1u : done;
+                    const float n0 = __fmaf_rn(T, __fmul_rn(alpha, B.w), C0);
+                    const float n1 = __fmaf_rn(T, __fmul_rn(alpha, Cc.x), C1);
+                    const float n2 = __fmaf_rn(T, __fmul_rn(alpha, Cc.y), C2);
+                    C0 = contrib ? n0 : C0;
+                    C1 = contrib ? n1 : C1;
+                    C2 = contrib ? n2 : C2;
+                    T = contrib ? test_T : T;
+                    last = contrib ? wlast - msb : last;
                 }
                 if (__all_sync(0xffffffffu, done != 0u)) break;
             }
