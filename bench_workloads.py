@@ -34,6 +34,7 @@ def reference_ops(torch, ref_mod):
     """The reference's building blocks behind the `ops` interface of sugar_b200/steps.py."""
     from oracle import field_oracle as fo
     from oracle import meshbind_oracle as mo
+    from oracle import ssim_oracle as so
 
     def bind(verts, faces, bary, scales_raw, complex_raw, thickness):
         p, s, q = mo.bind_to_mesh_torch(verts, faces, bary, scales_raw, complex_raw, thickness)
@@ -43,7 +44,7 @@ def reference_ops(torch, ref_mod):
         colors=lambda points, sh, campos, deg: fo.points_rgb_torch(points, sh, campos, deg + 1),
         field_values=lambda x, nbr, points, scaling, quats, strengths, density_factor=1.0, density_threshold=1.0, **_:
             fo.field_values_torch(x, nbr, points, scaling, quats, strengths, density_factor, density_threshold),
-        better_normal_loss=fo.better_normal_loss_torch, bind_to_mesh=bind)
+        better_normal_loss=fo.better_normal_loss_torch, bind_to_mesh=bind, l1_dssim=so.l1_dssim_torch)
 
 
 def run(args, scenes, load_peaks, ClockSampler, cpu_density_baseline):

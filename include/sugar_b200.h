@@ -381,6 +381,30 @@ SGR_API size_t sgr_knn_workspace_bytes(int32_t P);
 SGR_API int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int32_t K, int64_t *idx,
                     float *dist2, void *workspace, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Photometric loss of the trainers, (1 - f) * l1_loss + f * (1 - ssim) (sugar_utils/loss_utils.py:17-62, used as
+ * sugar_trainers/coarse_sdf.py:101-103, 452-457): per image b of img1, img2 f32[B,C,H,W] (contiguous planes), the
+ * mean over its C*H*W elements of |x - y| and of the SSIM map
+ *   S = (2 mu1 mu2 + c1)(2 sigma12 + c2) / ((mu1^2 + mu2^2 + c1)(sigma1^2 + sigma2^2 + c2))
+ * whose moments are 11x11 windowed sums with zero padding of 5, each (b, c) plane on its own.  The window is
+ * window[i] * window[j] (passed by value: the caller builds the 1-D weights by its recipe).
+ *   partial_maps  f32[3, B*C*H*W]  the op's saved state: dS/dmu1 (sigma1^2, sigma12 expanded), dS/dE[x^2], dS/dE[xy]
+ *   per_image_out f32[B, 2]        (l1 mean, ssim mean) per image, summed in a fixed order (run-to-run identical)
+ *   scratch       sgr_l1_ssim_scratch_bytes(B, C, H, W) bytes of device memory
+ * Backward: g_l1, g_ssim f32[B] (DEVICE: the upstream gradients of the two outputs) -> grad_img1 f32[B,C,H,W], fully
+ * written; only img1 is differentiated (sign(0) = 0 for the L1 term).  Limits: B*C*H*W <= 2^31 - 1, B*C <= 65535.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct SgrSsimParams {
+    int32_t B, C, H, W;
+    float c1, c2;      /* 0.01^2, 0.03^2 in the reference */
+    float window[11];  /* normalised 1-D weights */
+} SgrSsimParams;
+SGR_API size_t sgr_l1_ssim_scratch_bytes(int32_t B, int32_t C, int32_t H, int32_t W);
+SGR_API int sgr_l1_ssim_forward(const SgrSsimParams *p, const float *img1, const float *img2, float *partial_maps,
+                                float *per_image_out, void *scratch, void *stream);
+SGR_API int sgr_l1_ssim_backward(const SgrSsimParams *p, const float *img1, const float *img2, const float *partial_maps,
+                                 const float *g_l1, const float *g_ssim, float *grad_img1, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */
@@ -391,8 +415,8 @@ SGR_API int sgr_profile_enable(int on);
 SGR_API int sgr_profile_read(float *total_ms, int *counts);
 SGR_API int sgr_profile_timeline(int max_records, int *kinds, float *t_begin_ms, float *t_end_ms);
 
-/* sizeof of an ABI struct as the library was compiled (0 SgrView, 1 SgrGaussians, 2 SgrBackwardPlan, 3 SgrFieldParams;
- * else 0): lets a foreign-language binding check its own struct layout. */
+/* sizeof of an ABI struct as the library was compiled (0 SgrView, 1 SgrGaussians, 2 SgrBackwardPlan, 3 SgrFieldParams,
+ * 4 SgrSsimParams; else 0): lets a foreign-language binding check its own struct layout. */
 SGR_API size_t sgr_struct_bytes(int32_t which);
 SGR_API const char *sgr_last_error(void);
 SGR_API const char *sgr_version(void);

@@ -39,6 +39,11 @@ class SgrFieldParams(C.Structure):
                 ("density_threshold", C.c_float), ("opacity_min_clamp", C.c_float), ("samples_per_idx_row", C.c_int32)]
 
 
+class SgrSsimParams(C.Structure):
+    _fields_ = [("B", C.c_int32), ("C", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("c1", C.c_float),
+                ("c2", C.c_float), ("window", C.c_float * 11)]
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 STAGE_HOOK = C.CFUNCTYPE(None, C.c_void_p, C.c_int32)
 
@@ -99,6 +104,9 @@ PROTOTYPES = {
     "sgr_knn_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_knn": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                           C.c_void_p]),
+    "sgr_l1_ssim_scratch_bytes": (C.c_size_t, [C.c_int32] * 4),
+    "sgr_l1_ssim_forward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 6),
+    "sgr_l1_ssim_backward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 7),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),
@@ -125,7 +133,7 @@ def _load():
 
 
 lib = _load()
-for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams)):
+for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams, SgrSsimParams)):
     if lib.sgr_struct_bytes(_i) != C.sizeof(_t):   # a stale library or a binding edited without the header
         raise SgrError(f"{LIB_PATH}: struct {_t.__name__} is {lib.sgr_struct_bytes(_i)} bytes in the library, "
                        f"{C.sizeof(_t)} in this binding -- rebuild with `python sugar_b200/build.py`")

@@ -39,7 +39,7 @@ int device_sm_count()
 static const char *const g_kind_names[K_NUM_KINDS] = {
     "preprocess", "tile_scan", "scatter", "tile_sort_smem", "tile_sort_global", "blend_forward", "blend_backward",
     "preprocess_backward", "field_pack", "field_forward", "field_backward", "field_unpack", "knn_build", "knn_query",
-    "misc", "view_finalize", "peer_reduce", "peer_sync"};
+    "misc", "view_finalize", "peer_reduce", "peer_sync", "loss_forward", "loss_backward"};
 struct ProfRec {
     cudaEvent_t a, b;
     int kind;
@@ -221,6 +221,7 @@ size_t sgr_struct_bytes(int32_t which)
         case 1: return sizeof(SgrGaussians);
         case 2: return sizeof(SgrBackwardPlan);
         case 3: return sizeof(SgrFieldParams);
+        case 4: return sizeof(SgrSsimParams);
         default: return 0;
     }
 }

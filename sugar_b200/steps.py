@@ -23,9 +23,11 @@ fused kernels and over the reference's own building blocks (its CUDA rasterizer 
     ops.colors(points, sh, campos, sh_deg) -> colors_precomp or None (None: pass `shs` to the rasterizer)
     ops.field_values(x, nbr_idx, points, scaling, quaternions, strengths, **kw) -> dict
     ops.better_normal_loss(x, idx, nbr_idx, points, scaling, quaternions, nbr_opacity) -> [N]
+    ops.l1_dssim(pred, gt, dssim_factor) -> scalar   (only called with dssim_factor > 0)
 
-What is NOT reproduced: the photometric loss is plain L1 (the reference adds 0.2 x DSSIM, a 11x11 convolution outside
-the path), and the camera is this package's pinhole convention (scenes.py) rather than pytorch3d's.
+The photometric term is plain L1 by default (dssim_factor=0.0, what bench.py times); dssim_factor=0.2 gives the
+trainers' (1 - 0.2) L1 + 0.2 (1 - SSIM) (coarse_sdf.py:101-103, 452-457, refine.py:103-105, 499-504).  What is NOT
+reproduced: the camera is this package's pinhole convention (scenes.py) rather than pytorch3d's.
 """
 import math
 from types import SimpleNamespace
@@ -83,10 +85,17 @@ def render(ops, a, cam, bg, sh_deg, point_colors=None):
     return image, radii, means2D
 
 
+def photometric_loss(ops, image, gt_rgb, dssim_factor):
+    """Plain L1 when dssim_factor == 0, else the trainers' (1 - f) L1 + f (1 - SSIM) through ops.l1_dssim."""
+    if dssim_factor == 0.0:
+        return (image - gt_rgb).abs().mean()
+    return ops.l1_dssim(image, gt_rgb, dssim_factor)
+
+
 def coarse_sdf_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, density_factor=1.0 / 16.0,
                     density_threshold=1.0, sdf_estimation_factor=0.2, sdf_better_normal_factor=0.2,
                     close_gaussian_threshold=2.0, sampling_scale_factor=1.5, spatial_extent=10.0, znear=0.01,
-                    generator=None, backward=True):
+                    generator=None, backward=True, dssim_factor=0.0):
     """One regularised coarse-training iteration.  `raw`: dict of the model's raw parameter tensors (points,
     sh_dc [P,1,3], sh_rest [P,15,3], densities [P,1], scales [P,3], quaternions [P,4]); `cam`: namespace with
     viewmatrix / projmatrix / campos device tensors and width, height, tanfovx, tanfovy; `knn_idx` [P,16]."""
@@ -95,7 +104,7 @@ def coarse_sdf_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, density
     dev = a.points.device
     # 1. RGB
     image, radii, viewspace = render(ops, a, cam, torch.zeros(3, device=dev), sh_deg=3)
-    loss = (image - gt_rgb).abs().mean()
+    loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
     vis = radii > 0
     # 2. depth, with gradient
     point_depth = world_to_view(a.points, cam.viewmatrix)[:, 2:].expand(-1, 3)
@@ -135,7 +144,7 @@ def coarse_sdf_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, density
     return loss.detach(), stats
 
 
-def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True):
+def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0):
     """One refinement iteration's render for mesh-bound Gaussians (sugar_trainers/refine.py; model properties
     sugar_model.py:384-398 points, :415-441 scaling, :443-479 quaternions).  `raw`: verts [V,3], sh_dc, sh_rest,
     densities [P,1], scales [P,2] (in-plane), quaternions [P,2] (the learned 2-D rotation as a complex number);
@@ -145,7 +154,7 @@ def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True):
                         strengths=torch.sigmoid(raw["densities"]).view(-1, 1),
                         sh=torch.cat([raw["sh_dc"], raw["sh_rest"]], dim=1))
     image, radii, _ = render(ops, b, cam, torch.zeros(3, device=b.points.device), sh_deg=3)
-    loss = (image - gt_rgb).abs().mean()
+    loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
     if backward:
         loss.backward()
     return loss.detach(), {"visible": int((radii > 0).sum())}
@@ -159,9 +168,10 @@ def camera_from_scene(sc, device):
 
 
 def ours_ops():
-    """This package's operators: in-kernel SH colours, fused field / normal-loss kernels, fused mesh binding."""
+    """This package's operators: in-kernel SH colours, fused field / normal-loss kernels, fused mesh binding, fused
+    L1 + D-SSIM loss."""
     from . import diff_gaussian_rasterization as dgr
-    from . import field, meshbind
+    from . import field, loss, meshbind
     return SimpleNamespace(rasterizer=dgr, colors=lambda points, sh, campos, deg: None,
                            field_values=field.field_values, better_normal_loss=field.better_normal_loss,
-                           bind_to_mesh=meshbind.bind_to_mesh)
+                           bind_to_mesh=meshbind.bind_to_mesh, l1_dssim=loss.l1_dssim_loss)
