@@ -405,6 +405,29 @@ SGR_API int sgr_l1_ssim_forward(const SgrSsimParams *p, const float *img1, const
 SGR_API int sgr_l1_ssim_backward(const SgrSsimParams *p, const float *img1, const float *img2, const float *partial_maps,
                                  const float *g_l1, const float *g_ssim, float *grad_img1, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Mesh normal consistency of the refinement stage (sugar_trainers/refine.py:775-783: pytorch3d 0.7.4
+ * mesh_normal_consistency of the one surface mesh): the mean over the Q pairs of faces that share an edge of
+ *   1 - cosine_similarity(n_a, -n_b, eps = 1e-8),  n_x = (verts[v1] - verts[v0]) x (verts[x] - verts[v0])
+ * over a pair table built once per topology (sugar_b200/meshloss.py: mesh_topology):
+ *   verts    f32[V,3]
+ *   pairs    i32[Q,4]   rows (v0, v1, a, b): the shared edge (v0 < v1) and the two faces' opposite vertices
+ *   vert_ptr i32[V+1], vert_inc i32[4Q]   for each vertex, the entries 4 q + slot of `pairs` that name it, in
+ *                                          ascending order (CSR)
+ *   loss     f32[1]     the mean; summed in a fixed order (run-to-run identical); Q = 0 gives 0 (a memset only)
+ * The per-pair arithmetic is in double; where both normals are longer than eps the term is evaluated as
+ * |n_a/|n_a| + n_b/|n_b||^2 / 2, which keeps its digits at small angles.
+ * Backward: g_loss f32[1] (DEVICE: the upstream gradient) -> g_verts f32[V,3], fully written, each vertex summed
+ * over its CSR list in order (run-to-run identical).  Limits: 0 <= Q <= (2^31 - 1) / 4.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API size_t sgr_mesh_nc_forward_scratch_bytes(int32_t Q);
+SGR_API size_t sgr_mesh_nc_backward_scratch_bytes(int32_t Q);
+SGR_API int sgr_mesh_nc_forward(int32_t Q, int32_t V, const float *verts, const int32_t *pairs, float *loss,
+                                void *scratch, void *stream);
+SGR_API int sgr_mesh_nc_backward(int32_t Q, int32_t V, const float *verts, const int32_t *pairs,
+                                 const int32_t *vert_ptr, const int32_t *vert_inc, const float *g_loss, float *g_verts,
+                                 void *scratch, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */

@@ -107,6 +107,10 @@ PROTOTYPES = {
     "sgr_l1_ssim_scratch_bytes": (C.c_size_t, [C.c_int32] * 4),
     "sgr_l1_ssim_forward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 6),
     "sgr_l1_ssim_backward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 7),
+    "sgr_mesh_nc_forward_scratch_bytes": (C.c_size_t, [C.c_int32]),
+    "sgr_mesh_nc_backward_scratch_bytes": (C.c_size_t, [C.c_int32]),
+    "sgr_mesh_nc_forward": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 5),
+    "sgr_mesh_nc_backward": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 8),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),

@@ -117,6 +117,54 @@ def with_camera_offset(sc: Scene, yaw: float, shift) -> Scene:
     return sc._replace(viewmatrix=V2.T.astype(np.float32), projmatrix=(V2.T @ Pm.T).astype(np.float32), campos=campos)
 
 
+def height_field_mesh(nx: int, ny: int, seed: int = 0, amplitude: float = 0.05, noise: float = 0.01,
+                      permute: bool = False):
+    """Connected triangle mesh of a noisy height field over the unit square: an nx x ny vertex grid, two triangles
+    per cell (F = 2 (nx - 1)(ny - 1)), z = amplitude * (a few smooth waves) + noise * grid spacing * N(0, 1), so
+    that adjacent faces are a few hundredths of a radian apart, as on the smooth meshes refinement binds to.
+    `permute` shuffles the vertex ids and the face order (seeded), for the scattered access of a decimated Poisson
+    mesh.  -> (verts float32 [V,3], faces int64 [F,3])."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    x, y = np.meshgrid(np.linspace(0.0, 1.0, nx), np.linspace(0.0, 1.0, ny), indexing="xy")
+    h = 1.0 / max(nx - 1, ny - 1, 1)
+    z = amplitude * (np.sin(2 * math.pi * (1.5 * x + 0.3)) * np.cos(2 * math.pi * (1.0 * y - 0.2)) + 0.5 * x * y)
+    z = z + noise * h * rng.normal(size=z.shape)
+    verts = np.stack([x.ravel(), y.ravel(), z.ravel()], 1)
+    i, j = np.meshgrid(np.arange(nx - 1), np.arange(ny - 1), indexing="xy")
+    v00 = (j * nx + i).ravel()
+    v10, v01, v11 = v00 + 1, v00 + nx, v00 + nx + 1
+    faces = np.stack([np.stack([v00, v10, v11], 1), np.stack([v00, v11, v01], 1)], 1).reshape(-1, 3)
+    if permute:
+        perm = rng.permutation(len(verts))            # new id of old vertex k is inv[k]
+        inv = np.empty_like(perm)
+        inv[perm] = np.arange(len(perm))
+        verts = verts[perm]
+        faces = inv[faces][rng.permutation(len(faces))]
+    return np.ascontiguousarray(verts, np.float32), np.ascontiguousarray(faces, np.int64)
+
+
+def icosphere(subdivisions: int, radius: float = 1.0):
+    """Closed subdivided icosahedron (every edge shared by exactly two faces): V = 10 * 4^s + 2, F = 20 * 4^s,
+    outward winding.  -> (verts float32 [V,3], faces int64 [F,3])."""
+    t = (1.0 + math.sqrt(5.0)) / 2.0
+    verts = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
+                      [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], np.float64)
+    faces = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
+                      [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5],
+                      [2, 4, 11], [6, 2, 10], [8, 6, 7], [9, 8, 1]], np.int64)
+    verts /= np.linalg.norm(verts, axis=1, keepdims=True)
+    for _ in range(subdivisions):
+        edges = np.sort(np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]]), axis=1)
+        uniq, inv = np.unique(edges, axis=0, return_inverse=True)
+        mid = verts[uniq[:, 0]] + verts[uniq[:, 1]]
+        verts = np.concatenate([verts, mid / np.linalg.norm(mid, axis=1, keepdims=True)])
+        m = len(verts) - len(uniq) + inv.reshape(3, -1).T   # midpoints of (v0 v1), (v1 v2), (v2 v0)
+        a, b, c = faces.T
+        faces = np.concatenate([np.stack([a, m[:, 0], m[:, 2]], 1), np.stack([b, m[:, 1], m[:, 0]], 1),
+                                np.stack([c, m[:, 2], m[:, 1]], 1), m])
+    return np.ascontiguousarray(verts * radius, np.float32), np.ascontiguousarray(faces, np.int64)
+
+
 def upstream_grad(width: int, height: int, seed: int = 1) -> np.ndarray:
     """Fixed dL/dimage: loss = (image * Wt).sum(), Wt ~ N(0,1)/(3HW)."""
     rng = np.random.Generator(np.random.PCG64(seed))

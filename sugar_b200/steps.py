@@ -24,6 +24,7 @@ fused kernels and over the reference's own building blocks (its CUDA rasterizer 
     ops.field_values(x, nbr_idx, points, scaling, quaternions, strengths, **kw) -> dict
     ops.better_normal_loss(x, idx, nbr_idx, points, scaling, quaternions, nbr_opacity) -> [N]
     ops.l1_dssim(pred, gt, dssim_factor) -> scalar   (only called with dssim_factor > 0)
+    ops.mesh_normal_consistency(verts, faces, topology) -> scalar   (only called with normal_consistency_factor > 0)
 
 The photometric term is plain L1 by default (dssim_factor=0.0, what bench.py times); dssim_factor=0.2 gives the
 trainers' (1 - 0.2) L1 + 0.2 (1 - SSIM) (coarse_sdf.py:101-103, 452-457, refine.py:103-105, 499-504).  What is NOT
@@ -144,17 +145,22 @@ def coarse_sdf_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, density
     return loss.detach(), stats
 
 
-def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0):
+def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0, normal_consistency_factor=0.0):
     """One refinement iteration's render for mesh-bound Gaussians (sugar_trainers/refine.py; model properties
     sugar_model.py:384-398 points, :415-441 scaling, :443-479 quaternions).  `raw`: verts [V,3], sh_dc, sh_rest,
     densities [P,1], scales [P,2] (in-plane), quaternions [P,2] (the learned 2-D rotation as a complex number);
-    `mesh`: faces [F,3] int64, bary [n,3,1], thickness; P = F * n."""
+    `mesh`: faces [F,3] int64, bary [n,3,1], thickness, optionally `topology` (meshloss.mesh_topology of the faces,
+    built once); P = F * n.  normal_consistency_factor > 0 adds the surface mesh's normal consistency
+    (refine.py:775-783, 0.1 in the trainers) through ops.mesh_normal_consistency."""
     a = ops.bind_to_mesh(raw["verts"], mesh.faces, mesh.bary, raw["scales"], raw["quaternions"], mesh.thickness)
     b = SimpleNamespace(points=a.points, scaling=a.scaling, quaternions=a.quaternions,
                         strengths=torch.sigmoid(raw["densities"]).view(-1, 1),
                         sh=torch.cat([raw["sh_dc"], raw["sh_rest"]], dim=1))
     image, radii, _ = render(ops, b, cam, torch.zeros(3, device=b.points.device), sh_deg=3)
     loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
+    if normal_consistency_factor > 0.0:
+        loss = loss + normal_consistency_factor * ops.mesh_normal_consistency(raw["verts"], mesh.faces,
+                                                                              getattr(mesh, "topology", None))
     if backward:
         loss.backward()
     return loss.detach(), {"visible": int((radii > 0).sum())}
@@ -169,9 +175,10 @@ def camera_from_scene(sc, device):
 
 def ours_ops():
     """This package's operators: in-kernel SH colours, fused field / normal-loss kernels, fused mesh binding, fused
-    L1 + D-SSIM loss."""
+    L1 + D-SSIM loss, fused mesh normal consistency."""
     from . import diff_gaussian_rasterization as dgr
-    from . import field, loss, meshbind
+    from . import field, loss, meshbind, meshloss
     return SimpleNamespace(rasterizer=dgr, colors=lambda points, sh, campos, deg: None,
                            field_values=field.field_values, better_normal_loss=field.better_normal_loss,
-                           bind_to_mesh=meshbind.bind_to_mesh, l1_dssim=loss.l1_dssim_loss)
+                           bind_to_mesh=meshbind.bind_to_mesh, l1_dssim=loss.l1_dssim_loss,
+                           mesh_normal_consistency=meshloss.mesh_normal_consistency)
