@@ -7,7 +7,6 @@ guard; all arithmetic happens in the hand-written sm_90a kernels.
 """
 import contextlib
 import ctypes as C
-import os
 import threading
 from typing import Tuple
 
@@ -15,8 +14,6 @@ import torch
 
 from . import _lib
 from ._lib import SgrGaussians, SgrView, check, lib
-
-_USE_HINT = os.environ.get("SGR_NO_CAPACITY_HINT", "0") != "1"
 
 
 class Context:
@@ -76,41 +73,6 @@ def _ptr(t: torch.Tensor, name: str):
 
 _ROUND = 64 << 20  # arena sizes are rounded up to 64 MiB so the caching allocator sees few distinct sizes
 
-# Optional workspace cache (SGR_WORKSPACE_CACHE=1).  The per-call buffers of this op are large
-# (0.5-1 GB at 3M Gaussians); a cudaMalloc inside the training loop is a 10-160 ms device-wide
-# stall.  By default torch's caching allocator is enough: each call makes one rounded allocation
-# for the forward state and one for the gradients, and `_Arena.release()` breaks the callback
-# reference cycle so they are returned by reference counting, not at the next cyclic GC (which is
-# what used to fragment the allocator; scripts/step_times.py shows the difference).  With the
-# cache on, blocks are additionally pinned here and handed out again as soon as nothing references
-# their storage (stream-ordered reuse, like the caching allocator's).
-_ws_cache = {}
-_WS_MAX_PER_KEY = 6
-_USE_WS_CACHE = os.environ.get("SGR_WORKSPACE_CACHE", "0") == "1"
-
-
-def _use_count(t: torch.Tensor) -> int:
-    return torch._C._storage_Use_Count(t.untyped_storage()._cdata)
-
-
-def _big_empty(numel: int, dtype, device) -> torch.Tensor:
-    """1-D tensor of `numel` elements for a per-call arena, recycled once all its views are dead."""
-    if not _USE_WS_CACHE:
-        return torch.empty(numel, dtype=dtype, device=device)
-    key = (device.index, torch.cuda.current_stream(device).cuda_stream, dtype, numel)
-    entries = _ws_cache.setdefault(key, [])
-    for blk, baseline in entries:
-        if _use_count(blk) == baseline:
-            return blk
-    blk = torch.empty(numel, dtype=dtype, device=device)
-    if len(entries) < _WS_MAX_PER_KEY:
-        entries.append((blk, _use_count(blk)))
-    return blk
-
-
-def clear_workspace_cache() -> None:
-    _ws_cache.clear()
-
 
 def _round_up(n: int, a: int) -> int:
     return (n + a - 1) // a * a
@@ -123,7 +85,8 @@ class _Arena:
 
     def __init__(self, device, reserve_bytes: int):
         self.device = device
-        self.block = _big_empty(_round_up(reserve_bytes, _ROUND), torch.uint8, device) if reserve_bytes else None
+        self.block = (torch.empty(_round_up(reserve_bytes, _ROUND), dtype=torch.uint8, device=device)
+                      if reserve_bytes else None)
         self.used = 0
         self.parts = {}
         self.error = None   # an exception raised inside a callback (e.g. torch OOM): re-raised after the C call returns
@@ -137,7 +100,7 @@ class _Arena:
                 t = self.block[off:off + nbytes]
                 self.used = off + nbytes
             else:  # no (or too small a) reservation: plain allocation, still rounded
-                t = _big_empty(_round_up(nbytes, _ROUND), torch.uint8, self.device)[:nbytes]
+                t = torch.empty(_round_up(nbytes, _ROUND), dtype=torch.uint8, device=self.device)[:nbytes]
             self.parts[name] = t
             return t.data_ptr()
         except BaseException as e:  # never unwind through the C frame: NULL makes the library stop with an error status
@@ -149,7 +112,9 @@ class _Arena:
 
     def release(self):
         """Break the arena <-> callback reference cycle so the block is released by reference
-        counting as soon as the autograd graph lets go of the views (not at the next cyclic GC)."""
+        counting as soon as the autograd graph lets go of the views (not at the next cyclic GC).
+        Blocks left to the cyclic GC come back in bursts, and the caching allocator then splits them and
+        calls cudaMalloc inside the training loop, a device-wide stall (scripts/step_times.py)."""
         self.cbs = None
         self.block = None
         self.parts = {}
@@ -214,7 +179,7 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         out_color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
         radii = torch.empty((P,), dtype=torch.int32, device=dev)
         key = (dev.index, H, W)
-        hint = context.capacity_hint.get(key, 0) if _USE_HINT else 0
+        hint = context.capacity_hint.get(key, 0)
         reserve = lib.sgr_geometry_bytes(P) + lib.sgr_image_bytes(W, H) + 1024
         if hint:
             reserve += lib.sgr_binning_bytes(hint)
@@ -264,7 +229,7 @@ def _alloc_backward(P: int, M: int, dev, with_records: bool, split_sh: bool = Fa
         # so that one all-gather carries a view's SH factors and its camera
         o = _round_up(o + P * w + (4 if name == "colors" else 0), _PART_ALIGN)
     total = o + n_scratch + 64
-    flat = _big_empty(_round_up(4 * total, _ROUND) // 4, torch.float32, dev)
+    flat = torch.empty(_round_up(4 * total, _ROUND) // 4, dtype=torch.float32, device=dev)
     skew = (-(flat.data_ptr() // 4)) % _PART_ALIGN  # the allocator aligns to 512 B; be explicit anyway
     shapes = {"means3D": (P, 3), "opacity": (P, 1), "scales": (P, 3), "rotations": (P, 4),
               "sh": (P, 1 if split_sh else M, 3), "sh_rest": (P, max(M - 1, 0), 3), "means2D": (P, 3), "colors": (P, 3),

@@ -78,15 +78,6 @@ void prof_end(cudaStream_t st)
     g_prof_n++;
 }
 
-bool ids_packed(int P)
-{
-    static const bool force_unpacked = [] {
-        const char *e = getenv("SGR_FORCE_UNPACKED_IDS");
-        return e && e[0] == '1';
-    }();
-    return !force_unpacked && P < SGR_PACKED_MAX_P;  // strict: id 0xffffff | mask 0xff would read as the "no record" word
-}
-
 static int validate(const SgrView *view, const SgrGaussians *g, bool forward)
 {
     if (!view || !g) {

@@ -361,9 +361,11 @@ __device__ __forceinline__ uint32_t block_mask_of_record(float x, float y, float
 // Instance words carry the footprint mask next to the Gaussian id when the ids fit 24 bits:
 //   low word of the sort key = id << 8 | mask   (the order by (depth, id) is unchanged: ids are unique)
 // and the sorted list the blend kernels read holds the same low words.  For P >= 2^24 Gaussians the low
-// word is the plain id and the blend kernels compute the mask while staging the record.
+// word is the plain id and the blend kernels compute the mask while staging the record.  The format is a
+// function of P alone, so the forward, the backward and sgr_inspect_state agree on it.
 #define SGR_PACKED_MAX_P (1 << 24)
-bool ids_packed(int P);  // host (sgr_api.cu): P < 2^24, unless SGR_FORCE_UNPACKED_IDS=1 (tests of the other format)
+// strict: id 0xffffff with mask 0xff would read as the "no record" word
+inline bool ids_packed(int P) { return P < SGR_PACKED_MAX_P; }
 
 __device__ __forceinline__ float warp_sum(float v)
 {

@@ -164,13 +164,34 @@ def to_torch(sc, device="cuda"):
                                            "viewmatrix", "projmatrix", "campos")}
 
 
+PACKED_MAX_P = 1 << 24   # SGR_PACKED_MAX_P (sgr_internal.cuh): the instance lists of P >= 2^24 Gaussians hold plain ids
+
+
+def pad_culled(t, names, pad_to=PACKED_MAX_P):
+    """The per-Gaussian tensors t[name] (names as in to_torch) with culled Gaussians appended up to pad_to rows, built
+    on their device.  The padding's means sit at the camera centre, at view depth 0, so preprocess culls them at the
+    near plane; they have finite scales, identity rotations, opacity and colour 0.5 and zero SH rows."""
+    import torch
+    P = t["means3D"].shape[0]
+    fill = dict(means3D=t["campos"].reshape(3), scales=0.01, rotations=torch.tensor([1.0, 0.0, 0.0, 0.0]),
+                opacities=0.5, colors_precomp=0.5, shs=0.0)
+    out = {}
+    for k in names:
+        row = torch.as_tensor(fill[k], dtype=t[k].dtype).to(t[k].device)
+        out[k] = torch.cat([t[k], row.expand((pad_to - P,) + t[k].shape[1:])])
+    return out
+
+
 def run_module(mod, sc, bg, dL=None, use_sh=True, use_cov_precomp=False, sh_degree=3, cov3D=None, device="cuda",
-               debug=False):
+               debug=False, pad_to=None):
     """Run GaussianRasterizer of `mod` (ours or the reference build).  Returns dict with image, radii, grads and
-    the saved opaque buffers."""
+    the saved opaque buffers.  pad_to: the Gaussians of `sc` followed by culled ones up to pad_to (pad_culled)."""
     import torch
     t = to_torch(sc, device)
-    leaf = lambda x: x.clone().requires_grad_(True)
+    if pad_to:
+        t.update(pad_culled(t, ["means3D", "opacities", "shs" if use_sh else "colors_precomp", "scales", "rotations"],
+                            pad_to))
+    leaf = lambda x: x.detach().requires_grad_(True)   # to_torch and pad_culled made fresh tensors
     means3D = leaf(t["means3D"]); opac = leaf(t["opacities"])
     means2D = torch.zeros_like(means3D, requires_grad=True)
     settings = mod.GaussianRasterizationSettings(
@@ -199,6 +220,40 @@ def run_module(mod, sc, bg, dL=None, use_sh=True, use_cov_precomp=False, sh_degr
     if dL is not None:
         (color * torch.from_numpy(dL).to(device)).sum().backward()
         out["grads"] = {k: v.grad.detach() for k, v in leaves.items() if v.grad is not None}
+    return out
+
+
+PER_GAUSSIAN = ("radii", "depths", "means2D", "conic_opacity", "rgb", "clamped", "tiles_touched")
+
+
+def run_state(sc, bg, dL=None, plain_ids=False, pad_to=PACKED_MAX_P, **opts):
+    """`sc` through ours, as numpy arrays: the forward state (_C.inspect_state), num_rendered, radii and color of a
+    forward-only run, and with an upstream gradient dL the image (color_bw) and gradients (grad_<name>) of a
+    forward + backward run.  plain_ids: culled Gaussians are appended up to pad_to (pad_culled), so that the library
+    lists plain ids, as it does for any cloud that large.  The padded rows must have radius 0, no tiles and zero
+    gradients; every per-Gaussian array is returned for the Gaussians of `sc` alone (the visible ids, and so the
+    lists, do not change)."""
+    import torch
+    from sugar_b200 import _C, diff_gaussian_rasterization as ours
+    P, W, H = sc.means3D.shape[0], sc.width, sc.height
+    pad = pad_to if plain_ids else None
+
+    def rows(k, v):
+        if plain_ids and (k in ("radii", "tiles_touched") or k.startswith("grad_")):
+            assert not v[P:].any(), f"{k}: a padded Gaussian is not culled"
+        return (v[:P] if k in PER_GAUSSIAN or k.startswith("grad_") else v).cpu().numpy()
+    a = run_module(ours, sc, bg, None, pad_to=pad, **opts)
+    st = _C.inspect_state(pad or P, W, H, a["num_rendered"], a["geom"], a["binning"], a["img"])
+    out = {k: rows(k, v) for k, v in dict(st, radii=a["radii"], color=a["color"]).items()}
+    out["num_rendered"] = np.int64(a["num_rendered"])
+    del a, st
+    if dL is not None:
+        b = run_module(ours, sc, bg, dL, pad_to=pad, **opts)
+        out.update({"grad_" + k: rows("grad_" + k, v) for k, v in b["grads"].items()})
+        out["color_bw"] = b["color"].cpu().numpy()
+        del b
+    if plain_ids:
+        torch.cuda.empty_cache()
     return out
 
 

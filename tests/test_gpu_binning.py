@@ -24,17 +24,15 @@ state before anything is compared:
 Depths never follow ids, so a sort that leaves a tile in scatter order fails.  Opacities are 0.01-0.05, so hundreds
 of list positions reach the image and the gradients.  Every scene is compared with the CPU oracle in both instance-list
 formats (keys, point_list and ranges bit-identical, n_contrib, final_T, image and every gradient at the oracle bars of
-tests/test_gpu_parity.py), and its lists are also checked without the oracle: (depth bits, id) strictly increasing in
-every tile and each tile's ids exactly those the means and radii imply.  test_id_format_boundary runs P = 2^24 - 1
+tests/test_gpu_parity.py; the plain-id run appends culled Gaussians up to P = 2^24, helpers.run_state), and its
+lists are also checked without the oracle: (depth bits, id) strictly increasing in every tile and each tile's ids
+exactly those the means and radii imply.  test_id_format_boundary runs P = 2^24 - 1
 (packed ids, whose largest word 0xfffffeff sits one below the "no record" word) and P = 2^24 (plain ids, chosen by P)
 against the same visible splats compacted into a five-Gaussian scene.  test_binning_scene_shapes_on_cpu_oracle builds
 the scenes and asserts their designed shape on the CPU oracle alone."""
 import math
 import os
 import re
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -63,7 +61,6 @@ def _constants():
 
 
 K = _constants()
-PACKED_MAX_P = 1 << 24    # SGR_PACKED_MAX_P (sgr_internal.cuh): ids of P >= 2^24 Gaussians are not packed
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -417,46 +414,7 @@ def test_binning_scene_shapes_on_cpu_oracle(name):
 # ------------------------------------------------------------------------------------------------------------------
 # GPU: both id formats against the oracle
 # ------------------------------------------------------------------------------------------------------------------
-def _run(name):
-    """Image, gradients and the forward state of `name` through ours, as numpy arrays."""
-    from sugar_b200 import _C, diff_gaussian_rasterization as ours, scenes
-    sc, _ = _make(name)
-    P, W, H = sc.means3D.shape[0], sc.width, sc.height
-    a0 = h.run_module(ours, sc, BG, None, use_sh=False)
-    st = _C.inspect_state(P, W, H, a0["num_rendered"], a0["geom"], a0["binning"], a0["img"])
-    a = h.run_module(ours, sc, BG, scenes.upstream_grad(W, H), use_sh=False)
-    out = {k: v.cpu().numpy() for k, v in st.items()}
-    out.update(color=a0["color"].cpu().numpy(), radii=a0["radii"].cpu().numpy(), color_bw=a["color"].cpu().numpy(),
-               **{"grad_" + k: v.cpu().numpy() for k, v in a["grads"].items()})
-    return out
-
-
-def _run_unpacked(names):
-    """_run of every scene with the instance lists in the plain-id format (read once per process: a subprocess)."""
-    code = ("import sys, numpy as np; sys.path[:0] = [%r, %r]; import test_gpu_binning as t; "
-            "np.savez(sys.argv[1], **{n + '/' + k: v for n in %r for k, v in t._run(n).items()})"
-            % (h.ROOT, os.path.join(h.ROOT, "tests"), list(names)))
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "u.npz")
-        subprocess.run([sys.executable, "-c", code, path], check=True,
-                       env=dict(os.environ, SGR_FORCE_UNPACKED_IDS="1"), timeout=900)
-        with np.load(path) as z:
-            res = {n: {} for n in names}
-            for k in z.files:
-                n, f = k.split("/", 1)
-                res[n][f] = z[k]
-            return res
-
-
-_UNPACKED, _ORACLE = {}, {}
-
-
-def _outputs(name, unpacked):
-    if not unpacked:
-        return _run(name)
-    if not _UNPACKED:
-        _UNPACKED.update(_run_unpacked(list(BUILDERS)))
-    return _UNPACKED[name]
+_ORACLE = {}
 
 
 def _oracle(name):
@@ -511,9 +469,10 @@ def _check_masks(o, W, H):
 @pytest.mark.parametrize("name", list(BUILDERS))
 def test_binning_edges_match_cpu_oracle(name, unpacked):
     import torch
+    from sugar_b200 import scenes
     sc, _ = _make(name)
     W, H = sc.width, sc.height
-    o = _outputs(name, unpacked)
+    o = h.run_state(sc, BG, scenes.upstream_grad(W, H), plain_ids=unpacked, use_sh=False)
     o = dict(o, point_list=o["point_list"].astype(np.int64))
     _check_shape(name, o, W, H, formats=(False,) if unpacked else (False, True))
     if name in ("radix_many", "merge_many"):
@@ -566,32 +525,18 @@ def _boundary_scene(P):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("P", [PACKED_MAX_P - 1, PACKED_MAX_P], ids=["packed_2^24-1", "plain_2^24"])
+@pytest.mark.parametrize("P", [h.PACKED_MAX_P - 1, h.PACKED_MAX_P], ids=["packed_2^24-1", "plain_2^24"])
 def test_id_format_boundary(P):
     """P = 2^24 - 1 keeps packed ids (the last id with a full mask is the word 0xfffffeff, one below the "no record"
     word); P = 2^24 switches to plain ids by P alone.  Both must give what the five visible splats give alone."""
     import torch
-    from sugar_b200 import _C, diff_gaussian_rasterization as ours, scenes
-    if os.environ.get("SGR_FORCE_UNPACKED_IDS", "") == "1":
-        pytest.skip("the format must be chosen by P")
+    from sugar_b200 import scenes
     big, small, vis = _boundary_scene(P)
     W, H = small.width, small.height
     dL = scenes.upstream_grad(W, H)
-
-    def run(sc):
-        n = sc.means3D.shape[0]
-        a0 = h.run_module(ours, sc, BG, None, use_sh=False)
-        st = {k: v.cpu().numpy() for k, v in
-              _C.inspect_state(n, W, H, a0["num_rendered"], a0["geom"], a0["binning"], a0["img"]).items()
-              if k in ("point_list", "ranges", "final_T", "n_contrib", "footprint")}
-        a = h.run_module(ours, sc, BG, dL, use_sh=False)
-        st.update(color=a0["color"].cpu().numpy(), radii=a0["radii"].cpu().numpy(),
-                  **{"grad_" + k: v.cpu().numpy() for k, v in a["grads"].items()})
-        del a0, a
-        torch.cuda.empty_cache()
-        return st
-    want = run(small)
-    got = run(big)
+    want = h.run_state(small, BG, dL, use_sh=False)
+    got = h.run_state(big, BG, dL, use_sh=False)
+    torch.cuda.empty_cache()
     others = np.ones(P, bool)
     others[vis] = False
     assert np.array_equal(got["radii"][vis], want["radii"]) and not got["radii"][others].any()
@@ -602,7 +547,7 @@ def test_id_format_boundary(P):
     assert np.array_equal(got["point_list"].astype(np.int64), vis[want["point_list"].astype(np.int64)])
     last = got["point_list"].astype(np.int64) == P - 1
     assert last.sum() == (W // 16) * (H // 16)
-    if P < PACKED_MAX_P:                                 # the largest packed word, id 2^24 - 2 with mask 0xff
+    if P < h.PACKED_MAX_P:                               # the largest packed word, id 2^24 - 2 with mask 0xff
         assert np.all(got["footprint"][last] == 0xff)
         assert ((P - 1) << 8 | 0xff) == 0xfffffeff
     for k in GRAD_NAMES:

@@ -8,12 +8,9 @@ releases the stage, so a chunk can hold splats of two stages.  Each scene below 
 batches (with a chunk that straddles them), a member without a valid lane followed by a contributing one, and a second
 member whose alpha is exactly 1/255.  The test checks that the list has that shape (from the forward state and the
 footprint masks) and holds the gradients to the CPU oracle at the tolerance of tests/test_gpu_parity.py, for both
-instance-list formats (packed ids with masks, and plain ids with the masks computed in the blend)."""
+instance-list formats (packed ids with masks, and plain ids with the masks computed in the blend; the plain-id run
+appends culled Gaussians up to P = 2^24, helpers.run_state)."""
 import math
-import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -88,48 +85,6 @@ def _make(name):
     return _scene(W, H, splats, seed=len(name))
 
 
-def _run(name):
-    """Image, gradients and the forward state of `name` through ours, as numpy arrays."""
-    from sugar_b200 import _C, diff_gaussian_rasterization as ours, scenes
-    sc = _make(name)
-    P, W, H = sc.means3D.shape[0], sc.width, sc.height
-    bg = (0.25, 0.5, 1.0)
-    a0 = h.run_module(ours, sc, bg, None, use_sh=False)
-    st = _C.inspect_state(P, W, H, a0["num_rendered"], a0["geom"], a0["binning"], a0["img"])
-    a = h.run_module(ours, sc, bg, scenes.upstream_grad(W, H), use_sh=False)
-    out = {k: v.cpu().numpy() for k, v in st.items()}
-    out.update(color=a0["color"].cpu().numpy(), **{"grad_" + k: v.cpu().numpy() for k, v in a["grads"].items()})
-    return out
-
-
-def _run_unpacked(names):
-    """_run of every scene with the instance lists in the plain-id format (read once per process: a subprocess)."""
-    code = ("import sys, numpy as np; sys.path[:0] = [%r, %r]; import test_gpu_blend_backward_overlap as t; "
-            "np.savez(sys.argv[1], **{n + '/' + k: v for n in %r for k, v in t._run(n).items()})"
-            % (h.ROOT, os.path.join(h.ROOT, "tests"), list(names)))
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "u.npz")
-        subprocess.run([sys.executable, "-c", code, path], check=True,
-                       env=dict(os.environ, SGR_FORCE_UNPACKED_IDS="1"), timeout=600)
-        with np.load(path) as z:
-            res = {n: {} for n in names}
-            for k in z.files:
-                n, f = k.split("/", 1)
-                res[n][f] = z[k]
-            return res
-
-
-_UNPACKED = {}
-
-
-def _outputs(name, unpacked):
-    if not unpacked:
-        return _run(name)
-    if not _UNPACKED:
-        _UNPACKED.update(_run_unpacked(list(SCENES)))
-    return _UNPACKED[name]
-
-
 def _walk(o, tile, W, wid):
     """(instance ids, walk slots) of warp `wid`'s members in tile `tile`, in walk order (back to front), from the
     forward state and the packed lists' footprint masks."""
@@ -197,7 +152,7 @@ def test_backward_walk_boundaries_match_cpu_oracle(name, unpacked):
     sc = _make(name)
     P, W, H = sc.means3D.shape[0], sc.width, sc.height
     fw, bw = h.run_oracle(sc, np.asarray((0.25, 0.5, 1.0), np.float32), scenes.upstream_grad(W, H), use_sh=False)
-    o = _outputs(name, unpacked)
+    o = h.run_state(sc, (0.25, 0.5, 1.0), scenes.upstream_grad(W, H), plain_ids=unpacked, use_sh=False)
     if not unpacked:
         _check_shape(name, o)   # the plain-id lists carry no masks; the packed run checks the scene
     assert np.array_equal(o["point_list"].view(np.uint32), fw["point_list"])

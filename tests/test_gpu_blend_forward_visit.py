@@ -17,12 +17,9 @@ while the warp's other lanes go on.  Each scene below puts one edge of that tail
 
 The test checks that each list has that shape (from the forward state and the footprint masks), then compares
 n_contrib exactly and final_T and the image with the CPU oracle at the tolerance of tests/test_gpu_parity.py, for both
-instance-list formats (packed ids with masks, and plain ids with the masks computed in the blend)."""
+instance-list formats (packed ids with masks, and plain ids with the masks computed in the blend; the plain-id run
+appends culled Gaussians up to P = 2^24, helpers.run_state)."""
 import math
-import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -99,46 +96,6 @@ def _power(o, g, px, py):
     return -0.5 * (a * dx * dx + c * dy * dy) - b * dx * dy
 
 
-def _run(name):
-    """Image and forward state of `name` through ours, as numpy arrays."""
-    from sugar_b200 import _C, diff_gaussian_rasterization as ours
-    sc = _make(name)
-    P, W, H = sc.means3D.shape[0], sc.width, sc.height
-    a = h.run_module(ours, sc, BG, None, use_sh=False)
-    st = _C.inspect_state(P, W, H, a["num_rendered"], a["geom"], a["binning"], a["img"])
-    out = {k: v.cpu().numpy() for k, v in st.items()}
-    out.update(color=a["color"].cpu().numpy())
-    return out
-
-
-def _run_unpacked(names):
-    """_run of every scene with the instance lists in the plain-id format (read once per process: a subprocess)."""
-    code = ("import sys, numpy as np; sys.path[:0] = [%r, %r]; import test_gpu_blend_forward_visit as t; "
-            "np.savez(sys.argv[1], **{n + '/' + k: v for n in %r for k, v in t._run(n).items()})"
-            % (h.ROOT, os.path.join(h.ROOT, "tests"), list(names)))
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "u.npz")
-        subprocess.run([sys.executable, "-c", code, path], check=True,
-                       env=dict(os.environ, SGR_FORCE_UNPACKED_IDS="1"), timeout=600)
-        with np.load(path) as z:
-            res = {n: {} for n in names}
-            for k in z.files:
-                n, f = k.split("/", 1)
-                res[n][f] = z[k]
-            return res
-
-
-_UNPACKED = {}
-
-
-def _outputs(name, unpacked):
-    if not unpacked:
-        return _run(name)
-    if not _UNPACKED:
-        _UNPACKED.update(_run_unpacked(list(SCENES)))
-    return _UNPACKED[name]
-
-
 def _check_shape(name, o, masks):
     """The list has the shape the scene is built for (o: the forward state; masks: whether o holds footprint masks)."""
     W, H, _ = SCENES[name]
@@ -190,7 +147,7 @@ def test_forward_visit_edges_match_cpu_oracle(name, unpacked):
     sc = _make(name)
     W, H = sc.width, sc.height
     fw, _ = h.run_oracle(sc, np.asarray(BG, np.float32), use_sh=False)
-    o = _outputs(name, unpacked)
+    o = h.run_state(sc, BG, plain_ids=unpacked, use_sh=False)
     _check_shape(name, o, masks=not unpacked)
     assert np.array_equal(o["point_list"].view(np.uint32), fw["point_list"])
     assert np.array_equal(o["ranges"].view(np.uint32), fw["ranges"])

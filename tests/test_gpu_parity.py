@@ -198,36 +198,6 @@ def test_matches_cpu_oracle(case):
     assert not bad, "; ".join(bad)
 
 
-def edge_outputs(bg):
-    """Forward state, image and gradients of helpers.opacity_edge_scene through ours, as numpy arrays."""
-    from sugar_b200 import _C, diff_gaussian_rasterization as ours, scenes
-    sc = h.opacity_edge_scene()
-    P, W, H = sc.means3D.shape[0], sc.width, sc.height
-    a0 = h.run_module(ours, sc, bg, None, use_sh=False)
-    st = _C.inspect_state(P, W, H, a0["num_rendered"], a0["geom"], a0["binning"], a0["img"])
-    a = h.run_module(ours, sc, bg, scenes.upstream_grad(W, H), use_sh=False)
-    out = {k: v.cpu().numpy() for k, v in st.items()}
-    out.update(num_rendered=np.int64(a0["num_rendered"]), radii=a0["radii"].cpu().numpy(), color=a0["color"].cpu().numpy(),
-               color_bw=a["color"].cpu().numpy(), **{"grad_" + k: v.cpu().numpy() for k, v in a["grads"].items()})
-    return out
-
-
-def _edge_outputs_unpacked(bg):
-    """edge_outputs with the instance lists in the unpacked-id format (read once per process: a subprocess)."""
-    import os
-    import subprocess
-    import sys
-    import tempfile
-    code = ("import sys, numpy as np; sys.path[:0] = [%r, %r]; import test_gpu_parity as t; "
-            "np.savez(sys.argv[1], **t.edge_outputs(%r))" % (h.ROOT, os.path.join(h.ROOT, "tests"), tuple(bg)))
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "u.npz")
-        subprocess.run([sys.executable, "-c", code, out], check=True, env=dict(os.environ, SGR_FORCE_UNPACKED_IDS="1"),
-                       timeout=600)
-        with np.load(out) as z:
-            return {k: z[k] for k in z.files}
-
-
 @pytest.mark.parametrize("unpacked", [False, True], ids=["packed_ids", "unpacked_ids"])
 @pytest.mark.parametrize("bg", [(0.0, 0.0, 0.0), (0.25, 0.5, 1.0)], ids=["bg0", "bg"])
 def test_opacity_at_the_alpha_threshold_matches_cpu_oracle(bg, unpacked):
@@ -239,7 +209,7 @@ def test_opacity_at_the_alpha_threshold_matches_cpu_oracle(bg, unpacked):
     P, W, H = sc.means3D.shape[0], sc.width, sc.height
     from sugar_b200 import scenes
     fw, bw = h.run_oracle(sc, np.asarray(bg, np.float32), scenes.upstream_grad(W, H), use_sh=False)
-    o = _edge_outputs_unpacked(bg) if unpacked else edge_outputs(bg)
+    o = h.run_state(sc, bg, scenes.upstream_grad(W, H), plain_ids=unpacked, use_sh=False)
     c = (W - 1) // 2
     assert int(fw["n_contrib"][c, c]) == P   # the oracle draws the farthest splat, of opacity 1/255 (test_oracle_properties)
     assert int(o["num_rendered"]) == fw["num_rendered"]
