@@ -428,6 +428,33 @@ SGR_API int sgr_mesh_nc_backward(int32_t Q, int32_t V, const float *verts, const
                                  const int32_t *vert_ptr, const int32_t *vert_inc, const float *g_loss, float *g_verts,
                                  void *scratch, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Splatted mesh and nearest-face triangle z-buffer: the default depth source of the level-set extraction
+ * (compute_level_surface_points_from_camera_fast with use_gaussian_depth=False, sugar_model.py:1880-1968).
+ * sgr_splat_mesh: SuGaR.splat_mesh(camera) for primitive 'diamond', mode 'perspective' (sugar_model.py:481-514,
+ * 695-728): four vertices per Gaussian, mu -/+ t s_a1 R[:,a1], mu +/- t s_a2 R[:,a2] (a0 = argmin s, lowest index on
+ * ties; a1, a2 the next two axes cyclically; t = triangle_scale; vertex order (-a1, +a2, +a1, -a2)), each moved along
+ * its view ray onto the plane through the centre perpendicular to the centre's ray.
+ *   points f32[P,3], scaling f32[P,3] (activated), quaternions f32[P,4] (w first; 16-byte aligned),
+ *   viewmatrix f32[16] (the rasterizer's transposed world->view), view_inverse f32[16] (its inverse, same layout),
+ *   verts f32[4P,3] (16-byte aligned), fully written.  The arithmetic is in double.  P = 0 launches nothing.
+ * sgr_mesh_raster: pytorch3d 0.7.4 MeshRasterizer (blur_radius 0, perspective-correct, no culling) read at its first
+ * face per pixel, for any mesh verts f32[V,3], faces i64[F,3] (ids outside [0, V) make the face cover nothing):
+ * vertices through viewmatrix (view z) and projmatrix (/ (w + 1e-7)), pixel (i, j) sampled at the rasterizer's ndc
+ * (2i+1)/W - 1; a face covers a pixel when every perspective-corrected barycentric is > 0 and the depth pz >= 0, and
+ * the pixel keeps the face of least pz (equal pz: the lower face id).  Unlike pytorch3d's binned path the result is
+ * complete however many faces overlap one region.
+ *   zbuf f32[H,W] (pz, -1 where no face covers), pix_to_face i64[H,W] (-1 there), fully written; identical from run to
+ *   run.  Limits: W, H <= 65535, W*H <= 2^31 - 1.  `scratch`: sgr_mesh_raster_scratch_bytes(F, W, H) bytes.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API int sgr_splat_mesh(int32_t P, const float *points, const float *scaling, const float *quaternions,
+                           const float *viewmatrix, const float *view_inverse, float triangle_scale, float *verts,
+                           void *stream);
+SGR_API size_t sgr_mesh_raster_scratch_bytes(int32_t F, int32_t W, int32_t H);
+SGR_API int sgr_mesh_raster(int32_t V, int32_t F, const float *verts, const int64_t *faces, const float *viewmatrix,
+                            const float *projmatrix, int32_t W, int32_t H, float *zbuf, int64_t *pix_to_face,
+                            void *scratch, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */

@@ -111,6 +111,10 @@ PROTOTYPES = {
     "sgr_mesh_nc_backward_scratch_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_mesh_nc_forward": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 5),
     "sgr_mesh_nc_backward": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 8),
+    "sgr_splat_mesh": (C.c_int, [C.c_int32] + [C.c_void_p] * 5 + [C.c_float, C.c_void_p, C.c_void_p]),
+    "sgr_mesh_raster_scratch_bytes": (C.c_size_t, [C.c_int32] * 3),
+    "sgr_mesh_raster": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32, C.c_int32] +
+                        [C.c_void_p] * 4),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),

@@ -7,13 +7,15 @@ Gaussian each one fell on, sample `n_points_in_range` (21) positions per ray wit
 standard deviations, evaluate the density at every sample from the K tracked neighbours, find the
 first crossing of each surface level and interpolate it; optionally the normals there.
 
-`level_surface_points_from_camera` is the whole per-view call with the reference's `use_gaussian_depth=True`
-branch in front (:1898-1909, 1926-1962): depth render of the view with this package's rasterizer (colours =
-view-space z, background -1), back-projection of every covered pixel, K nearest Gaussians of each point with
-the grid K-NN (get_gaussians_closest_to_samples, :1335-1343).  The reference's default branch rasterises a
-triangle soup with pytorch3d's MeshRasterizer instead; that renderer is outside this path.  The density evaluation -- in the reference 2M-point
-passes of gathered N x K x 3 x 3 matrices -- is ONE launch of the fused field kernel
-(sgr_field_forward) over all n_points * 21 samples; normals come from its backward (d density / d x).
+`level_surface_points_from_camera` is the whole per-view call with either depth source in front:
+  use_gaussian_depth=True (this function's default; :1898-1909, 1926-1964): depth render of the view with this
+    package's rasterizer (colours = view-space z, background -1), back-projection of every covered pixel, K nearest
+    Gaussians of each point with the grid K-NN (get_gaussians_closest_to_samples, :1335-1343);
+  use_gaussian_depth=False (the reference's default, which the extraction driver keeps; :1912-1928, 1965-1968): the
+    splatted diamond mesh z-buffered by `splatmesh.rasterize_mesh`, back-projection, and the ray's Gaussian
+    pix_to_face // 2 with its neighbours from the model's knn_idx table (no per-point K-NN search).
+The density evaluation -- in the reference 2M-point passes of gathered N x K x 3 x 3 matrices -- is ONE launch of the
+fused field kernel (sgr_field_forward) over all n_points * 21 samples; normals come from its backward (d density / d x).
 """
 import torch
 
@@ -80,33 +82,54 @@ def level_surface_points(world_points, camera_center, closest_gaussians_idx, poi
 
 def level_surface_points_from_camera(points, scaling, quaternions, strengths, cam, surface_levels=(0.1, 0.3, 0.5),
                                      n_surface_points=-1, n_points_in_range=21, range_size=3.0, density_factor=1.0,
-                                     knn_to_track=16, return_normals=False, return_pixel_idx=False, generator=None):
-    """compute_level_surface_points_from_camera_fast(use_gaussian_depth=True) for one view
-    (sugar_scene/sugar_model.py:1848-2083; driver loop: sugar_extractors/coarse_mesh.py:246-327).
+                                     knn_to_track=16, return_normals=False, return_pixel_idx=False, generator=None,
+                                     use_gaussian_depth=True, knn_idx=None, triangle_scale=2.0, return_gaussian_idx=False):
+    """compute_level_surface_points_from_camera_fast for one view (sugar_scene/sugar_model.py:1848-2083; driver loop:
+    sugar_extractors/coarse_mesh.py:246-327).
 
     `cam`: namespace with viewmatrix / projmatrix / campos device tensors (the rasterizer's transposed matrices) and
-    width, height, tanfovx, tanfovy (sugar_b200.steps.camera_from_scene).  Returns the dict of
-    `level_surface_points` plus, per level, 'pixel_idx' (flat index of each valid ray's pixel) when asked."""
+    width, height, tanfovx, tanfovy (sugar_b200.steps.camera_from_scene).  `use_gaussian_depth` keeps the reference's
+    flag name; True (the default here) renders the Gaussians' blended depth and searches the `knn_to_track` nearest
+    Gaussians of every back-projected point; False z-buffers the splatted mesh (`triangle_scale`, 2 in the
+    extraction) and takes the neighbours of the pixel's Gaussian from `knn_idx` (int64 [P,K], the model's
+    knn.reset_neighbors(points, K)[1] table; required there).  Returns the dict of `level_surface_points` plus, per
+    level, 'pixel_idx' (flat index of each valid ray's pixel) and 'gaussian_idx' (each valid ray's Gaussian: the
+    nearest one on the blended-depth branch, pix_to_face // 2 on the mesh branch) when asked."""
     from . import knn
     from .diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
     dev = points.device
     H, W = int(cam.height), int(cam.width)
+    if not use_gaussian_depth:
+        if knn_idx is None:
+            raise ValueError("use_gaussian_depth=False takes the neighbours from the model's table: pass knn_idx "
+                             "(knn.reset_neighbors(points, K)[1])")
+        if knn_idx.dtype != torch.int64 or knn_idx.dim() != 2 or knn_idx.shape[0] != points.shape[0]:
+            raise ValueError(f"knn_idx must be int64 [{points.shape[0]},K], got {knn_idx.dtype} {tuple(knn_idx.shape)}")
+        if knn_idx.device != dev:
+            raise ValueError(f"knn_idx on {knn_idx.device}, points on {dev}")
     with torch.no_grad():
-        # splatted depth (:1898-1909): colours = view-space z, background -1 marks uncovered pixels
-        view = points @ cam.viewmatrix[:3, :3] + cam.viewmatrix[3, :3]
-        st = GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=cam.tanfovx, tanfovy=cam.tanfovy,
-                                           bg=-torch.ones(3, device=dev), scale_modifier=1.0, viewmatrix=cam.viewmatrix,
-                                           projmatrix=cam.projmatrix, sh_degree=0, campos=cam.campos, prefiltered=False,
-                                           debug=False)
-        depth = GaussianRasterizer(st)(means3D=points, means2D=torch.zeros_like(points), opacities=strengths.view(-1, 1),
-                                       colors_precomp=view[:, 2:].expand(-1, 3).contiguous(), scales=scaling,
-                                       rotations=quaternions)[0][0]
-        no_depth = depth < 0.0                                                       # :1926
-        depth = torch.where(no_depth, depth.max() * 1.05, depth)                     # :1927
-        # back-projection of the covered pixels (:1929-1955) in the rasterizer's pixel convention
+        if use_gaussian_depth:
+            # splatted depth (:1898-1909): colours = view-space z, background -1 marks uncovered pixels
+            view = points @ cam.viewmatrix[:3, :3] + cam.viewmatrix[3, :3]
+            st = GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=cam.tanfovx, tanfovy=cam.tanfovy,
+                                               bg=-torch.ones(3, device=dev), scale_modifier=1.0,
+                                               viewmatrix=cam.viewmatrix, projmatrix=cam.projmatrix, sh_degree=0,
+                                               campos=cam.campos, prefiltered=False, debug=False)
+            depth = GaussianRasterizer(st)(means3D=points, means2D=torch.zeros_like(points),
+                                           opacities=strengths.view(-1, 1),
+                                           colors_precomp=view[:, 2:].expand(-1, 3).contiguous(), scales=scaling,
+                                           rotations=quaternions)[0][0]
+        else:
+            # splatted diamond mesh, nearest face per pixel (:1920-1928)
+            from . import splatmesh
+            verts, faces = splatmesh.splat_mesh(points, scaling, quaternions, cam, triangle_scale=triangle_scale)
+            depth, pix_to_face = splatmesh.rasterize_mesh(verts, faces, cam)
+        no_depth = depth < 0.0                                                       # :1929
+        depth = torch.where(no_depth, depth.max() * 1.05, depth)                     # :1930
+        # back-projection of the covered pixels (:1932-1959) in the rasterizer's pixel convention
         # (ndc2Pix, auxiliary.h:41-44: pixel = ((ndc + 1) S - 1) / 2)
         keep = (~no_depth).view(-1).nonzero()[:, 0]
-        if n_surface_points != -1 and n_surface_points < keep.numel():               # :1948-1951
+        if n_surface_points != -1 and n_surface_points < keep.numel():               # :1952-1958
             keep = keep[torch.randperm(keep.numel(), device=dev, generator=generator)[:n_surface_points]]
         py, px = (keep // W).float(), (keep % W).float()
         z = depth.view(-1)[keep]
@@ -114,12 +137,20 @@ def level_surface_points_from_camera(points, scaling, quaternions, strengths, ca
         yv = ((2.0 * py + 1.0) / H - 1.0) * cam.tanfovy * z
         Rt, t = cam.viewmatrix[:3, :3], cam.viewmatrix[3, :3]                        # p_view = p_world @ Rt + t
         world = (torch.stack([xv, yv, z], dim=1) - t) @ Rt.transpose(0, 1)
-        # the K Gaussians around every point (:1958-1960)
-        closest = knn.knn_points(world, points, knn_to_track)[1]
+        if use_gaussian_depth:
+            # the K Gaussians around every point (:1962-1964)
+            closest = knn.knn_points(world, points, knn_to_track)[1]
+            gaussian_idx = closest[:, 0]
+        else:
+            # the pixel's Gaussian and its neighbours from the model's table (:1965-1968)
+            gaussian_idx = pix_to_face.view(-1)[keep] // 2
+            closest = knn_idx[gaussian_idx]
     out = level_surface_points(world, cam.campos, closest, points, scaling, quaternions, strengths,
                                surface_levels=surface_levels, n_points_in_range=n_points_in_range,
                                range_size=range_size, density_factor=density_factor, return_normals=return_normals)
-    if return_pixel_idx:
-        for res in out.values():
+    for res in out.values():
+        if return_pixel_idx:
             res["pixel_idx"] = keep[res["valid"]]
+        if return_gaussian_idx:
+            res["gaussian_idx"] = gaussian_idx[res["valid"]]                        # :2048-2049
     return out
