@@ -455,6 +455,33 @@ SGR_API int sgr_mesh_raster(int32_t V, int32_t F, const float *verts, const int6
                             const float *projmatrix, int32_t W, int32_t H, float *zbuf, int64_t *pix_to_face,
                             void *scratch, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * UV texture of a mesh with n Gaussians bound per face (extract_texture_image_and_uv_from_gaussians,
+ * sugar_model.py:2464-2677, n_sh 1, texture_with_gaussian_renders).  The layout: square size s >= 3,
+ * n_sq = int(sqrt(F / 2 + 1) + 1), T = s * n_sq; square k = (k / n_sq, k % n_sq) holds face 2k (bottom) and 2k + 1 (top).
+ * sgr_texture_init: the initial texels, float32 as the reference computes them.  Every texel a face owns takes
+ * SH2RGB(sh_dc) of the face's Gaussian (f*n ... f*n + n-1) of greatest density at the texel's fixed barycentric point
+ * (torch argmax: NaN first, ties to the first); every other texel is 0.5.
+ *   verts f32[V,3], faces i64[F,3] (a face with an id outside [0, V) owns no texel), points / scaling f32[F*n,3],
+ *   quaternions f32[F*n,4] (w first; 16-byte aligned), sh_dc f32[F*n,3], texture f32[T,T,3] fully written.
+ *   T must equal the layout's; T*T <= 2^31 - 1.
+ * sgr_texture_bake_view: one view of the bake.  Every pixel with pix_to_face >= 0 and zbuf > 0 finds its texel
+ * (perspective-correct barycentrics in double through the z-buffer's projection, UV interpolated in float32, TexturesUV's
+ * nearest lookup); per texel, the pixel of highest row-major index adds clamp(image, 0, 1) to tex_sum and 1 to
+ * tex_count.  No float atomics: the sums are identical from run to run.
+ *   verts_uv f32[n_uv,2] (8-byte aligned), faces_uv i64[F,3], image f32[3,H,W], zbuf f32[H,W], pix_to_face i64[H,W]
+ *   (values outside [0, F) are empty pixels), tex_sum f32[T,T,3], tex_count i32[T,T] (accumulated), owner i32[T,T]
+ *   (all -1 on entry and on return), pix_texel i32[H,W] scratch.  T*T, W*H <= 2^31 - 1.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API int sgr_texture_init(int32_t F, int32_t n, int32_t V, int32_t square_size, int32_t T, const float *verts,
+                             const int64_t *faces, const float *points, const float *scaling, const float *quaternions,
+                             const float *sh_dc, float *texture, void *stream);
+SGR_API int sgr_texture_bake_view(int32_t V, int32_t F, int32_t n_uv, int32_t T, const float *verts,
+                                  const int64_t *faces, const float *verts_uv, const int64_t *faces_uv,
+                                  const float *viewmatrix, const float *projmatrix, int32_t W, int32_t H,
+                                  const float *image, const float *zbuf, const int64_t *pix_to_face, float *tex_sum,
+                                  int32_t *tex_count, int32_t *owner, int32_t *pix_texel, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */

@@ -115,6 +115,9 @@ PROTOTYPES = {
     "sgr_mesh_raster_scratch_bytes": (C.c_size_t, [C.c_int32] * 3),
     "sgr_mesh_raster": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32, C.c_int32] +
                         [C.c_void_p] * 4),
+    "sgr_texture_init": (C.c_int, [C.c_int32] * 5 + [C.c_void_p] * 8),
+    "sgr_texture_bake_view": (C.c_int, [C.c_int32] * 4 + [C.c_void_p] * 6 + [C.c_int32, C.c_int32] +
+                              [C.c_void_p] * 8),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),
