@@ -117,6 +117,34 @@ SGR_API int sgr_rasterize_backward(const SgrView *view, const SgrGaussians *g, c
                            float *dL_dscales, float *dL_drotations,
                            void *grad_scratch, void *stream);
 
+/* Forward and backward with one extra blended channel: a scalar per Gaussian (e.g. its view-space depth) blended
+ * with the same alphas and transmittances as the colours, over its own background.  One call renders what two
+ * sgr_rasterize_forward calls would (the second with colors_precomp = values in every channel and bg = *feature_bg),
+ * and out_color / out_feature are bit-identical to theirs (out_feature to channel 0 of the second).
+ *   values      f32[P]      the blended scalar (an input: its gradient is dL_dvalues)
+ *   feature_bg  f32[1]      DEVICE pointer to the channel's background
+ *   out_feature f32[H,W]    (fully written; zeros when P == 0, like out_color)
+ * The backward equals the sum of the two calls' backwards up to fp32 summation order:
+ *   dL_dout_feature f32[H,W] in, dL_dvalues f32[P] out (every row written, zeros for culled Gaussians);
+ *   the other outputs as in sgr_rasterize_backward, dL_dmeans2D / dL_dopacity / dL_dmeans3D ... holding both
+ *   channels' terms.
+ * Raw-parameter mode (SgrGaussians.activations != 0) is not supported. */
+SGR_API int sgr_rasterize_forward_feature(const SgrView *view, const SgrGaussians *g,
+                          SgrAlloc geom_alloc, void *geom_ctx,
+                          SgrAlloc binning_alloc, void *binning_ctx,
+                          SgrAlloc image_alloc, void *image_ctx,
+                          const float *values, const float *feature_bg,
+                          float *out_color, float *out_feature, int32_t *radii,
+                          int64_t capacity_hint, int64_t *num_rendered, void *stream);
+SGR_API int sgr_rasterize_backward_feature(const SgrView *view, const SgrGaussians *g, const int32_t *radii,
+                           const void *geom_buffer, const void *binning_buffer, const void *image_buffer,
+                           int64_t num_rendered, const float *dL_dout_color,
+                           const float *values, const float *feature_bg, const float *dL_dout_feature,
+                           float *dL_dmeans2D, float *dL_dcolors, float *dL_dopacity,
+                           float *dL_dmeans3D, float *dL_dcov3D, float *dL_dsh,
+                           float *dL_dscales, float *dL_drotations, float *dL_dvalues,
+                           void *grad_scratch, void *stream);
+
 /* The same backward with a plan: stage hooks, a chunked per-Gaussian pass and record-form outputs.  This is
  * what the view-parallel (one view per GPU) step drives, sugar_b200/parallel.py; the reference has no
  * counterpart (it renders one view on one GPU, sugar_trainers/coarse_sdf.py:98,507).

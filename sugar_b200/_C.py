@@ -291,6 +291,97 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     return out + (b["sh_rest"],) if raw else out
 
 
+def _no_exchange(context: Context):
+    if context.exchange is not None and context.exchange.enabled():
+        raise NotImplementedError("rasterize_with_depth under a view-parallel exchange: the exchange sums only the "
+                                  "rasterizer's own gradients, dL/dvalues would reach the points unsummed")
+
+
+def rasterize_gaussians_feature(background, means3D, colors, opacity, scales, rotations, scale_modifier,
+                                cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width,
+                                sh, degree, campos, prefiltered, debug, values, feature_bg, *, context: Context = None):
+    """rasterize_gaussians with one extra blended channel (sgr_rasterize_forward_feature): `values` f32[P] blended
+    over `feature_bg` (device f32[1]).  -> (R, color[3,H,W], feature[H,W], radii, geom, binning, img)."""
+    context = context or current_context()
+    _no_exchange(context)
+    if means3D.dim() != 2 or means3D.size(1) != 3:
+        raise RuntimeError("means3D must have dimensions (num_points, 3)")
+    if not means3D.is_cuda:
+        raise _lib.SgrError("sugar_b200 needs CUDA tensors: there is no CPU fallback")
+    dev = means3D.device
+    P, H, W = means3D.size(0), int(image_height), int(image_width)
+    if values.numel() != P or feature_bg.numel() != 1:
+        raise RuntimeError(f"values must hold one scalar per Gaussian ({P}, got {values.numel()}) and feature_bg one")
+    M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
+    with torch.cuda.device(dev):
+        out_color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        out_feature = torch.empty((H, W), dtype=torch.float32, device=dev)
+        radii = torch.empty((P,), dtype=torch.int32, device=dev)
+        key = (dev.index, H, W)
+        hint = context.capacity_hint.get(key, 0)
+        reserve = lib.sgr_geometry_bytes(P) + lib.sgr_image_bytes(W, H) + 1024
+        if hint:
+            reserve += lib.sgr_binning_bytes(hint)
+        arena = _Arena(dev, reserve if P else 0)
+        means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, values, feature_bg = map(
+            _c, (means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, values, feature_bg))
+        background, viewmatrix, projmatrix, campos = map(_c, (background, viewmatrix, projmatrix, campos))
+        view = _view_struct(background, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy, H, W, degree,
+                            campos, prefiltered, debug)
+        g = _gauss_struct(P, M, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp)
+        rendered = C.c_int64(0)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        status = lib.sgr_rasterize_forward_feature(
+            C.byref(view), C.byref(g), arena.cbs["geom"], None, arena.cbs["binning"], None, arena.cbs["img"], None,
+            _ptr(values, "values"), _ptr(feature_bg, "feature_bg"), out_color.data_ptr(), out_feature.data_ptr(),
+            radii.data_ptr() if P else None, hint, C.byref(rendered), stream)
+        if arena.error is not None:
+            err = arena.error
+            arena.release()
+            raise err
+        check(status)
+        R = int(rendered.value)
+        if P:
+            context.capacity_hint[key] = _round_up(int(R * 1.25) + 65536, 1 << 20)
+    geom_t, binning_t, img_t = arena.get("geom"), arena.get("binning"), arena.get("img")
+    arena.release()
+    return R, out_color, out_feature, radii, geom_t, binning_t, img_t
+
+
+def rasterize_gaussians_feature_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
+                                         cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh,
+                                         degree, campos, geomBuffer, R, binningBuffer, imageBuffer, debug, values,
+                                         feature_bg, dL_dout_feature, *, context: Context = None):
+    """rasterize_gaussians_backward of the feature forward (sgr_rasterize_backward_feature): the eight gradients of
+    rasterize_gaussians_backward, each holding both channels' terms, then dL/dvalues [P]."""
+    context = context or current_context()
+    _no_exchange(context)
+    dev = means3D.device
+    P, H, W = means3D.size(0), dL_dout_color.size(1), dL_dout_color.size(2)
+    M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
+    with torch.cuda.device(dev):
+        b = _alloc_backward(P, M, dev, with_records=False)
+        dL_dvalues = torch.empty((P,), dtype=torch.float32, device=dev)  # every row written by the library
+        if P != 0:
+            means3D, colors, scales, rotations, cov3D_precomp, sh, dL_dout_color, dL_dout_feature, values, feature_bg = \
+                map(_c, (means3D, colors, scales, rotations, cov3D_precomp, sh, dL_dout_color, dL_dout_feature, values,
+                         feature_bg))
+            background, viewmatrix, projmatrix, campos = map(_c, (background, viewmatrix, projmatrix, campos))
+            view = _view_struct(background, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy, H, W, degree,
+                                campos, False, debug)
+            g = _gauss_struct(P, M, means3D, None, sh, colors, scales, rotations, cov3D_precomp)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            check(lib.sgr_rasterize_backward_feature(
+                C.byref(view), C.byref(g), radii.data_ptr(), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
+                imageBuffer.data_ptr(), int(R), _ptr(dL_dout_color, "dL_dout_color"), _ptr(values, "values"),
+                _ptr(feature_bg, "feature_bg"), _ptr(dL_dout_feature, "dL_dout_feature"), b["means2D"].data_ptr(),
+                b["colors"].data_ptr(), b["opacity"].data_ptr(), b["means3D"].data_ptr(), b["cov3D"].data_ptr(),
+                b["sh"].data_ptr() if M else None, b["scales"].data_ptr(), b["rotations"].data_ptr(),
+                dL_dvalues.data_ptr(), b["scratch"].data_ptr(), stream))
+    return (b["means2D"], b["colors"], b["opacity"], b["means3D"], b["cov3D"], b["sh"], b["scales"], b["rotations"],
+            dL_dvalues)
+
+
 def mark_visible(means3D, viewmatrix, projmatrix) -> torch.Tensor:
     """markVisible (rasterize_points.cu:198-216)."""
     P = means3D.size(0)

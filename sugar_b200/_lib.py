@@ -69,7 +69,12 @@ PROTOTYPES = {
                                [C.c_int64] + [C.c_void_p] * 11),
     "sgr_rasterize_backward_staged": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians)] + [C.c_void_p] * 4 +
                                       [C.c_int64] + [C.c_void_p] * 11 + [C.POINTER(SgrBackwardPlan)]),
-    "sgr_backward_chunk_range": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "sgr_rasterize_forward_feature": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians), ALLOC_FN, C.c_void_p,
+                                                ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p] + [C.c_void_p] * 5 +
+                                      [C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
+    "sgr_rasterize_backward_feature": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians)] + [C.c_void_p] * 4 +
+                                       [C.c_int64] + [C.c_void_p] * 15),
+    "sgr_backward_chunk_range":(C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "sgr_backward_chunk_range_tapered": (C.c_int, [C.c_int32] * 4 + [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "sgr_view_grad_finalize": (C.c_int, [C.c_int32] * 6 + [C.c_void_p] * 3 + [C.c_int64, C.c_int32] + [C.c_void_p] * 2 +
                                [C.c_float] + [C.c_void_p] * 5),

@@ -305,7 +305,39 @@ int sgr_rasterize_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc g
         return SGR_EINVAL;
     }
     return launch_forward(view, g, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, out_color,
-                          radii, capacity_hint, num_rendered, st);
+                          radii, capacity_hint, num_rendered, st, nullptr);
+}
+
+int sgr_rasterize_forward_feature(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_alloc, void *geom_ctx,
+                                  SgrAlloc binning_alloc, void *binning_ctx, SgrAlloc image_alloc, void *image_ctx,
+                                  const float *values, const float *feature_bg, float *out_color, float *out_feature,
+                                  int32_t *radii, int64_t capacity_hint, int64_t *num_rendered, void *stream)
+{
+    int rc = validate(view, g, true);
+    if (rc) return rc;
+    if (!out_color || !out_feature || !num_rendered || !geom_alloc || !binning_alloc || !image_alloc) {
+        set_error("null output / allocator");
+        return SGR_EINVAL;
+    }
+    if (g->activations != 0) {
+        set_error("sgr_rasterize_forward_feature: raw-parameter mode is not supported");
+        return SGR_EINVAL;
+    }
+    *num_rendered = 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t npix = (size_t)view->image_width * view->image_height;
+    if (g->P == 0) {
+        SGR_CUDA(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * npix, st));
+        SGR_CUDA(cudaMemsetAsync(out_feature, 0, sizeof(float) * npix, st));
+        return SGR_OK;
+    }
+    if (!radii || !values || !feature_bg) {
+        set_error("radii / values / feature_bg must be non-null");
+        return SGR_EINVAL;
+    }
+    const FeatureChannel feat = {values, feature_bg, out_feature, nullptr, nullptr};
+    return launch_forward(view, g, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, out_color,
+                          radii, capacity_hint, num_rendered, st, &feat);
 }
 
 int sgr_rasterize_backward_staged(const SgrView *view, const SgrGaussians *g, const int32_t *radii, const void *geom_buffer,
@@ -325,7 +357,34 @@ int sgr_rasterize_backward_staged(const SgrView *view, const SgrGaussians *g, co
     }
     return launch_backward(view, g, radii, geom_buffer, binning_buffer, image_buffer, num_rendered, dL_dout_color,
                            dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
-                           dL_drotations, grad_scratch, (cudaStream_t)stream, plan);
+                           dL_drotations, grad_scratch, (cudaStream_t)stream, plan, nullptr);
+}
+
+int sgr_rasterize_backward_feature(const SgrView *view, const SgrGaussians *g, const int32_t *radii,
+                                   const void *geom_buffer, const void *binning_buffer, const void *image_buffer,
+                                   int64_t num_rendered, const float *dL_dout_color, const float *values,
+                                   const float *feature_bg, const float *dL_dout_feature, float *dL_dmeans2D,
+                                   float *dL_dcolors, float *dL_dopacity, float *dL_dmeans3D, float *dL_dcov3D,
+                                   float *dL_dsh, float *dL_dscales, float *dL_drotations, float *dL_dvalues,
+                                   void *grad_scratch, void *stream)
+{
+    int rc = validate(view, g, false);
+    if (rc) return rc;
+    if (g->activations != 0) {
+        set_error("sgr_rasterize_backward_feature: raw-parameter mode is not supported");
+        return SGR_EINVAL;
+    }
+    if (g->P == 0) return SGR_OK;
+    if (!radii || !geom_buffer || !binning_buffer || !image_buffer || !dL_dout_color || !values || !feature_bg ||
+        !dL_dout_feature || !dL_dmeans2D || !dL_dcolors || !dL_dopacity || !dL_dmeans3D || !dL_dcov3D ||
+        !dL_dscales || !dL_drotations || !dL_dvalues || !grad_scratch) {
+        set_error("null pointer passed to sgr_rasterize_backward_feature");
+        return SGR_EINVAL;
+    }
+    const FeatureChannel feat = {values, feature_bg, nullptr, dL_dout_feature, dL_dvalues};
+    return launch_backward(view, g, radii, geom_buffer, binning_buffer, image_buffer, num_rendered, dL_dout_color,
+                           dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
+                           dL_drotations, grad_scratch, (cudaStream_t)stream, nullptr, &feat);
 }
 
 int sgr_rasterize_backward(const SgrView *view, const SgrGaussians *g, const int32_t *radii, const void *geom_buffer,

@@ -98,6 +98,13 @@ constexpr uint32_t SM_A = 0, SM_B = SM_A + BWD_NS * BWD_B * 16, SM_C = SM_B + BW
                    BWD_SMEM_BYTES = SM_CHUNK + BWD_NW * CB_BYTES;
 static_assert(SM_BAR % 8 == 0 && BWD_B % 32 == 0, "mbarriers are 8-byte aligned; a batch is whole membership words");
 static_assert(4 * (BWD_SMEM_BYTES + 1024) <= 228 * 1024, "four CTAs of the backward blend must fit one SM's shared memory");
+// The feature blend (FEAT) adds 1 KB: the records' values, one f32 per stage slot, behind the plain layout.  Its dp
+// table holds (dL/dpixel r g b, dL/dpixel feature), so phase 2 gets the fourth channel from the load it already does;
+// the background term -T_final (<bg, dL/dpixel> + bg_feature dL/dpixel_feature) moves to the spare (pitch) column of
+// the pixel's row of the pair tile.  The chunk scratch keeps its size, and four CTAs still fit.
+constexpr uint32_t SM_V = BWD_SMEM_BYTES, BWD_SMEM_BYTES_FEAT = SM_V + BWD_NS * BWD_B * 4;
+static_assert(4 * (BWD_SMEM_BYTES_FEAT + 1024) <= 228 * 1024, "four CTAs of the feature blend must fit one SM");
+__host__ __device__ constexpr uint32_t CB_BGT(uint32_t px) { return (px * CH_PITCH + CH) * 8u; }
 
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar)
 {
@@ -119,8 +126,11 @@ __device__ __forceinline__ float ex2_approx(float x)
 
 // phase 2: reduce the parked chunk (nf splats) over the block's pixels and add it to the Gaussians'
 // accumulators.  Lane = (chunk slot, half): half h holds block rows 2h, 2h+1 = phase-1 lanes 16h..16h+15.
+// FEAT: also c3 = sum of dchannel * dL/dpixel(feature) over the pixels, added to dval[id] (no clamp mask)
+template <bool FEAT>
 __device__ __forceinline__ void chunk_flush(uint32_t cb, int nf, float blk_x0, float blk_y0, float ddelx_dx,
-                                            float ddely_dy, float *__restrict__ gacc, float *__restrict__ dcol)
+                                            float ddely_dy, float *__restrict__ gacc, float *__restrict__ dcol,
+                                            float *__restrict__ dval)
 {
     const unsigned lane = threadIdx.x & 31u;
     const int slot = (int)(lane & (CH - 1)), half = (int)(lane >> 4);
@@ -130,7 +140,7 @@ __device__ __forceinline__ void chunk_flush(uint32_t cb, int nf, float blk_x0, f
     // d = mean - pixel = (ax - cx_i, ay - cy_i) with the half's centre as origin: cx_i = (i & 7) - 3.5,
     // cy_i = (i >> 3) - 0.5
     const float ax = M0.x - (blk_x0 + 3.5f), ay = M0.y - (blk_y0 + 2.0f * (float)half + 0.5f);
-    float s_lo = 0.f, s_hi = 0.f, t_lo = 0.f, t_hi = 0.f, u = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f;
+    float s_lo = 0.f, s_hi = 0.f, t_lo = 0.f, t_hi = 0.f, u = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f;
     const uint32_t pa = cb + (half * 16 * CH_PITCH + slot) * 8, da = cb + CB_DP + half * 16 * 16;
 #pragma unroll
     for (int i = 0; i < 16; i++) {
@@ -148,6 +158,7 @@ __device__ __forceinline__ void chunk_flush(uint32_t cb, int nf, float blk_x0, f
         c0 = fmaf(pr.y, d.x, c0);
         c1 = fmaf(pr.y, d.y, c1);
         c2 = fmaf(pr.y, d.z, c2);
+        if (FEAT) c3 = fmaf(pr.y, d.w, c3);
     }
     const float s0 = s_lo + s_hi, sx = t_lo + t_hi, sy = 0.5f * (s_hi - s_lo), sxy = 0.5f * (t_hi - t_lo);
     float m0 = s0;
@@ -165,6 +176,7 @@ __device__ __forceinline__ void chunk_flush(uint32_t cb, int nf, float blk_x0, f
     c0 += __shfl_xor_sync(0xffffffffu, c0, 16);
     c1 += __shfl_xor_sync(0xffffffffu, c1, 16);
     c2 += __shfl_xor_sync(0xffffffffu, c2, 16);
+    if (FEAT) c3 += __shfl_xor_sync(0xffffffffu, c3, 16);
     if (slot < nf) {
         // moments -> gradients (backward.cu:537-554): dG/ddel = -G (Q d)
         float *g = gacc + (size_t)id * 8, *dc = dcol + (size_t)id * 3;
@@ -173,6 +185,7 @@ __device__ __forceinline__ void chunk_flush(uint32_t cb, int nf, float blk_x0, f
             const float gmy = -(M1.x * m2 + M0.w * m1) * ddely_dy;
             red_add_v4(g, gmx, gmy, -0.5f * m3, -0.5f * m4);
             if (!(clamp & 1u)) atomicAdd(dc, c0);
+            if (FEAT) atomicAdd(dval + id, c3);
         } else {
             red_add_v2(g + 4, -0.5f * m5, __fdividef(m0, M1.y));
             if (!(clamp & 2u)) atomicAdd(dc + 1, c1);
@@ -182,12 +195,15 @@ __device__ __forceinline__ void chunk_flush(uint32_t cb, int nf, float blk_x0, f
     __syncwarp();
 }
 
-template <bool packed>
+// FEAT: the feature channel of the forward's FEAT blend: values[P], its background *feat_bg, dL/d(feature map)
+// dL_dfeat[H,W] in, dL/dvalues into dval[P]; the FEAT = false instantiations ignore the last four arguments.
+template <bool packed, bool FEAT>
 __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
     const uint32_t *__restrict__ tile_order, const uint32_t *__restrict__ tile_start, const uint32_t *__restrict__ plist,
     const float4 *__restrict__ rec, int W, int H, int gx, const float *__restrict__ bg,
     const float *__restrict__ final_Ts, const uint32_t *__restrict__ n_contrib, const float *__restrict__ dL_dpixels,
-    float *__restrict__ gacc, float *__restrict__ dcol)
+    float *__restrict__ gacc, float *__restrict__ dcol, const float *__restrict__ values,
+    const float *__restrict__ feat_bg, const float *__restrict__ dL_dfeat, float *__restrict__ dval)
 {
     extern __shared__ __align__(16) unsigned char s_raw[];
     const int tile = (int)tile_order[blockIdx.x];
@@ -210,22 +226,29 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
     const int last_contributor = inside ? (int)n_contrib[pix] : 0;
     const uint32_t cb = sm + SM_CHUNK + wid * CB_BYTES;
     {
-        float dp0 = 0.f, dp1 = 0.f, dp2 = 0.f;
+        float dp0 = 0.f, dp1 = 0.f, dp2 = 0.f, dp3 = 0.f;
         if (inside) {
             dp0 = dL_dpixels[pix];
             dp1 = dL_dpixels[plane + pix];
             dp2 = dL_dpixels[2 * plane + pix];
+            if (FEAT) dp3 = dL_dfeat[pix];
         }
         // (dL/dpixel, -T_final * <bg, dL/dpixel>) of this pixel: phase 2 reads the block's table; the
         // hit path of phase 1 reloads its own entry instead of pinning four registers across the loop
-        sts128(cb + CB_DP + lane * 16, dp0, dp1, dp2, -T * fmaf(bg[2], dp2, fmaf(bg[1], dp1, bg[0] * dp0)));
+        const float bgdp = fmaf(bg[2], dp2, fmaf(bg[1], dp1, bg[0] * dp0));
+        if (FEAT) {  // (dL/dpixel r g b feature) in the table, the background term in the pair tile's spare column
+            sts128(cb + CB_DP + lane * 16, dp0, dp1, dp2, dp3);
+            sts32(cb + CB_BGT(lane), __float_as_uint(-T * fmaf(feat_bg[0], dp3, bgdp)));
+        } else {
+            sts128(cb + CB_DP + lane * 16, dp0, dp1, dp2, -T * bgdp);
+        }
     }
     // the pixel centre, pinned: under register pressure nvcc otherwise re-derives it from special
     // registers inside the splat loop
     float pxf = (float)pxi, pyf = (float)pyi;
     asm volatile("mov.f32 %0, %0;" : "+f"(pxf));
     asm volatile("mov.f32 %0, %0;" : "+f"(pyf));
-    float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
+    float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f, acc3 = 0.f;
     // Splats behind the deepest last contributor of the warp (of the tile) cannot touch any of its
     // pixels: the tile only walks list positions [0, tile_last), each warp only [0, warp_last).
     const int warp_last = __reduce_max_sync(0xffffffffu, last_contributor);
@@ -276,6 +299,7 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
             cp_async16_a(sm + SM_A + e * 16, r);
             cp_async16_a(sm + SM_B + e * 16, r + 1);
             cp_async16_a(sm + SM_C + e * 16, r + 2);
+            if (FEAT) cp_async4_a(sm + SM_V + e * 4, values + id);
             if (packed) mask = w & 0xffu;
         }
         if (!packed) {  // the mask needs the landed record
@@ -374,14 +398,21 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
                 float dL_dalpha = (B.w - acc0) * dp.x;
                 dL_dalpha = fmaf(Cc.x - acc1, dp.y, dL_dalpha);
                 dL_dalpha = fmaf(Cc.y - acc2, dp.z, dL_dalpha);
+                float fv = 0.f, bgt = dp.w;
+                if (FEAT) {
+                    fv = __uint_as_float(lds32(sm + SM_V + (buf * BWD_B + j) * 4));
+                    dL_dalpha = fmaf(fv - acc3, dp.w, dL_dalpha);
+                    bgt = __uint_as_float(lds32(cb + CB_BGT(lane)));
+                }
                 dL_dalpha *= Tn;
-                dL_dalpha = fmaf(dp.w, inv, dL_dalpha);
+                dL_dalpha = fmaf(bgt, inv, dL_dalpha);
                 const float S = hit ? B.z * dL_dalpha * G : 0.f;
                 const float dchannel = hit ? alpha * Tn : 0.f;
                 if (hit) {
                     acc0 = fmaf(alpha, B.w, om * acc0);
                     acc1 = fmaf(alpha, Cc.x, om * acc1);
                     acc2 = fmaf(alpha, Cc.y, om * acc2);
+                    if (FEAT) acc3 = fmaf(alpha, fv, om * acc3);
                     T = Tn;
                 }
                 // park: every lane its pair, lane `nfill` the batch slot (the metadata follows in stash_meta)
@@ -389,7 +420,7 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
                 if ((int)lane == nfill) pj = j;
                 if (++nfill == CH) {
                     stash_meta(sa, sb, sc, CH);
-                    chunk_flush(cb, CH, blk_x0, blk_y0, 0.5f * W, 0.5f * H, gacc, dcol);
+                    chunk_flush<FEAT>(cb, CH, blk_x0, blk_y0, 0.5f * W, 0.5f * H, gacc, dcol, dval);
                     nfill = nmeta = 0;
                 }
             }
@@ -398,7 +429,7 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars[BWD_NS + buf]);  // this warp no longer reads the stage
     }
-    if (nfill) chunk_flush(cb, nfill, blk_x0, blk_y0, 0.5f * W, 0.5f * H, gacc, dcol);
+    if (nfill) chunk_flush<FEAT>(cb, nfill, blk_x0, blk_y0, 0.5f * W, 0.5f * H, gacc, dcol, dval);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1270,11 +1301,32 @@ static void chunk_blocks(int blocks, int nchunks, int c, int taper, int *b0, int
     *b1 = c + 1 == nchunks ? blocks : edge(c + 1);
 }
 
+template <bool FEAT>
+static void launch_blend_backward(const SgrView *view, int P, const ImageState &img, const BinState &bin,
+                                  const GeomState &geom, const float *dL_dout_color, float *gacc, float *dL_dcolors,
+                                  const FeatureChannel *feat, cudaStream_t st)
+{
+    const int W = view->image_width, H = view->image_height;
+    const int gx = (W + SGR_TILE - 1) / SGR_TILE, gy = (H + SGR_TILE - 1) / SGR_TILE;
+    const uint32_t smem = FEAT ? BWD_SMEM_BYTES_FEAT : BWD_SMEM_BYTES;
+    const float *values = FEAT ? feat->values : nullptr, *feat_bg = FEAT ? feat->bg : nullptr;
+    const float *dL_dfeat = FEAT ? feat->dL_dout : nullptr;
+    float *dval = FEAT ? feat->dL_dvalues : nullptr;
+    if (ids_packed(P))
+        blend_backward_kernel<true, FEAT><<<gx * gy, 256, smem, st>>>(
+            img.tile_order, img.tile_start, bin.plist, geom.rec, W, H, gx, view->bg, img.final_T, img.n_contrib,
+            dL_dout_color, gacc, dL_dcolors, values, feat_bg, dL_dfeat, dval);
+    else
+        blend_backward_kernel<false, FEAT><<<gx * gy, 256, smem, st>>>(
+            img.tile_order, img.tile_start, bin.plist, geom.rec, W, H, gx, view->bg, img.final_T, img.n_contrib,
+            dL_dout_color, gacc, dL_dcolors, values, feat_bg, dL_dfeat, dval);
+}
+
 int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *radii, const void *geom_buffer,
                     const void *binning_buffer, const void *image_buffer, int64_t num_rendered,
                     const float *dL_dout_color, float *dL_dmeans2D, float *dL_dcolors, float *dL_dopacity,
                     float *dL_dmeans3D, float *dL_dcov3D, float *dL_dsh, float *dL_dscales, float *dL_drotations,
-                    void *grad_scratch, cudaStream_t st, const SgrBackwardPlan *plan)
+                    void *grad_scratch, cudaStream_t st, const SgrBackwardPlan *plan, const FeatureChannel *feat)
 {
     const int P = g->P, W = view->image_width, H = view->image_height;
     const int gx = (W + SGR_TILE - 1) / SGR_TILE, gy = (H + SGR_TILE - 1) / SGR_TILE;
@@ -1294,10 +1346,14 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
         SGR_CUDA(cudaGetDevice(&dev));
         std::lock_guard<std::mutex> lock(mu);
         if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)BWD_SMEM_BYTES));
-            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)BWD_SMEM_BYTES));
+            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true, false>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<false, false>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true, true>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES_FEAT));
+            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<false, true>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES_FEAT));
             SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           200 * 1024));
             SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1310,16 +1366,11 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     // the blend accumulators: 32 B per Gaussian of scratch + the dL_dcolors output itself
     SGR_CUDA(cudaMemsetAsync(gacc, 0, (size_t)P * 32, st));
     SGR_CUDA(cudaMemsetAsync(dL_dcolors, 0, (size_t)P * 12, st));
+    if (feat) SGR_CUDA(cudaMemsetAsync(feat->dL_dvalues, 0, (size_t)P * 4, st));
     if (num_rendered > 0) {
         SGR_LAUNCH(K_BLEND_BWD, st,
-                   if (ids_packed(P))
-                       blend_backward_kernel<true><<<gx * gy, 256, BWD_SMEM_BYTES, st>>>(
-                           img.tile_order, img.tile_start, bin.plist, geom.rec, W, H, gx, view->bg, img.final_T,
-                           img.n_contrib, dL_dout_color, gacc, dL_dcolors);
-                   else
-                       blend_backward_kernel<false><<<gx * gy, 256, BWD_SMEM_BYTES, st>>>(
-                           img.tile_order, img.tile_start, bin.plist, geom.rec, W, H, gx, view->bg, img.final_T,
-                           img.n_contrib, dL_dout_color, gacc, dL_dcolors));
+                   if (feat) launch_blend_backward<true>(view, P, img, bin, geom, dL_dout_color, gacc, dL_dcolors, feat, st);
+                   else launch_blend_backward<false>(view, P, img, bin, geom, dL_dout_color, gacc, dL_dcolors, feat, st));
     }
     // dL_dcolors is final here (with SH colours: the clamp-masked dL/dRGB, i.e. this view's SH factor)
     if (hook) hook(hook_ctx, SGR_STAGE_BLEND_DONE);

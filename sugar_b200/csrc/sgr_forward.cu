@@ -960,7 +960,9 @@ __device__ __forceinline__ uint32_t low_mask(uint32_t n)
 // No minimum CTA count in the launch bounds: with a minimum of 1 nvcc gives the packed format 38 registers (6 CTAs per
 // SM) instead of 32 (8 CTAs), and the unpacked one 53 instead of 48.  The extra CTAs outweigh the one instruction per
 // visit the 32-register code spends (DESIGN.md §3).
-template <bool packed>
+// FEAT: also blend one per-Gaussian scalar (values[P]) over its own background (*feat_bg) into out_feature[H,W],
+// with the colour channels' exact operations; the FEAT = false instantiations ignore the last three arguments.
+template <bool packed, bool FEAT>
 __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *__restrict__ tile_order,
                                                                 const uint32_t *__restrict__ tile_start,
                                                                 const uint32_t *__restrict__ plist,
@@ -969,11 +971,15 @@ __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *
                                                                 int W, int H, int gx, const float *__restrict__ bg,
                                                                 float *__restrict__ final_T,
                                                                 uint32_t *__restrict__ n_contrib,
-                                                                float *__restrict__ out_color)
+                                                                float *__restrict__ out_color,
+                                                                const float *__restrict__ values,
+                                                                const float *__restrict__ feat_bg,
+                                                                float *__restrict__ out_feature)
 {
-    // A batch slot is 48 contiguous bytes: (x, y, conic a, conic b), (conic c, tau, opacity, r), (g, b, -): one IMAD
-    // gives the slot's address and the loads take immediate offsets.  Every lane of a warp reads the same slot, so
-    // the loads are broadcasts and the 48-byte stride costs no bank conflicts.
+    // A batch slot is 48 contiguous bytes: (x, y, conic a, conic b), (conic c, tau, opacity, r), (g, b, value, -):
+    // one IMAD gives the slot's address and the loads take immediate offsets.  Every lane of a warp reads the same
+    // slot, so the loads are broadcasts and the 48-byte stride costs no bank conflicts.  `value` is only staged (and
+    // read) by FEAT.
     __shared__ __align__(16) float4 s_rec[BLEND_T * 3];
     // s_member[w][k]: slots 32k..32k+31 whose footprint mask has block w, bit-reversed (slot 32k + i is bit 31 - i)
     // so that the walk finds the next member with one clz
@@ -989,7 +995,7 @@ __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *
     const float pxf = (float)pxi, pyf = (float)pyi;
     const uint32_t lo = tile_start[tile], hi = tile_start[tile + 1];
     uint32_t done = inside ? 0u : 1u;  // 32-bit flag: a bool makes nvcc shuffle bytes (PRMT) in the hot loop
-    float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f;
+    float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, C3 = 0.f;
     uint32_t last = 0;
     const uint32_t srec = smem_addr_pinned(s_rec);
     const uint32_t smem_put = smem_addr_pinned(&s_member[0][wid]), smem_get = smem_addr_pinned(&s_member[wid][0]);
@@ -1006,11 +1012,13 @@ __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *
             if (!packed || mask) {
                 const float4 *r = rec + (size_t)id * 3;
                 const float4 r0 = __ldg(r), r1 = __ldg(r + 1), r2 = __ldg(r + 2);
+                const float fv = FEAT ? __ldg(values + id) : 0.f;
                 if (!packed) mask = block_mask_of_record(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, tx0, ty0);
                 const uint32_t p = srec + (uint32_t)tid * 48u;
                 sts128(p, r0.x, r0.y, r0.z, r0.w);
                 sts128(p + 16, r1.x, r1.y, r1.z, r1.w);
                 sts64(p + 32, r2.x, r2.y);
+                if (FEAT) sts32(p + 40, __float_as_uint(fv));
             }
         }
 #pragma unroll
@@ -1064,7 +1072,14 @@ __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *
                     if (!__any_sync(0xffffffffu, cand)) continue;
                     // Every lane of a warp with a candidate evaluates the tail; selects (not products with 0) keep
                     // what a lane that does not contribute had, signed zeros and NaNs included.
-                    const float2 Cc = lds64(p + 32);
+                    float4 Cc;  // (g, b, value, -): one LDS.128 with FEAT, an LDS.64 of (g, b) without
+                    if (FEAT) {
+                        Cc = lds128(p + 32);
+                    } else {
+                        const float2 gb = lds64(p + 32);
+                        Cc.x = gb.x;
+                        Cc.y = gb.y;
+                    }
                     const float alpha = fminf(0.99f, __fmul_rn(B.z, expf(power)));
                     const float test_T = __fmul_rn(T, __fsub_rn(1.0f, alpha));
                     const bool hit = cand && !(alpha < 1.0f / 255.0f);
@@ -1076,6 +1091,10 @@ __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *
                     C0 = contrib ? n0 : C0;
                     C1 = contrib ? n1 : C1;
                     C2 = contrib ? n2 : C2;
+                    if (FEAT) {
+                        const float n3 = __fmaf_rn(T, __fmul_rn(alpha, Cc.z), C3);
+                        C3 = contrib ? n3 : C3;
+                    }
                     T = contrib ? test_T : T;
                     last = contrib ? wlast - msb : last;
                 }
@@ -1090,6 +1109,7 @@ __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *
         out_color[pix] = __fmaf_rn(T, bg[0], C0);
         out_color[plane + pix] = __fmaf_rn(T, bg[1], C1);
         out_color[2 * plane + pix] = __fmaf_rn(T, bg[2], C2);
+        if (FEAT) out_feature[pix] = __fmaf_rn(T, feat_bg[0], C3);
     }
 }
 
@@ -1178,8 +1198,29 @@ struct SlotLease {  // returns the slot to its pool on every exit path
 
 static inline bool aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
 
+template <bool FEAT>
+static void launch_blend_forward(const ViewConsts &v, int P, const GeomState &geom, const ImageState &img,
+                                 const BinState &bin, uint64_t capacity, float *out_color, const FeatureChannel *feat,
+                                 cudaStream_t st)
+{
+    const int T = v.gx * v.gy;
+    const float *values = FEAT ? feat->values : nullptr, *feat_bg = FEAT ? feat->bg : nullptr;
+    float *out_feature = FEAT ? feat->out : nullptr;
+    if (ids_packed(P))
+        blend_forward_kernel<true, FEAT><<<T, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec,
+                                                                img.counters, capacity, v.W, v.H, v.gx, v.bg,
+                                                                img.final_T, img.n_contrib, out_color, values, feat_bg,
+                                                                out_feature);
+    else
+        blend_forward_kernel<false, FEAT><<<T, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec,
+                                                                 img.counters, capacity, v.W, v.H, v.gx, v.bg,
+                                                                 img.final_T, img.n_contrib, out_color, values, feat_bg,
+                                                                 out_feature);
+}
+
 static int launch_binning_and_blend(const ViewConsts &v, int P, const GeomState &geom, const ImageState &img,
-                                    const BinState &bin, uint64_t capacity, float *out_color, cudaStream_t st)
+                                    const BinState &bin, uint64_t capacity, float *out_color,
+                                    const FeatureChannel *feat, cudaStream_t st)
 {
     const int T = v.gx * v.gy;
     SGR_LAUNCH(K_SCATTER, st,
@@ -1199,21 +1240,16 @@ static int launch_binning_and_blend(const ViewConsts &v, int P, const GeomState 
                tile_sort_global_kernel<<<small_grid, GSORT_T, 0, st>>>(img.tile_start, img.counters, capacity,
                                                                        bin.inst_a, bin.inst_b, bin.plist, T));
     SGR_LAUNCH(K_BLEND_FWD, st,
-               if (ids_packed(P))
-                   blend_forward_kernel<true><<<T, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec,
-                                                                     img.counters, capacity, v.W, v.H, v.gx, v.bg,
-                                                                     img.final_T, img.n_contrib, out_color);
-               else
-                   blend_forward_kernel<false><<<T, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec,
-                                                                      img.counters, capacity, v.W, v.H, v.gx, v.bg,
-                                                                      img.final_T, img.n_contrib, out_color));
+               if (feat) launch_blend_forward<true>(v, P, geom, img, bin, capacity, out_color, feat, st);
+               else launch_blend_forward<false>(v, P, geom, img, bin, capacity, out_color, feat, st));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }
 
 int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_alloc, void *geom_ctx,
                    SgrAlloc binning_alloc, void *binning_ctx, SgrAlloc image_alloc, void *image_ctx, float *out_color,
-                   int32_t *radii, int64_t capacity_hint, int64_t *num_rendered, cudaStream_t st)
+                   int32_t *radii, int64_t capacity_hint, int64_t *num_rendered, cudaStream_t st,
+                   const FeatureChannel *feat)
 {
     const int P = g->P, W = view->image_width, H = view->image_height;
     SlotLease lease;
@@ -1312,7 +1348,7 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
             return SGR_ENOMEM;
         }
         bin = BinState::carve(bin_mem, capacity);
-        rc = launch_binning_and_blend(v, P, geom, img, bin, capacity, out_color, st);
+        rc = launch_binning_and_blend(v, P, geom, img, bin, capacity, out_color, feat, st);
         if (rc) return rc;
         launched = true;
     }
@@ -1329,7 +1365,7 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
         if (launched) {  // cursors were not advanced by the guarded attempt, but be explicit
             SGR_CUDA(cudaMemcpyAsync(img.tile_cursor, img.tile_start, sizeof(uint32_t) * T, cudaMemcpyDeviceToDevice, st));
         }
-        rc = launch_binning_and_blend(v, P, geom, img, bin, capacity, out_color, st);
+        rc = launch_binning_and_blend(v, P, geom, img, bin, capacity, out_color, feat, st);
         if (rc) return rc;
     }
     *num_rendered = (int64_t)R;

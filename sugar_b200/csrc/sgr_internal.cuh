@@ -468,6 +468,10 @@ __device__ __forceinline__ void cp_async8_a(uint32_t dst, const void *src)
 {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst), "l"(src) : "memory");
 }
+__device__ __forceinline__ void cp_async4_a(uint32_t dst, const void *src)
+{
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
 __device__ __forceinline__ void sts64(uint32_t addr, float a, float b)
 {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
@@ -479,14 +483,25 @@ __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c,
 
 #endif  // __CUDACC__
 
+// The extra blended channel of sgr_rasterize_{forward,backward}_feature: one scalar per Gaussian, blended with the
+// colour channels' alphas and transmittances over its own background.  A null pointer to it selects the plain blend.
+struct FeatureChannel {
+    const float *values;      // f32[P]
+    const float *bg;          // device f32[1]
+    float *out;               // forward: f32[H,W]
+    const float *dL_dout;     // backward: f32[H,W]
+    float *dL_dvalues;        // backward: f32[P]
+};
+
 // host-side stage entry points (defined in the .cu files)
 int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_alloc, void *geom_ctx,
                    SgrAlloc binning_alloc, void *binning_ctx, SgrAlloc image_alloc, void *image_ctx, float *out_color,
-                   int32_t *radii, int64_t capacity_hint, int64_t *num_rendered, cudaStream_t stream);
+                   int32_t *radii, int64_t capacity_hint, int64_t *num_rendered, cudaStream_t stream,
+                   const FeatureChannel *feat);
 int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *radii, const void *geom_buffer,
                     const void *binning_buffer, const void *image_buffer, int64_t num_rendered,
                     const float *dL_dout_color, float *dL_dmeans2D, float *dL_dcolors, float *dL_dopacity,
                     float *dL_dmeans3D, float *dL_dcov3D, float *dL_dsh, float *dL_dscales, float *dL_drotations,
-                    void *grad_scratch, cudaStream_t stream, const SgrBackwardPlan *plan);
+                    void *grad_scratch, cudaStream_t stream, const SgrBackwardPlan *plan, const FeatureChannel *feat);
 
 }  // namespace sgr

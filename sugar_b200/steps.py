@@ -25,6 +25,8 @@ fused kernels and over the reference's own building blocks (its CUDA rasterizer 
     ops.better_normal_loss(x, idx, nbr_idx, points, scaling, quaternions, nbr_opacity) -> [N]
     ops.l1_dssim(pred, gt, dssim_factor) -> scalar   (only called with dssim_factor > 0)
     ops.mesh_normal_consistency(verts, faces, topology) -> scalar   (only called with normal_consistency_factor > 0)
+    ops.rasterize_with_depth   sugar_b200.depth.rasterize_with_depth (only called with fused_depth=True; the
+                               reference has no counterpart)
 
 The photometric term is plain L1 by default (dssim_factor=0.0, what bench.py times); dssim_factor=0.2 gives the
 trainers' (1 - 0.2) L1 + 0.2 (1 - SSIM) (coarse_sdf.py:101-103, 452-457, refine.py:103-105, 499-504).  What is NOT
@@ -86,6 +88,20 @@ def render(ops, a, cam, bg, sh_deg, point_colors=None):
     return image, radii, means2D
 
 
+def render_with_depth(ops, a, cam, bg, sh_deg, point_values, depth_bg):
+    """`render` and the depth render of the same view in one call: ops.rasterize_with_depth, colours as `render`
+    picks them, `point_values` [P] blended over `depth_bg`.  -> (image, depth [H,W], radii)."""
+    st = ops.rasterizer.GaussianRasterizationSettings(
+        image_height=cam.height, image_width=cam.width, tanfovx=cam.tanfovx, tanfovy=cam.tanfovy, bg=bg,
+        scale_modifier=1.0, viewmatrix=cam.viewmatrix, projmatrix=cam.projmatrix, sh_degree=sh_deg, campos=cam.campos,
+        prefiltered=False, debug=False)
+    means2D = torch.zeros_like(a.points, requires_grad=True)
+    point_colors = ops.colors(a.points, a.sh, cam.campos, sh_deg)
+    kw = dict(colors_precomp=point_colors) if point_colors is not None else dict(shs=a.sh)
+    return ops.rasterize_with_depth(a.points, means2D, a.strengths, point_values, st, depth_bg, scales=a.scaling,
+                                    rotations=a.quaternions, **kw)
+
+
 def photometric_loss(ops, image, gt_rgb, dssim_factor):
     """Plain L1 when dssim_factor == 0, else the trainers' (1 - f) L1 + f (1 - SSIM) through ops.l1_dssim."""
     if dssim_factor == 0.0:
@@ -96,21 +112,35 @@ def photometric_loss(ops, image, gt_rgb, dssim_factor):
 def coarse_sdf_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, density_factor=1.0 / 16.0,
                     density_threshold=1.0, sdf_estimation_factor=0.2, sdf_better_normal_factor=0.2,
                     close_gaussian_threshold=2.0, sampling_scale_factor=1.5, spatial_extent=10.0, znear=0.01,
-                    generator=None, backward=True, dssim_factor=0.0):
+                    generator=None, backward=True, dssim_factor=0.0, fused_depth=False):
     """One regularised coarse-training iteration.  `raw`: dict of the model's raw parameter tensors (points,
     sh_dc [P,1,3], sh_rest [P,15,3], densities [P,1], scales [P,3], quaternions [P,4]); `cam`: namespace with
-    viewmatrix / projmatrix / campos device tensors and width, height, tanfovx, tanfovy; `knn_idx` [P,16]."""
+    viewmatrix / projmatrix / campos device tensors and width, height, tanfovx, tanfovy; `knn_idx` [P,16].
+    fused_depth=True renders steps 1 and 2 with one ops.rasterize_with_depth call instead of two rasterizer calls:
+    the same image, depth map and loss, one rasterization fewer."""
     from .field import sample_points_in_gaussians
     a = activate(raw)
     dev = a.points.device
-    # 1. RGB
-    image, radii, viewspace = render(ops, a, cam, torch.zeros(3, device=dev), sh_deg=3)
-    loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
-    vis = radii > 0
-    # 2. depth, with gradient
-    point_depth = world_to_view(a.points, cam.viewmatrix)[:, 2:].expand(-1, 3)
-    max_depth = point_depth.max()
-    depth = render(ops, a, cam, max_depth.detach() + torch.zeros(3, device=dev), sh_deg=0, point_colors=point_depth)[0][0]
+    if fused_depth:
+        if getattr(ops, "rasterize_with_depth", None) is None:
+            raise ValueError("fused_depth=True needs ops.rasterize_with_depth")
+        # 1. + 2. RGB and depth in one rasterizer call
+        point_depth = world_to_view(a.points, cam.viewmatrix)[:, 2]
+        max_depth = point_depth.max()
+        image, depth, radii = render_with_depth(ops, a, cam, torch.zeros(3, device=dev), 3, point_depth,
+                                                max_depth.detach())
+        loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
+        vis = radii > 0
+    else:
+        # 1. RGB
+        image, radii, viewspace = render(ops, a, cam, torch.zeros(3, device=dev), sh_deg=3)
+        loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
+        vis = radii > 0
+        # 2. depth, with gradient
+        point_depth = world_to_view(a.points, cam.viewmatrix)[:, 2:].expand(-1, 3)
+        max_depth = point_depth.max()
+        depth = render(ops, a, cam, max_depth.detach() + torch.zeros(3, device=dev), sh_deg=0,
+                       point_colors=point_depth)[0][0]
     # 3. which Gaussians sit on the rendered surface
     with torch.no_grad():
         to_cam = torch.nn.functional.normalize(cam.campos.view(1, 3) - a.points, dim=-1)
@@ -175,10 +205,11 @@ def camera_from_scene(sc, device):
 
 def ours_ops():
     """This package's operators: in-kernel SH colours, fused field / normal-loss kernels, fused mesh binding, fused
-    L1 + D-SSIM loss, fused mesh normal consistency."""
+    L1 + D-SSIM loss, fused mesh normal consistency, colour + depth in one rasterizer call."""
     from . import diff_gaussian_rasterization as dgr
-    from . import field, loss, meshbind, meshloss
+    from . import depth, field, loss, meshbind, meshloss
     return SimpleNamespace(rasterizer=dgr, colors=lambda points, sh, campos, deg: None,
+                           rasterize_with_depth=depth.rasterize_with_depth,
                            field_values=field.field_values, better_normal_loss=field.better_normal_loss,
                            bind_to_mesh=meshbind.bind_to_mesh, l1_dssim=loss.l1_dssim_loss,
                            mesh_normal_consistency=meshloss.mesh_normal_consistency)
