@@ -1,6 +1,9 @@
 """`_C`-compatible shim: the three symbols the reference's pybind module exports
 (diff-gaussian-rasterization/ext.cpp:15-19, rasterize_points.h:19-67), same positional
-signatures and return tuples, implemented over the C ABI of libsugar_b200.so.
+signatures and return tuples, implemented over the C ABI of libsugar_b200.so.  Keyword-only extras of
+`rasterize_gaussians` / `rasterize_gaussians_backward` select raw-parameter mode (`sh_rest`, sugar_b200/fused.py) and
+one more blended channel (`values`, sugar_b200/depth.py).  Each appends its gradient to the backward's tuple;
+`values` also appends the blended map to the forward's.
 
 torch is used only for device memory (caching allocator), the current stream and the device
 guard; all arithmetic happens in the hand-written sm_90a kernels.
@@ -154,21 +157,34 @@ def _c(t):
     return t if (t is None or t.is_contiguous()) else t.contiguous()
 
 
+def _no_exchange(context: Context):
+    if context.exchange is not None and context.exchange.enabled():
+        raise NotImplementedError("rasterize_with_depth under a view-parallel exchange: the exchange sums only the "
+                                  "rasterizer's own gradients, dL/dvalues would reach the points unsummed")
+
+
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                        prefiltered, debug, *, context: Context = None, sh_rest: torch.Tensor = None
-                        ) -> Tuple[int, torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
-    """RasterizeGaussiansCUDA (rasterize_points.cu:36-115).  Keyword-only extras that are not part of the
-    reference signature: `context` selects whose capacity hint is used (default: the calling thread's current
-    one); `sh_rest` selects raw-parameter mode (sugar_b200/fused.py): `sh` is then the model's DC array [P,1,3],
-    `sh_rest` [P,M-1,3], and opacity / scales / rotations are the RAW parameters, activated in the kernel."""
+                        prefiltered, debug, *, context: Context = None, sh_rest: torch.Tensor = None,
+                        values: torch.Tensor = None, feature_bg: torch.Tensor = None) -> Tuple:
+    """RasterizeGaussiansCUDA (rasterize_points.cu:36-115) -> (R, color[3,H,W], radii, geom, binning, img).
+    Keyword-only extras that are not part of the reference signature: `context` selects whose capacity hint is used
+    (default: the calling thread's current one); `sh_rest` selects raw-parameter mode (sugar_b200/fused.py): `sh` is
+    then the model's DC array [P,1,3], `sh_rest` [P,M-1,3], and opacity / scales / rotations are the RAW parameters,
+    activated in the kernel; `values` f32[P] blends one extra channel over `feature_bg` (device f32[1])
+    (sgr_rasterize_forward_feature, sugar_b200/depth.py) and appends that map [H,W] to the returned tuple."""
     context = context or current_context()
+    feature = values is not None
+    if feature:
+        _no_exchange(context)
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
     if not means3D.is_cuda:
         raise _lib.SgrError("sugar_b200 needs CUDA tensors: there is no CPU fallback")
     dev = means3D.device
     P, H, W = means3D.size(0), int(image_height), int(image_width)
+    if feature and (values.numel() != P or feature_bg.numel() != 1):
+        raise RuntimeError(f"values must hold one scalar per Gaussian ({P}, got {values.numel()}) and feature_bg one")
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     if sh_rest is not None:
         if M != 1 or sh_rest.dim() != 3 or sh_rest.size(0) != P:
@@ -177,6 +193,7 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         sh_rest = _c(sh_rest)
     with torch.cuda.device(dev):
         out_color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        out_feature = torch.empty((H, W), dtype=torch.float32, device=dev) if feature else None
         radii = torch.empty((P,), dtype=torch.int32, device=dev)
         key = (dev.index, H, W)
         hint = context.capacity_hint.get(key, 0)
@@ -184,17 +201,22 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         if hint:
             reserve += lib.sgr_binning_bytes(hint)
         arena = _Arena(dev, reserve if P else 0)
-        means3D, colors, opacity, scales, rotations, cov3D_precomp, sh = map(
-            _c, (means3D, colors, opacity, scales, rotations, cov3D_precomp, sh))
+        means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, values, feature_bg = map(
+            _c, (means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, values, feature_bg))
         background, viewmatrix, projmatrix, campos = map(_c, (background, viewmatrix, projmatrix, campos))
         view = _view_struct(background, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy, H, W, degree,
                             campos, prefiltered, debug)
         g = _gauss_struct(P, M, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp, sh_rest)
         rendered = C.c_int64(0)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        status = lib.sgr_rasterize_forward(C.byref(view), C.byref(g), arena.cbs["geom"], None, arena.cbs["binning"], None,
-                                           arena.cbs["img"], None, out_color.data_ptr(), radii.data_ptr() if P else None,
-                                           hint, C.byref(rendered), stream)
+        allocs = (arena.cbs["geom"], None, arena.cbs["binning"], None, arena.cbs["img"], None)
+        tail = (radii.data_ptr() if P else None, hint, C.byref(rendered), stream)
+        if feature:
+            status = lib.sgr_rasterize_forward_feature(
+                C.byref(view), C.byref(g), *allocs, _ptr(values, "values"), _ptr(feature_bg, "feature_bg"),
+                out_color.data_ptr(), out_feature.data_ptr(), *tail)
+        else:
+            status = lib.sgr_rasterize_forward(C.byref(view), C.byref(g), *allocs, out_color.data_ptr(), *tail)
         if arena.error is not None:   # the allocator callback failed (e.g. out of memory): its own exception, not
             err = arena.error         # the library's generic "allocator returned NULL"
             arena.release()
@@ -206,7 +228,8 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
             context.capacity_hint[key] = _round_up(int(R * 1.25) + 65536, 1 << 20)
     geom_t, binning_t, img_t = arena.get("geom"), arena.get("binning"), arena.get("img")
     arena.release()
-    return R, out_color, radii, geom_t, binning_t, img_t
+    out = (R, out_color, radii, geom_t, binning_t, img_t)
+    return out + (out_feature,) if feature else out
 
 
 _PART_ALIGN = 16  # floats: every gradient array starts on a 64-byte boundary (TMA bulk stores need 16)
@@ -243,12 +266,18 @@ def _alloc_backward(P: int, M: int, dev, with_records: bool, split_sh: bool = Fa
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
                                  cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh,
                                  degree, campos, geomBuffer, R, binningBuffer, imageBuffer, debug, *,
-                                 context: Context = None, sh_rest: torch.Tensor = None):
+                                 context: Context = None, sh_rest: torch.Tensor = None, values: torch.Tensor = None,
+                                 feature_bg: torch.Tensor = None, dL_dout_feature: torch.Tensor = None):
     """RasterizeGaussiansBackwardCUDA (rasterize_points.cu:118-196).  With a view-parallel exchange attached to
     `context` (sugar_b200/parallel.py) the gradients come back already summed over the ranks.  With `sh_rest`
     (raw-parameter mode, see rasterize_gaussians) a ninth tensor dL_dsh_rest is returned and dL_dopacity /
-    dL_dscales / dL_drotations / dL_dsh are gradients of the raw parameters."""
+    dL_dscales / dL_drotations / dL_dsh are gradients of the raw parameters.  With `values` (the extra channel of
+    rasterize_gaussians, gradient `dL_dout_feature` [H,W]; sgr_rasterize_backward_feature) each of the eight
+    gradients holds both channels' terms and a ninth tensor dL_dvalues [P] is returned."""
     context = context or current_context()
+    feature = values is not None
+    if feature:
+        _no_exchange(context)
     dev = means3D.device
     P, H, W = means3D.size(0), dL_dout_color.size(1), dL_dout_color.size(2)
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
@@ -264,122 +293,46 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         has_cov = cov3D_precomp is not None and cov3D_precomp.numel() != 0
         # the peer-memory exchange keeps its records in its own peer-visible buffer
         b = _alloc_backward(P, M, dev, with_records=ex is not None and not ex.uses_peer_memory(M, has_cov), split_sh=raw)
+        dL_dvalues = torch.empty((P,), dtype=torch.float32, device=dev) if feature else None  # every row written
         if P != 0:
             means3D, colors, scales, rotations, cov3D_precomp, sh, dL_dout_color = map(
                 _c, (means3D, colors, scales, rotations, cov3D_precomp, sh, dL_dout_color))
+            values, feature_bg, dL_dout_feature = map(_c, (values, feature_bg, dL_dout_feature))
             background, viewmatrix, projmatrix, campos = map(_c, (background, viewmatrix, projmatrix, campos))
             view = _view_struct(background, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy, H, W, degree,
                                 campos, False, debug)
             # opacities are not an input of the reference's backward; the forward stored them
             g = _gauss_struct(P, M, means3D, None, sh, colors, scales, rotations, cov3D_precomp, sh_rest)
             stream = torch.cuda.current_stream(dev).cuda_stream
-            factor = ex is not None and bool(M) and ex.sh_factors
-            args = (C.byref(view), C.byref(g), radii.data_ptr(), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
-                    imageBuffer.data_ptr(), int(R), _ptr(dL_dout_color, "dL_dout_color"), b["means2D"].data_ptr(),
-                    b["colors"].data_ptr(), b["opacity"].data_ptr(), b["means3D"].data_ptr(), b["cov3D"].data_ptr(),
-                    b["sh"].data_ptr() if (M and not factor) else None, b["scales"].data_ptr(),
-                    b["rotations"].data_ptr(), b["scratch"].data_ptr(), stream)
-            if raw:
-                plan = _lib.SgrBackwardPlan(_lib.STAGE_HOOK(0), None, 1, None, b["sh_rest"].data_ptr() if M > 1 else None)
-                check(lib.sgr_rasterize_backward_staged(*args, C.byref(plan)))
-            elif ex is None:
-                check(lib.sgr_rasterize_backward(*args))
+            # the SH exchange rebuilds the summed dL_dsh from the views' colour gradients: the pass does not write it
+            dsh = b["sh"].data_ptr() if (M and not (ex is not None and ex.sh_factors)) else None
+            inputs = (C.byref(view), C.byref(g), radii.data_ptr(), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
+                      imageBuffer.data_ptr(), int(R), _ptr(dL_dout_color, "dL_dout_color"))
+
+            def grads(dL_dcolors, dL_dsh):   # the eight gradient arrays in the C argument order
+                return (b["means2D"].data_ptr(), dL_dcolors, b["opacity"].data_ptr(), b["means3D"].data_ptr(),
+                        b["cov3D"].data_ptr(), dL_dsh, b["scales"].data_ptr(), b["rotations"].data_ptr())
+
+            def launch(plan, *, dL_dcolors=b["colors"].data_ptr(), dL_dsh=dsh):
+                """Enqueue sgr_rasterize_backward_staged under `plan` (None: no stages); the view-parallel peer
+                exchange points the two outputs it sums itself into its own buffers."""
+                check(lib.sgr_rasterize_backward_staged(*inputs, *grads(dL_dcolors, dL_dsh), b["scratch"].data_ptr(),
+                                                        stream, None if plan is None else C.byref(plan)))
+
+            if feature:
+                check(lib.sgr_rasterize_backward_feature(
+                    *inputs, _ptr(values, "values"), _ptr(feature_bg, "feature_bg"),
+                    _ptr(dL_dout_feature, "dL_dout_feature"), *grads(b["colors"].data_ptr(), dsh),
+                    dL_dvalues.data_ptr(), b["scratch"].data_ptr(), stream))
+            elif ex is not None:
+                ex.run_backward(launch, b, P, M, int(degree), means3D, campos, has_cov_precomp=has_cov)
+            elif raw:   # the plan carries the second SH gradient array
+                launch(_lib.SgrBackwardPlan(_lib.STAGE_HOOK(0), None, 1, None,
+                                            b["sh_rest"].data_ptr() if M > 1 else None))
             else:
-                ex.run_backward(lib, check, _lib.STAGE_HOOK, _lib.SgrBackwardPlan, args, b, P, M, int(degree), means3D,
-                                campos, has_cov_precomp=has_cov)
+                launch(None)
     out = (b["means2D"], b["colors"], b["opacity"], b["means3D"], b["cov3D"], b["sh"], b["scales"], b["rotations"])
-    return out + (b["sh_rest"],) if raw else out
-
-
-def _no_exchange(context: Context):
-    if context.exchange is not None and context.exchange.enabled():
-        raise NotImplementedError("rasterize_with_depth under a view-parallel exchange: the exchange sums only the "
-                                  "rasterizer's own gradients, dL/dvalues would reach the points unsummed")
-
-
-def rasterize_gaussians_feature(background, means3D, colors, opacity, scales, rotations, scale_modifier,
-                                cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width,
-                                sh, degree, campos, prefiltered, debug, values, feature_bg, *, context: Context = None):
-    """rasterize_gaussians with one extra blended channel (sgr_rasterize_forward_feature): `values` f32[P] blended
-    over `feature_bg` (device f32[1]).  -> (R, color[3,H,W], feature[H,W], radii, geom, binning, img)."""
-    context = context or current_context()
-    _no_exchange(context)
-    if means3D.dim() != 2 or means3D.size(1) != 3:
-        raise RuntimeError("means3D must have dimensions (num_points, 3)")
-    if not means3D.is_cuda:
-        raise _lib.SgrError("sugar_b200 needs CUDA tensors: there is no CPU fallback")
-    dev = means3D.device
-    P, H, W = means3D.size(0), int(image_height), int(image_width)
-    if values.numel() != P or feature_bg.numel() != 1:
-        raise RuntimeError(f"values must hold one scalar per Gaussian ({P}, got {values.numel()}) and feature_bg one")
-    M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
-    with torch.cuda.device(dev):
-        out_color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        out_feature = torch.empty((H, W), dtype=torch.float32, device=dev)
-        radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        key = (dev.index, H, W)
-        hint = context.capacity_hint.get(key, 0)
-        reserve = lib.sgr_geometry_bytes(P) + lib.sgr_image_bytes(W, H) + 1024
-        if hint:
-            reserve += lib.sgr_binning_bytes(hint)
-        arena = _Arena(dev, reserve if P else 0)
-        means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, values, feature_bg = map(
-            _c, (means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, values, feature_bg))
-        background, viewmatrix, projmatrix, campos = map(_c, (background, viewmatrix, projmatrix, campos))
-        view = _view_struct(background, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy, H, W, degree,
-                            campos, prefiltered, debug)
-        g = _gauss_struct(P, M, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp)
-        rendered = C.c_int64(0)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        status = lib.sgr_rasterize_forward_feature(
-            C.byref(view), C.byref(g), arena.cbs["geom"], None, arena.cbs["binning"], None, arena.cbs["img"], None,
-            _ptr(values, "values"), _ptr(feature_bg, "feature_bg"), out_color.data_ptr(), out_feature.data_ptr(),
-            radii.data_ptr() if P else None, hint, C.byref(rendered), stream)
-        if arena.error is not None:
-            err = arena.error
-            arena.release()
-            raise err
-        check(status)
-        R = int(rendered.value)
-        if P:
-            context.capacity_hint[key] = _round_up(int(R * 1.25) + 65536, 1 << 20)
-    geom_t, binning_t, img_t = arena.get("geom"), arena.get("binning"), arena.get("img")
-    arena.release()
-    return R, out_color, out_feature, radii, geom_t, binning_t, img_t
-
-
-def rasterize_gaussians_feature_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
-                                         cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh,
-                                         degree, campos, geomBuffer, R, binningBuffer, imageBuffer, debug, values,
-                                         feature_bg, dL_dout_feature, *, context: Context = None):
-    """rasterize_gaussians_backward of the feature forward (sgr_rasterize_backward_feature): the eight gradients of
-    rasterize_gaussians_backward, each holding both channels' terms, then dL/dvalues [P]."""
-    context = context or current_context()
-    _no_exchange(context)
-    dev = means3D.device
-    P, H, W = means3D.size(0), dL_dout_color.size(1), dL_dout_color.size(2)
-    M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
-    with torch.cuda.device(dev):
-        b = _alloc_backward(P, M, dev, with_records=False)
-        dL_dvalues = torch.empty((P,), dtype=torch.float32, device=dev)  # every row written by the library
-        if P != 0:
-            means3D, colors, scales, rotations, cov3D_precomp, sh, dL_dout_color, dL_dout_feature, values, feature_bg = \
-                map(_c, (means3D, colors, scales, rotations, cov3D_precomp, sh, dL_dout_color, dL_dout_feature, values,
-                         feature_bg))
-            background, viewmatrix, projmatrix, campos = map(_c, (background, viewmatrix, projmatrix, campos))
-            view = _view_struct(background, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy, H, W, degree,
-                                campos, False, debug)
-            g = _gauss_struct(P, M, means3D, None, sh, colors, scales, rotations, cov3D_precomp)
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            check(lib.sgr_rasterize_backward_feature(
-                C.byref(view), C.byref(g), radii.data_ptr(), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
-                imageBuffer.data_ptr(), int(R), _ptr(dL_dout_color, "dL_dout_color"), _ptr(values, "values"),
-                _ptr(feature_bg, "feature_bg"), _ptr(dL_dout_feature, "dL_dout_feature"), b["means2D"].data_ptr(),
-                b["colors"].data_ptr(), b["opacity"].data_ptr(), b["means3D"].data_ptr(), b["cov3D"].data_ptr(),
-                b["sh"].data_ptr() if M else None, b["scales"].data_ptr(), b["rotations"].data_ptr(),
-                dL_dvalues.data_ptr(), b["scratch"].data_ptr(), stream))
-    return (b["means2D"], b["colors"], b["opacity"], b["means3D"], b["cov3D"], b["sh"], b["scales"], b["rotations"],
-            dL_dvalues)
+    return out + ((b["sh_rest"],) if raw else (dL_dvalues,) if feature else ())
 
 
 def mark_visible(means3D, viewmatrix, projmatrix) -> torch.Tensor:

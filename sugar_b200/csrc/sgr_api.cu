@@ -7,6 +7,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <mutex>
+
 #include "sgr_internal.cuh"
 
 namespace sgr {
@@ -25,6 +27,29 @@ int cuda_fail(cudaError_t e, const char *what)
 {
     set_error("[CUDA ERROR] %s: %s", what, cudaGetErrorString(e));
     return SGR_ECUDA;
+}
+
+int current_device(int *dev)
+{
+    SGR_CUDA(cudaGetDevice(dev));
+    if (*dev < 0 || *dev >= SGR_MAX_DEVICES) {
+        set_error("device ordinal %d out of range", *dev);
+        return SGR_EINVAL;
+    }
+    return SGR_OK;
+}
+
+int once_per_device(DeviceOnce &once, int (*init)())
+{
+    static std::mutex mu;
+    int dev = 0;
+    int rc = current_device(&dev);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lock(mu);
+    if (once.done[dev]) return SGR_OK;
+    rc = init();
+    once.done[dev] = rc == SGR_OK;
+    return rc;
 }
 
 int device_sm_count()
@@ -113,6 +138,67 @@ static int validate(const SgrView *view, const SgrGaussians *g, bool forward)
         return SGR_EINVAL;
     }
     return SGR_OK;
+}
+
+// The plain and the feature forward (feat != NULL): argument checks, then P == 0 fills the outputs without launching
+// anything (rasterize_points.cu:81).  The feature adds only its own pointers and its rejection of raw-parameter mode.
+static int rasterize_forward(const char *who, const SgrView *view, const SgrGaussians *g, SgrAlloc geom_alloc,
+                             void *geom_ctx, SgrAlloc binning_alloc, void *binning_ctx, SgrAlloc image_alloc,
+                             void *image_ctx, float *out_color, int32_t *radii, int64_t capacity_hint,
+                             int64_t *num_rendered, void *stream, const FeatureChannel *feat)
+{
+    int rc = validate(view, g, true);
+    if (rc) return rc;
+    if (!out_color || !num_rendered || !geom_alloc || !binning_alloc || !image_alloc || (feat && !feat->out)) {
+        set_error("null output / allocator");
+        return SGR_EINVAL;
+    }
+    if (feat && g->activations != 0) {
+        set_error("%s: raw-parameter mode is not supported", who);
+        return SGR_EINVAL;
+    }
+    *num_rendered = 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t npix = (size_t)view->image_width * view->image_height;
+    if (g->P == 0) {
+        SGR_CUDA(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * npix, st));
+        if (feat) SGR_CUDA(cudaMemsetAsync(feat->out, 0, sizeof(float) * npix, st));
+        return SGR_OK;
+    }
+    if (!radii || (feat && (!feat->values || !feat->bg))) {
+        set_error(feat ? "radii / values / feature_bg must be non-null" : "radii must be non-null");
+        return SGR_EINVAL;
+    }
+    return launch_forward(view, g, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, out_color,
+                          radii, capacity_hint, num_rendered, st, feat);
+}
+
+// The plain / staged and the feature backward (feat != NULL): argument checks, P == 0 launches nothing.  The feature
+// adds only its own pointers and its rejection of raw-parameter mode.
+static int rasterize_backward(const char *who, const SgrView *view, const SgrGaussians *g, const int32_t *radii,
+                              const void *geom_buffer, const void *binning_buffer, const void *image_buffer,
+                              int64_t num_rendered, const float *dL_dout_color, float *dL_dmeans2D, float *dL_dcolors,
+                              float *dL_dopacity, float *dL_dmeans3D, float *dL_dcov3D, float *dL_dsh,
+                              float *dL_dscales, float *dL_drotations, void *grad_scratch, void *stream,
+                              const SgrBackwardPlan *plan, const FeatureChannel *feat)
+{
+    int rc = validate(view, g, false);
+    if (rc) return rc;
+    if (feat && g->activations != 0) {
+        set_error("%s: raw-parameter mode is not supported", who);
+        return SGR_EINVAL;
+    }
+    if (g->P == 0) return SGR_OK;
+    const bool records = plan && plan->reduce_records;
+    if (!radii || !geom_buffer || !binning_buffer || !image_buffer || !dL_dout_color || !dL_dmeans2D || !dL_dcolors ||
+        !dL_dcov3D || !grad_scratch || (!records && (!dL_dopacity || !dL_dmeans3D || !dL_dscales || !dL_drotations)) ||
+        (feat && (!feat->values || !feat->bg || !feat->dL_dout || !feat->dL_dvalues))) {
+        set_error("null pointer passed to %s", who);
+        return SGR_EINVAL;
+    }
+    return launch_backward(view, g, radii, geom_buffer, binning_buffer, image_buffer, num_rendered, dL_dout_color,
+                           dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
+                           dL_drotations, grad_scratch, (cudaStream_t)stream, plan, feat);
 }
 
 __global__ void fill_background_kernel(int W, int H, const float *__restrict__ bg, float *__restrict__ out)
@@ -288,24 +374,8 @@ int sgr_rasterize_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc g
                           SgrAlloc binning_alloc, void *binning_ctx, SgrAlloc image_alloc, void *image_ctx,
                           float *out_color, int32_t *radii, int64_t capacity_hint, int64_t *num_rendered, void *stream)
 {
-    int rc = validate(view, g, true);
-    if (rc) return rc;
-    if (!out_color || !num_rendered || !geom_alloc || !binning_alloc || !image_alloc) {
-        set_error("null output / allocator");
-        return SGR_EINVAL;
-    }
-    *num_rendered = 0;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (g->P == 0) {  // rasterize_points.cu:81: nothing is launched, outputs stay at their zero fill
-        SGR_CUDA(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * (size_t)view->image_width * view->image_height, st));
-        return SGR_OK;
-    }
-    if (!radii) {
-        set_error("radii must be non-null");
-        return SGR_EINVAL;
-    }
-    return launch_forward(view, g, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, out_color,
-                          radii, capacity_hint, num_rendered, st, nullptr);
+    return rasterize_forward("sgr_rasterize_forward", view, g, geom_alloc, geom_ctx, binning_alloc, binning_ctx,
+                             image_alloc, image_ctx, out_color, radii, capacity_hint, num_rendered, stream, nullptr);
 }
 
 int sgr_rasterize_forward_feature(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_alloc, void *geom_ctx,
@@ -313,31 +383,9 @@ int sgr_rasterize_forward_feature(const SgrView *view, const SgrGaussians *g, Sg
                                   const float *values, const float *feature_bg, float *out_color, float *out_feature,
                                   int32_t *radii, int64_t capacity_hint, int64_t *num_rendered, void *stream)
 {
-    int rc = validate(view, g, true);
-    if (rc) return rc;
-    if (!out_color || !out_feature || !num_rendered || !geom_alloc || !binning_alloc || !image_alloc) {
-        set_error("null output / allocator");
-        return SGR_EINVAL;
-    }
-    if (g->activations != 0) {
-        set_error("sgr_rasterize_forward_feature: raw-parameter mode is not supported");
-        return SGR_EINVAL;
-    }
-    *num_rendered = 0;
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t npix = (size_t)view->image_width * view->image_height;
-    if (g->P == 0) {
-        SGR_CUDA(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * npix, st));
-        SGR_CUDA(cudaMemsetAsync(out_feature, 0, sizeof(float) * npix, st));
-        return SGR_OK;
-    }
-    if (!radii || !values || !feature_bg) {
-        set_error("radii / values / feature_bg must be non-null");
-        return SGR_EINVAL;
-    }
     const FeatureChannel feat = {values, feature_bg, out_feature, nullptr, nullptr};
-    return launch_forward(view, g, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, out_color,
-                          radii, capacity_hint, num_rendered, st, &feat);
+    return rasterize_forward("sgr_rasterize_forward_feature", view, g, geom_alloc, geom_ctx, binning_alloc, binning_ctx,
+                             image_alloc, image_ctx, out_color, radii, capacity_hint, num_rendered, stream, &feat);
 }
 
 int sgr_rasterize_backward_staged(const SgrView *view, const SgrGaussians *g, const int32_t *radii, const void *geom_buffer,
@@ -346,18 +394,9 @@ int sgr_rasterize_backward_staged(const SgrView *view, const SgrGaussians *g, co
                            float *dL_dmeans3D, float *dL_dcov3D, float *dL_dsh, float *dL_dscales,
                            float *dL_drotations, void *grad_scratch, void *stream, const SgrBackwardPlan *plan)
 {
-    int rc = validate(view, g, false);
-    if (rc) return rc;
-    if (g->P == 0) return SGR_OK;
-    const bool records = plan && plan->reduce_records;
-    if (!radii || !geom_buffer || !binning_buffer || !image_buffer || !dL_dout_color || !dL_dmeans2D || !dL_dcolors ||
-        !dL_dcov3D || !grad_scratch || (!records && (!dL_dopacity || !dL_dmeans3D || !dL_dscales || !dL_drotations))) {
-        set_error("null pointer passed to sgr_rasterize_backward");
-        return SGR_EINVAL;
-    }
-    return launch_backward(view, g, radii, geom_buffer, binning_buffer, image_buffer, num_rendered, dL_dout_color,
-                           dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
-                           dL_drotations, grad_scratch, (cudaStream_t)stream, plan, nullptr);
+    return rasterize_backward("sgr_rasterize_backward", view, g, radii, geom_buffer, binning_buffer, image_buffer,
+                              num_rendered, dL_dout_color, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D,
+                              dL_dsh, dL_dscales, dL_drotations, grad_scratch, stream, plan, nullptr);
 }
 
 int sgr_rasterize_backward_feature(const SgrView *view, const SgrGaussians *g, const int32_t *radii,
@@ -368,23 +407,11 @@ int sgr_rasterize_backward_feature(const SgrView *view, const SgrGaussians *g, c
                                    float *dL_dsh, float *dL_dscales, float *dL_drotations, float *dL_dvalues,
                                    void *grad_scratch, void *stream)
 {
-    int rc = validate(view, g, false);
-    if (rc) return rc;
-    if (g->activations != 0) {
-        set_error("sgr_rasterize_backward_feature: raw-parameter mode is not supported");
-        return SGR_EINVAL;
-    }
-    if (g->P == 0) return SGR_OK;
-    if (!radii || !geom_buffer || !binning_buffer || !image_buffer || !dL_dout_color || !values || !feature_bg ||
-        !dL_dout_feature || !dL_dmeans2D || !dL_dcolors || !dL_dopacity || !dL_dmeans3D || !dL_dcov3D ||
-        !dL_dscales || !dL_drotations || !dL_dvalues || !grad_scratch) {
-        set_error("null pointer passed to sgr_rasterize_backward_feature");
-        return SGR_EINVAL;
-    }
     const FeatureChannel feat = {values, feature_bg, nullptr, dL_dout_feature, dL_dvalues};
-    return launch_backward(view, g, radii, geom_buffer, binning_buffer, image_buffer, num_rendered, dL_dout_color,
-                           dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
-                           dL_drotations, grad_scratch, (cudaStream_t)stream, nullptr, &feat);
+    return rasterize_backward("sgr_rasterize_backward_feature", view, g, radii, geom_buffer, binning_buffer,
+                              image_buffer, num_rendered, dL_dout_color, dL_dmeans2D, dL_dcolors, dL_dopacity,
+                              dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations, grad_scratch, stream, nullptr,
+                              &feat);
 }
 
 int sgr_rasterize_backward(const SgrView *view, const SgrGaussians *g, const int32_t *radii, const void *geom_buffer,

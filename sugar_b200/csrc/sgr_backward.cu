@@ -1301,25 +1301,57 @@ static void chunk_blocks(int blocks, int nchunks, int c, int taper, int *b0, int
     *b1 = c + 1 == nchunks ? blocks : edge(c + 1);
 }
 
-template <bool FEAT>
-static void launch_blend_backward(const SgrView *view, int P, const ImageState &img, const BinState &bin,
+static int set_backward_attributes()
+{
+    SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)BWD_SMEM_BYTES));
+    SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)BWD_SMEM_BYTES));
+    SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)BWD_SMEM_BYTES_FEAT));
+    SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)BWD_SMEM_BYTES_FEAT));
+    SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  200 * 1024));
+    SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  200 * 1024));
+    SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  200 * 1024));
+    return SGR_OK;
+}
+static DeviceOnce g_backward_attributes;
+
+// The events that order the peer exchange's launches on the plan's signal stream (side = 0) and side stream (side = 1)
+// behind earlier work, per device and launch index, created on first use and kept.
+static int peer_event(int side, int index, cudaEvent_t *out)
+{
+    static std::mutex mu;
+    static cudaEvent_t evs[SGR_MAX_DEVICES][2][20] = {};
+    int dev = 0;
+    const int rc = current_device(&dev);
+    if (rc) return rc;
+    if (index < 0 || index >= 20) {
+        set_error("%s: chunk index out of range", side ? "peer_side_stream" : "peer_signal_stream");
+        return SGR_EINVAL;
+    }
+    std::lock_guard<std::mutex> lock(mu);
+    cudaEvent_t *ev = &evs[dev][side][index];
+    if (!*ev) SGR_CUDA(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    *out = *ev;
+    return SGR_OK;
+}
+
+static void launch_blend_backward(const ViewConsts &v, int P, const ImageState &img, const BinState &bin,
                                   const GeomState &geom, const float *dL_dout_color, float *gacc, float *dL_dcolors,
                                   const FeatureChannel *feat, cudaStream_t st)
 {
-    const int W = view->image_width, H = view->image_height;
-    const int gx = (W + SGR_TILE - 1) / SGR_TILE, gy = (H + SGR_TILE - 1) / SGR_TILE;
-    const uint32_t smem = FEAT ? BWD_SMEM_BYTES_FEAT : BWD_SMEM_BYTES;
-    const float *values = FEAT ? feat->values : nullptr, *feat_bg = FEAT ? feat->bg : nullptr;
-    const float *dL_dfeat = FEAT ? feat->dL_dout : nullptr;
-    float *dval = FEAT ? feat->dL_dvalues : nullptr;
-    if (ids_packed(P))
-        blend_backward_kernel<true, FEAT><<<gx * gy, 256, smem, st>>>(
-            img.tile_order, img.tile_start, bin.plist, geom.rec, W, H, gx, view->bg, img.final_T, img.n_contrib,
-            dL_dout_color, gacc, dL_dcolors, values, feat_bg, dL_dfeat, dval);
-    else
-        blend_backward_kernel<false, FEAT><<<gx * gy, 256, smem, st>>>(
-            img.tile_order, img.tile_start, bin.plist, geom.rec, W, H, gx, view->bg, img.final_T, img.n_contrib,
-            dL_dout_color, gacc, dL_dcolors, values, feat_bg, dL_dfeat, dval);
+    const bool packed = ids_packed(P);
+    const auto kernel = feat ? (packed ? &blend_backward_kernel<true, true> : &blend_backward_kernel<false, true>)
+                             : (packed ? &blend_backward_kernel<true, false> : &blend_backward_kernel<false, false>);
+    kernel<<<v.gx * v.gy, 256, feat ? BWD_SMEM_BYTES_FEAT : BWD_SMEM_BYTES, st>>>(
+        img.tile_order, img.tile_start, bin.plist, geom.rec, v.W, v.H, v.gx, v.bg, img.final_T, img.n_contrib,
+        dL_dout_color, gacc, dL_dcolors, feat ? feat->values : nullptr, feat ? feat->bg : nullptr,
+        feat ? feat->dL_dout : nullptr, feat ? feat->dL_dvalues : nullptr);
 }
 
 int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *radii, const void *geom_buffer,
@@ -1329,7 +1361,6 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
                     void *grad_scratch, cudaStream_t st, const SgrBackwardPlan *plan, const FeatureChannel *feat)
 {
     const int P = g->P, W = view->image_width, H = view->image_height;
-    const int gx = (W + SGR_TILE - 1) / SGR_TILE, gy = (H + SGR_TILE - 1) / SGR_TILE;
     GeomState geom = GeomState::carve((void *)geom_buffer, P);
     ImageState img = ImageState::carve((void *)image_buffer, W, H);
     BinState bin = BinState::carve((void *)binning_buffer, (size_t)num_rendered);
@@ -1337,41 +1368,15 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     const SgrStageHook hook = plan ? plan->hook : nullptr;
     void *hook_ctx = plan ? plan->hook_ctx : nullptr;
     float *rec11 = plan ? plan->reduce_records : nullptr;
-    {
-        // opt in to > 48 KB of dynamic shared memory once per device (the call is not free); calls
-        // may come from several threads (autograd engine threads of different devices)
-        static std::mutex mu;
-        static bool attr_set[64] = {};
-        int dev = 0;
-        SGR_CUDA(cudaGetDevice(&dev));
-        std::lock_guard<std::mutex> lock(mu);
-        if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true, false>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<false, false>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true, true>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES_FEAT));
-            SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<false, true>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES_FEAT));
-            SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          200 * 1024));
-            SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          200 * 1024));
-            SGR_CUDA(cudaFuncSetAttribute(preprocess_backward_kernel<false, true>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            if (dev >= 0 && dev < 64) attr_set[dev] = true;
-        }
-    }
+    const ViewConsts v = view_consts(view, g->M);
+    int rc = once_per_device(g_backward_attributes, set_backward_attributes);
+    if (rc) return rc;
     // the blend accumulators: 32 B per Gaussian of scratch + the dL_dcolors output itself
     SGR_CUDA(cudaMemsetAsync(gacc, 0, (size_t)P * 32, st));
     SGR_CUDA(cudaMemsetAsync(dL_dcolors, 0, (size_t)P * 12, st));
     if (feat) SGR_CUDA(cudaMemsetAsync(feat->dL_dvalues, 0, (size_t)P * 4, st));
-    if (num_rendered > 0) {
-        SGR_LAUNCH(K_BLEND_BWD, st,
-                   if (feat) launch_blend_backward<true>(view, P, img, bin, geom, dL_dout_color, gacc, dL_dcolors, feat, st);
-                   else launch_blend_backward<false>(view, P, img, bin, geom, dL_dout_color, gacc, dL_dcolors, feat, st));
-    }
+    if (num_rendered > 0)
+        SGR_LAUNCH(K_BLEND_BWD, st, launch_blend_backward(v, P, img, bin, geom, dL_dout_color, gacc, dL_dcolors, feat, st));
     // dL_dcolors is final here (with SH colours: the clamp-masked dL/dRGB, i.e. this view's SH factor)
     if (hook) hook(hook_ctx, SGR_STAGE_BLEND_DONE);
     const bool peer = plan && plan->peer_flag_tab;
@@ -1380,26 +1385,19 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     auto signal = [&](int slot, int ev_index, bool on_main = false) -> int {
         cudaStream_t sig = st;
         if (plan->peer_signal_stream && !on_main) {
-            static std::mutex mu;
-            static cudaEvent_t evs[64][20] = {};
-            int dev = 0;
-            SGR_CUDA(cudaGetDevice(&dev));
-            if (dev < 0 || dev >= 64 || ev_index < 0 || ev_index >= 20) {
-                set_error("peer_signal_stream: device / chunk index out of range");
-                return SGR_EINVAL;
-            }
-            std::lock_guard<std::mutex> lock(mu);
-            if (!evs[dev][ev_index]) SGR_CUDA(cudaEventCreateWithFlags(&evs[dev][ev_index], cudaEventDisableTiming));
+            cudaEvent_t ev = nullptr;
+            const int rc = peer_event(0, ev_index, &ev);
+            if (rc) return rc;
             sig = (cudaStream_t)plan->peer_signal_stream;
-            SGR_CUDA(cudaEventRecord(evs[dev][ev_index], st));
-            SGR_CUDA(cudaStreamWaitEvent(sig, evs[dev][ev_index], 0));
+            SGR_CUDA(cudaEventRecord(ev, st));
+            SGR_CUDA(cudaStreamWaitEvent(sig, ev, 0));
         }
         return sgr_peer_signal(plan->peer_flag_tab, plan->peer_nranks, slot, plan->peer_rank, plan->peer_seq, sig);
     };
     if (peer) {
         // BLEND goes out on `st` itself: the wait right behind it spins, and a spinning kernel must never be dispatched
         // ahead of a signal of its own rank that the peers need in order to answer
-        int rc = signal(plan->peer_slot_blend, 0, true);
+        rc = signal(plan->peer_slot_blend, 0, true);
         if (rc) return rc;
         if (plan->peer_view_blocks && dL_dsh && g->shs) {
             // the per-Gaussian pass sums every view's SH gradient into dL_dsh: the peers' factor blocks must be final
@@ -1419,22 +1417,7 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     a.shs = g->shs;
     a.cov_pre = g->cov3D_precomp;
     a.sh_jac = geom.sh_jac;
-    a.v.viewmatrix = view->viewmatrix;
-    a.v.projmatrix = view->projmatrix;
-    a.v.campos = view->campos;
-    a.v.bg = view->bg;
-    a.v.W = W;
-    a.v.H = H;
-    a.v.gx = gx;
-    a.v.gy = gy;
-    a.v.tanfovx = view->tanfovx;
-    a.v.tanfovy = view->tanfovy;
-    a.v.focal_y = H / (2.0f * view->tanfovy);
-    a.v.focal_x = W / (2.0f * view->tanfovx);
-    a.v.scale_modifier = view->scale_modifier;
-    a.v.D = view->sh_degree;
-    a.v.M = g->M;
-    a.v.prefiltered = view->prefiltered;
+    a.v = v;
     a.radii = radii;
     a.gacc = gacc;
     a.dcol = dL_dcolors;
@@ -1471,26 +1454,19 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
         set_error("raw-parameter mode needs SgrBackwardPlan.dL_dsh_rest");
         return SGR_EINVAL;
     }
-    auto al16 = [](const void *p) { return ((uintptr_t)p & 15u) == 0; };
     // (the SH arrays are not read; sh_jac is 256-byte aligned by GeomState::carve)
-    a.in_bulk_ok = al16(gacc) && al16(dL_dcolors) && al16(g->means3D) && (!g->scales || al16(g->scales)) &&
-                   (!g->rotations || al16(g->rotations)) && (!g->cov3D_precomp || al16(g->cov3D_precomp));
-    a.out_bulk_ok = al16(dL_dmeans2D) && al16(dL_dcov3D) &&
-                    (rec11 ? al16(rec11) : (al16(dL_dopacity) && al16(dL_dmeans3D) && al16(dL_dscales) && al16(dL_drotations)));
-    if (raw && g->shs && dL_dsh) a.out_bulk_ok = a.out_bulk_ok && al16(dL_dsh) && (g->M == 1 || al16(a.dsh_rest));
+    a.in_bulk_ok = aligned16(gacc) && aligned16(dL_dcolors) && aligned16(g->means3D) &&
+                   (!g->scales || aligned16(g->scales)) && (!g->rotations || aligned16(g->rotations)) &&
+                   (!g->cov3D_precomp || aligned16(g->cov3D_precomp));
+    a.out_bulk_ok = aligned16(dL_dmeans2D) && aligned16(dL_dcov3D) &&
+                    (rec11 ? aligned16(rec11)
+                           : (aligned16(dL_dopacity) && aligned16(dL_dmeans3D) && aligned16(dL_dscales) &&
+                              aligned16(dL_drotations)));
+    if (raw && g->shs && dL_dsh)
+        a.out_bulk_ok = a.out_bulk_ok && aligned16(dL_dsh) && (g->M == 1 || aligned16(a.dsh_rest));
     a.sh_stride = 0;
     a.sh_vec = 0;
-    if (g->shs && !raw) {
-        const int row_f = g->M * 3;
-        if ((row_f % 4) == 0 && al16(dL_dsh)) {  // rows leave as 16-byte stores
-            int s4 = row_f / 4;
-            if ((s4 & 1) == 0) s4 += 1;
-            a.sh_stride = s4 * 4;
-            a.sh_vec = 1;
-        } else {
-            a.sh_stride = (row_f & 1) ? row_f : row_f + 1;
-        }
-    }
+    if (g->shs && !raw) a.sh_stride = sh_row_stride(g->M, aligned16(dL_dsh), &a.sh_vec);  // rows leave as 16-byte stores
     // the SH block: dL/dsh rows, and before them the Jacobian rows (9 floats per Gaussian, M = 1 has shorter rows)
     int sh_block = raw ? (g->M > 0 ? (g->M - 1) * 3 : 0) : a.sh_stride;
     if (g->shs && sh_block < 9) sh_block = 9;
@@ -1503,20 +1479,8 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     const int blocks = (P + PB_T - 1) / PB_T;
     if (nchunks > blocks) nchunks = blocks;
     int split_c = -1, split_p0 = 0, split_p1 = 0;
-    auto side_event = [&](int index, cudaEvent_t *out) -> int {
-        static std::mutex mu;
-        static cudaEvent_t evs[64][20] = {};
-        int dev = 0;
-        SGR_CUDA(cudaGetDevice(&dev));
-        if (dev < 0 || dev >= 64 || index < 0 || index >= 20) {
-            set_error("peer_side_stream: device / chunk index out of range");
-            return SGR_EINVAL;
-        }
-        std::lock_guard<std::mutex> lock(mu);
-        if (!evs[dev][index]) SGR_CUDA(cudaEventCreateWithFlags(&evs[dev][index], cudaEventDisableTiming));
-        *out = evs[dev][index];
-        return SGR_OK;
-    };
+    const auto preprocess = raw ? &preprocess_backward_kernel<true>
+                                : a.view_tab ? &preprocess_backward_kernel<false, true> : &preprocess_backward_kernel<false>;
     auto split_chunk = [&](cudaStream_t B, int c, int p0, int p1) -> int {
         int rc = sgr_peer_wait(plan->peer_flags, plan->peer_nranks, plan->peer_slot_reduced0 + c, 1, plan->peer_seq,
                                plan->peer_timeout_s, B);
@@ -1537,11 +1501,7 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
         chunk_blocks(blocks, nchunks, c, plan ? plan->chunk_taper : 0, &b0, &b1);
         a.p0 = b0 * PB_T;
         a.p1 = min(P, b1 * PB_T);
-        if (b1 > b0)
-            SGR_LAUNCH(K_PRE_BWD, st,
-                       if (raw) preprocess_backward_kernel<true><<<b1 - b0, PB_T, dyn, st>>>(a);
-                       else if (a.view_tab) preprocess_backward_kernel<false, true><<<b1 - b0, PB_T, dyn, st>>>(a);
-                       else preprocess_backward_kernel<false><<<b1 - b0, PB_T, dyn, st>>>(a));
+        if (b1 > b0) SGR_LAUNCH(K_PRE_BWD, st, preprocess<<<b1 - b0, PB_T, dyn, st>>>(a));
         if (hook) hook(hook_ctx, SGR_STAGE_CHUNK_DONE + c);
         if (peer) {
             int rc = signal(plan->peer_slot_chunk0 + c, 1 + c);
@@ -1553,7 +1513,7 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
                 cudaStream_t B = (cudaStream_t)plan->peer_side_stream;
                 cudaStream_t sig = plan->peer_signal_stream ? (cudaStream_t)plan->peer_signal_stream : st;
                 cudaEvent_t e2 = nullptr;
-                rc = side_event(c, &e2);
+                rc = peer_event(1, c, &e2);
                 if (rc) return rc;
                 SGR_CUDA(cudaEventRecord(e2, sig));
                 SGR_CUDA(cudaStreamWaitEvent(B, e2, 0));

@@ -1139,8 +1139,7 @@ __global__ void mark_visible_kernel(int P, const float *__restrict__ means, cons
 // ------------------------------------------------------------------------------------------------
 // Host-side per-call state: one pinned word (the instance count's read-back) and one event.  Calls
 // may overlap on one device (two streams / two threads), so every call takes its own slot from a small
-// per-device pool and returns it when it is done; the one-time function attributes are set under the
-// same lock.
+// per-device pool and returns it when it is done.
 struct CallSlot {
     uint32_t *pinned = nullptr;
     cudaEvent_t ev = nullptr;
@@ -1148,18 +1147,14 @@ struct CallSlot {
 struct DevicePool {
     std::mutex mu;
     std::vector<CallSlot> free_slots;
-    bool attrs_set = false;
 };
-static DevicePool g_pools[64];
+static DevicePool g_pools[SGR_MAX_DEVICES];
 
 static int current_pool(DevicePool **out)
 {
     int dev = 0;
-    SGR_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64) {
-        set_error("device ordinal %d out of range", dev);
-        return SGR_EINVAL;
-    }
+    const int rc = current_device(&dev);
+    if (rc) return rc;
     *out = &g_pools[dev];
     return SGR_OK;
 }
@@ -1167,13 +1162,6 @@ static int current_pool(DevicePool **out)
 static int acquire_slot(DevicePool *pool, CallSlot *slot)
 {
     std::lock_guard<std::mutex> lock(pool->mu);
-    if (!pool->attrs_set) {
-        SGR_CUDA(cudaFuncSetAttribute(preprocess_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        SGR_CUDA(cudaFuncSetAttribute(preprocess_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        SGR_CUDA(cudaFuncSetAttribute(tile_sort_merge_kernel<8192, 2048>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
-        pool->attrs_set = true;
-    }
     if (!pool->free_slots.empty()) {
         *slot = pool->free_slots.back();
         pool->free_slots.pop_back();
@@ -1196,26 +1184,27 @@ struct SlotLease {  // returns the slot to its pool on every exit path
     }
 };
 
-static inline bool aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
+static int set_forward_attributes()
+{
+    SGR_CUDA(cudaFuncSetAttribute(preprocess_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    SGR_CUDA(cudaFuncSetAttribute(preprocess_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    SGR_CUDA(cudaFuncSetAttribute(tile_sort_merge_kernel<8192, 2048>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  8192 * 8));
+    return SGR_OK;
+}
+static DeviceOnce g_forward_attributes;
 
-template <bool FEAT>
 static void launch_blend_forward(const ViewConsts &v, int P, const GeomState &geom, const ImageState &img,
                                  const BinState &bin, uint64_t capacity, float *out_color, const FeatureChannel *feat,
                                  cudaStream_t st)
 {
-    const int T = v.gx * v.gy;
-    const float *values = FEAT ? feat->values : nullptr, *feat_bg = FEAT ? feat->bg : nullptr;
-    float *out_feature = FEAT ? feat->out : nullptr;
-    if (ids_packed(P))
-        blend_forward_kernel<true, FEAT><<<T, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec,
-                                                                img.counters, capacity, v.W, v.H, v.gx, v.bg,
-                                                                img.final_T, img.n_contrib, out_color, values, feat_bg,
-                                                                out_feature);
-    else
-        blend_forward_kernel<false, FEAT><<<T, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec,
-                                                                 img.counters, capacity, v.W, v.H, v.gx, v.bg,
-                                                                 img.final_T, img.n_contrib, out_color, values, feat_bg,
-                                                                 out_feature);
+    const bool packed = ids_packed(P);
+    const auto kernel = feat ? (packed ? &blend_forward_kernel<true, true> : &blend_forward_kernel<false, true>)
+                             : (packed ? &blend_forward_kernel<true, false> : &blend_forward_kernel<false, false>);
+    kernel<<<v.gx * v.gy, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec, img.counters, capacity,
+                                            v.W, v.H, v.gx, v.bg, img.final_T, img.n_contrib, out_color,
+                                            feat ? feat->values : nullptr, feat ? feat->bg : nullptr,
+                                            feat ? feat->out : nullptr);
 }
 
 static int launch_binning_and_blend(const ViewConsts &v, int P, const GeomState &geom, const ImageState &img,
@@ -1239,9 +1228,7 @@ static int launch_binning_and_blend(const ViewConsts &v, int P, const GeomState 
     SGR_LAUNCH(K_SORT_GLOBAL, st,
                tile_sort_global_kernel<<<small_grid, GSORT_T, 0, st>>>(img.tile_start, img.counters, capacity,
                                                                        bin.inst_a, bin.inst_b, bin.plist, T));
-    SGR_LAUNCH(K_BLEND_FWD, st,
-               if (feat) launch_blend_forward<true>(v, P, geom, img, bin, capacity, out_color, feat, st);
-               else launch_blend_forward<false>(v, P, geom, img, bin, capacity, out_color, feat, st));
+    SGR_LAUNCH(K_BLEND_FWD, st, launch_blend_forward(v, P, geom, img, bin, capacity, out_color, feat, st));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }
@@ -1252,30 +1239,16 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
                    const FeatureChannel *feat)
 {
     const int P = g->P, W = view->image_width, H = view->image_height;
+    int rc = once_per_device(g_forward_attributes, set_forward_attributes);
+    if (rc) return rc;
     SlotLease lease;
-    int rc = current_pool(&lease.pool);
+    rc = current_pool(&lease.pool);
     if (rc) return rc;
     rc = acquire_slot(lease.pool, &lease.slot);
     if (rc) return rc;
     CallSlot *slot = &lease.slot;
 
-    ViewConsts v;
-    v.viewmatrix = view->viewmatrix;
-    v.projmatrix = view->projmatrix;
-    v.campos = view->campos;
-    v.bg = view->bg;
-    v.W = W;
-    v.H = H;
-    v.gx = (W + SGR_TILE - 1) / SGR_TILE;
-    v.gy = (H + SGR_TILE - 1) / SGR_TILE;
-    v.tanfovx = view->tanfovx;
-    v.tanfovy = view->tanfovy;
-    v.focal_y = H / (2.0f * view->tanfovy);  // rasterizer_impl.cu:222-223
-    v.focal_x = W / (2.0f * view->tanfovx);
-    v.scale_modifier = view->scale_modifier;
-    v.D = view->sh_degree;
-    v.M = g->M;
-    v.prefiltered = view->prefiltered;
+    const ViewConsts v = view_consts(view, g->M);
     const int T = v.gx * v.gy;
 
     void *geom_mem = geom_alloc(geom_ctx, GeomState::bytes(P));
@@ -1311,23 +1284,14 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
     if (g->shs && raw) {
         dyn = (size_t)PRE_T * (g->M - 1) * 3 * sizeof(float) + 16;  // rows of the `rest` block, unpadded
     } else if (g->shs) {
-        const int row_f = g->M * 3;
-        if ((row_f % 4) == 0 && aligned16(g->shs)) {
-            int s4 = row_f / 4;
-            if ((s4 & 1) == 0) s4 += 1;  // odd number of 16-byte units per row: conflict-free LDS
-            a.sh_stride = s4 * 4;
-            a.sh_vec = 1;
-        } else {
-            a.sh_stride = (row_f & 1) ? row_f : row_f + 1;
-        }
+        a.sh_stride = sh_row_stride(g->M, aligned16(g->shs), &a.sh_vec);
         dyn = (size_t)PRE_T * a.sh_stride * sizeof(float);
     }
     a.geom = geom;
     a.radii = radii;
     a.tile_count = img.tile_count;
-    SGR_LAUNCH(K_PREPROCESS, st,
-               if (raw) preprocess_kernel<true><<<(P + PRE_T - 1) / PRE_T, PRE_T, dyn, st>>>(a);
-               else preprocess_kernel<false><<<(P + PRE_T - 1) / PRE_T, PRE_T, dyn, st>>>(a));
+    const auto preprocess = raw ? &preprocess_kernel<true> : &preprocess_kernel<false>;
+    SGR_LAUNCH(K_PREPROCESS, st, preprocess<<<(P + PRE_T - 1) / PRE_T, PRE_T, dyn, st>>>(a));
     SGR_LAUNCH(K_TILE_SCAN, st,
                tile_scan_kernel<<<1, 1024, 0, st>>>(img.tile_count, img.tile_start, img.tile_cursor, img.tile_order,
                                                     img.counters, T, nullptr));

@@ -102,9 +102,8 @@ struct BinState {
     }
 };
 
-// Per-view constants passed by value (constant bank): the two matrices are read once on the
-// host side of the launch from device memory?  No: they stay device pointers in the reference
-// API, so kernels load them through the read-only path (16+16+3+3 floats, L1-resident).
+// Per-view constants passed by value (constant bank).  The matrices, camera position and background stay device
+// pointers, as in the reference API: kernels load them through the read-only path (16+16+3+3 floats, L1-resident).
 struct ViewConsts {
     const float *viewmatrix;
     const float *projmatrix;
@@ -116,9 +115,59 @@ struct ViewConsts {
     int prefiltered;
 };
 
+static inline ViewConsts view_consts(const SgrView *view, int M)
+{
+    ViewConsts v;
+    v.viewmatrix = view->viewmatrix;
+    v.projmatrix = view->projmatrix;
+    v.campos = view->campos;
+    v.bg = view->bg;
+    v.W = view->image_width;
+    v.H = view->image_height;
+    v.gx = (v.W + SGR_TILE - 1) / SGR_TILE;
+    v.gy = (v.H + SGR_TILE - 1) / SGR_TILE;
+    v.tanfovx = view->tanfovx;
+    v.tanfovy = view->tanfovy;
+    v.focal_y = v.H / (2.0f * view->tanfovy);  // rasterizer_impl.cu:222-223
+    v.focal_x = v.W / (2.0f * view->tanfovx);
+    v.scale_modifier = view->scale_modifier;
+    v.D = view->sh_degree;
+    v.M = M;
+    v.prefiltered = view->prefiltered;
+    return v;
+}
+
+static inline bool aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
+
+// Row stride in floats of the per-Gaussian passes' shared-memory SH rows (M coefficients x 3): an odd number of
+// 16-byte units when the rows can move as 16-byte copies (`vec_ok`: the global rows are 16-byte aligned), else an
+// odd number of floats -- conflict-free either way.  *vec = 1 selects the 16-byte copies.
+static inline int sh_row_stride(int M, bool vec_ok, int *vec)
+{
+    const int row_f = M * 3;
+    *vec = (row_f % 4) == 0 && vec_ok;
+    if (*vec) {
+        int s4 = row_f / 4;
+        if ((s4 & 1) == 0) s4 += 1;
+        return s4 * 4;
+    }
+    return (row_f & 1) ? row_f : row_f + 1;
+}
+
 void set_error(const char *fmt, ...);
 int cuda_fail(cudaError_t e, const char *what);
 int device_sm_count();  // SMs of the current device (grid sizes of the grid-stride kernels)
+
+// Per-device host state (slot pools, one-time set-up, events) is kept in tables of SGR_MAX_DEVICES entries.
+#define SGR_MAX_DEVICES 64
+int current_device(int *dev);  // the current device, or SGR_EINVAL if it is beyond SGR_MAX_DEVICES
+// One-time set-up per device, e.g. opting a kernel in to > 48 KB of dynamic shared memory (the call is not free).
+// once_per_device runs init() under a lock the first time it is called with `once` on the current device; calls may
+// come from several threads (autograd engine threads of different devices).  A failed init() is retried next time.
+struct DeviceOnce {
+    bool done[SGR_MAX_DEVICES];
+};
+int once_per_device(DeviceOnce &once, int (*init)());
 
 // Kernel bookkeeping: every launch of one of OUR kernels goes through SGR_LAUNCH so that
 // sgr_launch_count() is a measured number and, when profiling is switched on, each launch is

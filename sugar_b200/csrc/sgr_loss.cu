@@ -302,7 +302,13 @@ int sgr_l1_ssim_forward(const SgrSsimParams *p, const float *img1, const float *
     cudaStream_t st = (cudaStream_t)stream;
     const LossConsts k = loss_consts(p);
     double2 *partials = (double2 *)align_up((size_t)scratch);
-    SGR_CUDA(cudaFuncSetAttribute(loss_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LOSS_FWD_SMEM));
+    static DeviceOnce attributes;
+    rc = once_per_device(attributes, []() -> int {
+        SGR_CUDA(cudaFuncSetAttribute(loss_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)LOSS_FWD_SMEM));
+        return SGR_OK;
+    });
+    if (rc) return rc;
     SGR_LAUNCH(K_LOSS_FWD, st,
                loss_forward_kernel<<<g.grid, dim3(32, L_THREADS / 32), LOSS_FWD_SMEM, st>>>(
                    k, img1, img2, partial_maps, (size_t)g.n_total, partials));

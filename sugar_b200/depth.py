@@ -22,13 +22,15 @@ carries a fourth channel.
   its trainers stop densifying before the depth render starts.
 * A gradient of None for the image or the depth counts as zero.
 
-Raw-parameter mode (fused.py) and use under a view-parallel exchange (parallel.py) are not supported; the latter
-raises NotImplementedError, since the exchange sums only the rasterizer's own gradients.
+The op is `_C.rasterize_gaussians` / `_C.rasterize_gaussians_backward` with the keyword `values` (the C entry points
+sgr_rasterize_forward_feature / sgr_rasterize_backward_feature).  Raw-parameter mode (fused.py) and use under a
+view-parallel exchange (parallel.py) are not supported; the latter raises NotImplementedError, since the exchange sums
+only the rasterizer's own gradients.
 """
 import torch
 
 from . import _C
-from .diff_gaussian_rasterization import _call_with_dump
+from .diff_gaussian_rasterization import _call_with_dump, _optional_inputs
 
 
 class _RasterizeWithDepth(torch.autograd.Function):
@@ -39,10 +41,11 @@ class _RasterizeWithDepth(torch.autograd.Function):
         bg1 = depth_bg.detach().reshape(1)
         args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
                 rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh,
-                rs.sh_degree, rs.campos, rs.prefiltered, rs.debug, point_values, bg1)
+                rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
         ctx.sgr_context = _C.current_context()
-        num_rendered, color, depth, radii, geom, binning, img = _call_with_dump(
-            _C.rasterize_gaussians_feature, args, rs.debug, "snapshot_fw.dump", "forward", context=ctx.sgr_context)
+        num_rendered, color, radii, geom, binning, img, depth = _call_with_dump(
+            _C.rasterize_gaussians, args, rs.debug, "snapshot_fw.dump", "forward", context=ctx.sgr_context,
+            values=point_values, feature_bg=bg1)
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geom, binning,
@@ -66,10 +69,10 @@ class _RasterizeWithDepth(torch.autograd.Function):
             grad_depth = torch.zeros((H, W), dtype=torch.float32, device=dev)
         args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
                 rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_color, sh, rs.sh_degree, rs.campos,
-                geom, ctx.num_rendered, binning, img, rs.debug, point_values, bg1, grad_depth)
+                geom, ctx.num_rendered, binning, img, rs.debug)
         (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_scales, g_rotations, g_values) = \
-            _call_with_dump(_C.rasterize_gaussians_feature_backward, args, rs.debug, "snapshot_bw.dump", "backward",
-                            context=ctx.sgr_context)
+            _call_with_dump(_C.rasterize_gaussians_backward, args, rs.debug, "snapshot_bw.dump", "backward",
+                            context=ctx.sgr_context, values=point_values, feature_bg=bg1, dL_dout_feature=grad_depth)
         return (g_means3D, g_means2D, g_sh, g_colors, g_opacities, g_scales, g_rotations, g_cov3D, g_values, None,
                 None)
 
@@ -77,21 +80,12 @@ class _RasterizeWithDepth(torch.autograd.Function):
 def rasterize_with_depth(means3D, means2D, opacities, point_values, raster_settings, depth_bg, shs=None,
                          colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None):
     """-> (image [3,H,W], depth [H,W], radii [P]); see the module docstring."""
-    if (shs is None) == (colors_precomp is None):
-        raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-    has_sr = scales is not None or rotations is not None
-    if ((scales is None or rotations is None) and cov3D_precomp is None) or (has_sr and cov3D_precomp is not None):
-        raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+    shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales, rotations,
+                                                                             cov3D_precomp)
     P = means3D.shape[0]
     if point_values.numel() != P or (point_values.dim() == 2 and point_values.shape[1] != 1) or point_values.dim() > 2:
         raise ValueError(f"point_values must be [P] or [P,1] with P = {P}, got {tuple(point_values.shape)}")
     if not torch.is_tensor(depth_bg) or depth_bg.numel() != 1:
         raise ValueError("depth_bg must be a one-element tensor")
-    absent = torch.Tensor([])
-    shs = absent if shs is None else shs
-    colors_precomp = absent if colors_precomp is None else colors_precomp
-    scales = absent if scales is None else scales
-    rotations = absent if rotations is None else rotations
-    cov3D_precomp = absent if cov3D_precomp is None else cov3D_precomp
     return _RasterizeWithDepth.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                      cov3D_precomp, point_values.reshape(P), depth_bg, raster_settings)

@@ -36,15 +36,28 @@ class GaussianRasterizationSettings(NamedTuple):
     debug: bool
 
 
+def _optional_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp):
+    """The reference's "exactly one of" checks (:191-195); absent optionals then travel as empty tensors, as in the
+    reference (:197-206).  -> (shs, colors_precomp, scales, rotations, cov3D_precomp)"""
+    if (shs is None) == (colors_precomp is None):
+        raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+    has_sr = scales is not None or rotations is not None
+    if ((scales is None or rotations is None) and cov3D_precomp is None) or (has_sr and cov3D_precomp is not None):
+        raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+    absent = torch.Tensor([])
+    return tuple(absent if t is None else t for t in (shs, colors_precomp, scales, rotations, cov3D_precomp))
+
+
 def _snapshot(args):
     """debug=True keeps a CPU copy of the arguments so a failing call can be dumped (reference :17-19)."""
     return tuple(a.detach().cpu().clone() if isinstance(a, torch.Tensor) else a for a in args)
 
 
 def _call_with_dump(fn, args, debug, dump_name, what, **kw):
+    """fn(*args, **kw); with debug, a failing call dumps `args` followed by the keyword tensors."""
     if not debug:
         return fn(*args, **kw)
-    saved = _snapshot(args)
+    saved = _snapshot(args + tuple(v for v in kw.values() if isinstance(v, torch.Tensor)))
     try:
         return fn(*args, **kw)
     except Exception:
@@ -111,17 +124,7 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
-        if (shs is None) == (colors_precomp is None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        has_sr = scales is not None or rotations is not None
-        if ((scales is None or rotations is None) and cov3D_precomp is None) or (has_sr and cov3D_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
-        # absent optionals travel as empty tensors, as in the reference (:197-206)
-        absent = torch.Tensor([])
-        shs = absent if shs is None else shs
-        colors_precomp = absent if colors_precomp is None else colors_precomp
-        scales = absent if scales is None else scales
-        rotations = absent if rotations is None else rotations
-        cov3D_precomp = absent if cov3D_precomp is None else cov3D_precomp
+        shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales,
+                                                                                 rotations, cov3D_precomp)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                    cov3D_precomp, self.raster_settings)

@@ -242,16 +242,15 @@ class ViewParallel:
         return True
 
     # -- the exchange, driven from _C.rasterize_gaussians_backward ------------------------------------------
-    def run_backward(self, lib, check, stage_hook_type, plan_type, args, bufs, P, M, degree, means3D, campos,
-                     has_cov_precomp):
-        """`args`: the positional arguments of sgr_rasterize_backward_staged without the trailing plan;
-        `bufs`: dict of the gradient tensors + "records" f32[P,11].  Returns nothing: bufs hold the reduced
-        gradients when the enqueued work completes."""
+    def run_backward(self, launch, bufs, P, M, degree, means3D, campos, has_cov_precomp):
+        """`launch(plan, *, dL_dcolors=ptr, dL_dsh=ptr)` enqueues this view's sgr_rasterize_backward_staged under
+        `plan`, with the two gradient outputs optionally redirected; `bufs`: dict of the gradient tensors +
+        "records" f32[P,11].  Returns nothing: bufs hold the reduced gradients when the enqueued work completes."""
+        from ._lib import STAGE_HOOK, SgrBackwardPlan, check, lib
         if self.uses_peer_memory(M, has_cov_precomp):
             st = self._peer_state(lib, check, P, means3D.device)
             if st is not None:
-                return self._run_backward_peer(st, lib, check, stage_hook_type, plan_type, args, bufs, P, M, degree,
-                                               means3D, campos)
+                return self._run_backward_peer(st, launch, bufs, P, means3D, campos)
         if "records" not in bufs:   # "auto" just fell back to the NCCL exchange: the arena was sized for peer mode
             bufs["records"] = torch.empty((P, 11), dtype=torch.float32, device=means3D.device)
         world = _world(self.group)
@@ -303,10 +302,10 @@ class ViewParallel:
             except BaseException as e:  # never unwind through the C frame
                 failure.append(e)
 
-        cb = stage_hook_type(on_stage)
-        plan = plan_type(cb, None, nchunks, bufs["records"].data_ptr(), None)
+        cb = STAGE_HOOK(on_stage)
+        plan = SgrBackwardPlan(cb, None, nchunks, bufs["records"].data_ptr(), None)
         plan.chunk_taper = taper
-        check(lib.sgr_rasterize_backward_staged(*args, C.byref(plan)))
+        launch(plan)
         if failure:
             raise failure[0]
         main = torch.cuda.current_stream(dev)
@@ -366,7 +365,8 @@ class ViewParallel:
             self._peer_states[key] = st
         return self._peer_states[key]
 
-    def _run_backward_peer(self, st, lib, check, stage_hook_type, plan_type, args, bufs, P, M, degree, means3D, campos):
+    def _run_backward_peer(self, st, launch, bufs, P, means3D, campos):
+        from ._lib import STAGE_HOOK, SgrBackwardPlan
         dev = means3D.device
         world, rank = st.world, st.rank
         nchunks = max(1, self.chunks)
@@ -377,25 +377,24 @@ class ViewParallel:
         B, Csig, ev = st.streams(dev)
         F = st.F_local[par]
         F[3 * P:3 * P + 3].copy_(campos.reshape(3))     # the camera position rides behind the factors
-        args = list(args)
-        args[9] = F.data_ptr()       # dL_dcolors: the blend pass accumulates straight into the peer-visible factor block
-        args[13] = bufs["sh"].data_ptr()                 # dL_dsh: written by the per-Gaussian pass, summed over ALL views
         # main stream, all inside the C call: blend -> signal(BLEND) -> wait(BLEND, every rank) -> per-Gaussian pass in
         # chunks: TMA-loads the other ranks' factor blocks over NVLink, writes the summed dL_dsh, TMA-stores each CTA's
         # 44-byte records into the staging array of the rank that owns them -> signal(CHUNK c) after each chunk
         emulate = 0
         for r in self._emulated:
             emulate |= 1 << r
-        plan = plan_type(stage_hook_type(0), None, nchunks, st.R_ptr, None, st.flag_tab.data_ptr(), world, rank,
-                         _SLOT_BLEND, _SLOT_CHUNK0, seq, st.F_tab[par].data_ptr(), st.flags_ptr, self.scale,
-                         self.peer_timeout_s, taper, st.stage_tab.data_ptr(),
-                         Csig.cuda_stream, B.cuda_stream, st.rec_tab.data_ptr(),
-                         st.S_tab.data_ptr(), st.S_ptr, _SLOT_REDUCED0, emulate)
+        plan = SgrBackwardPlan(STAGE_HOOK(0), None, nchunks, st.R_ptr, None, st.flag_tab.data_ptr(), world, rank,
+                               _SLOT_BLEND, _SLOT_CHUNK0, seq, st.F_tab[par].data_ptr(), st.flags_ptr, self.scale,
+                               self.peer_timeout_s, taper, st.stage_tab.data_ptr(),
+                               Csig.cuda_stream, B.cuda_stream, st.rec_tab.data_ptr(),
+                               st.S_tab.data_ptr(), st.S_ptr, _SLOT_REDUCED0, emulate)
         # ... and on the side stream, also enqueued by the C call, chunk by chunk underneath the per-Gaussian pass of the
         # later chunks: [wait(CHUNK c, every rank) -> sum the slice this rank owns over the staging arrays (local loads)
         # -> store the sums into every rank's S (posted NVLink writes) -> signal(REDUCED c)] as ONE kernel, then behind
         # the next chunk's reduce: wait(REDUCED c) -> split S into the four gradient arrays (x scale)
-        check(lib.sgr_rasterize_backward_staged(*args, C.byref(plan)))
+        # dL_dcolors: the blend pass accumulates straight into the peer-visible factor block; dL_dsh: written by the
+        # per-Gaussian pass, summed over ALL views
+        launch(plan, dL_dcolors=F.data_ptr(), dL_dsh=bufs["sh"].data_ptr())
         main.wait_stream(B)
         main.wait_stream(Csig)
         self.stats["backwards"] += 1
