@@ -272,6 +272,37 @@ __global__ void inspect_bin_kernel(int T, int packed, const uint32_t *__restrict
     }
 }
 
+// n_contrib of the blend kernels counts positions in the tile's LIVE list (dead instances left out); the reference
+// counts the entries of the full list up to its last contributor.  The last contributor is the same instance in both,
+// so its position in the full sorted segment -- found by (depth bits, id), the sort key -- plus one is the reference's.
+__global__ void inspect_n_contrib_kernel(int W, int H, int gx, int packed, const uint32_t *__restrict__ tile_start,
+                                         const uint32_t *__restrict__ live, const uint32_t *__restrict__ full,
+                                         const float *__restrict__ depth, const uint32_t *__restrict__ n_live,
+                                         uint32_t *__restrict__ n_ref)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= W * H) return;
+    const uint32_t n = n_live[i];
+    uint32_t out = 0;
+    if (n) {
+        const int x = i % W, y = i / W, t = (y / SGR_TILE) * gx + x / SGR_TILE;
+        const uint32_t lo = tile_start[t], hi = tile_start[t + 1];
+        const auto key = [&](uint32_t w) {
+            const uint32_t id = packed ? (w >> 8) : w;
+            return ((uint64_t)__float_as_uint(depth[id]) << 32) | id;
+        };
+        const uint64_t k = key(live[lo + n - 1]);
+        uint32_t a = lo, b = hi;  // first position of [lo, hi) whose key is not below k
+        while (a < b) {
+            const uint32_t m = (a + b) >> 1;
+            if (key(full[m]) < k) a = m + 1;
+            else b = m;
+        }
+        out = a - lo + 1;
+    }
+    n_ref[i] = out;
+}
+
 __global__ void mark_visible_kernel(int P, const float *__restrict__ means, const float *__restrict__ vm,
                                     uint8_t *__restrict__ present);  // sgr_forward.cu
 
@@ -456,15 +487,45 @@ int sgr_inspect_state(int32_t P, int32_t width, int32_t height, int64_t num_rend
     const int T = ((width + 15) / 16) * ((height + 15) / 16);
     inspect_geom_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, geom, nullptr, depths, means2D, conic_opacity, rgb, clamped,
                                                          tiles_touched);
-    if (binning_buffer && (keys || point_list || ranges || footprint)) {
-        BinState bin = BinState::carve((void *)binning_buffer, (size_t)num_rendered);
-        inspect_bin_kernel<<<T, 128, 0, st>>>(T, ids_packed(P) ? 1 : 0, img.tile_start, bin.plist, geom.depth, keys,
-                                              point_list, ranges, footprint);
-    }
     const size_t npix = (size_t)width * height;
     if (final_T) SGR_CUDA(cudaMemcpyAsync(final_T, img.final_T, npix * 4, cudaMemcpyDeviceToDevice, st));
-    if (n_contrib) SGR_CUDA(cudaMemcpyAsync(n_contrib, img.n_contrib, npix * 4, cudaMemcpyDeviceToDevice, st));
-    SGR_CUDA(cudaGetLastError());
+    if (num_rendered == 0) {
+        if (n_contrib) SGR_CUDA(cudaMemsetAsync(n_contrib, 0, npix * 4, st));
+        SGR_CUDA(cudaGetLastError());
+        return SGR_OK;
+    }
+    if (!(keys || point_list || ranges || footprint || n_contrib)) {
+        SGR_CUDA(cudaGetLastError());
+        return SGR_OK;
+    }
+    if (!binning_buffer) {
+        set_error("sgr_inspect_state: the list and n_contrib need the binning buffer");
+        return SGR_EINVAL;
+    }
+    // The forward kept only the live instances; the reference's list (dead ones included, with their masks) is
+    // rebuilt here in scratch of its own by the forward's scatter and sorts.  A diagnostic path: it allocates.
+    const int gx = (width + 15) / 16;
+    const size_t R = (size_t)num_rendered, cursor_bytes = align_up((size_t)T * 4);
+    void *mem = nullptr;
+    SGR_CUDA(cudaMallocAsync(&mem, cursor_bytes + BinState::bytes(R) + SGR_ALIGN, st));
+    uint32_t *cursor = (uint32_t *)align_up((size_t)mem);
+    const BinState full = BinState::carve((char *)cursor + cursor_bytes, R);
+    const BinState live = BinState::carve((void *)binning_buffer, R);
+    const int packed = ids_packed(P) ? 1 : 0;
+    int rc = build_full_list(P, width, height, geom, img, R, full, cursor, st);
+    if (rc == SGR_OK) {
+        if (keys || point_list || ranges || footprint)
+            inspect_bin_kernel<<<T, 128, 0, st>>>(T, packed, img.tile_start, full.plist, geom.depth, keys, point_list,
+                                                  ranges, footprint);
+        if (n_contrib)
+            inspect_n_contrib_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(
+                width, height, gx, packed, img.tile_start, live.plist, full.plist, geom.depth, img.n_contrib, n_contrib);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) rc = cuda_fail(e, "sgr_inspect_state");
+    }
+    const cudaError_t ef = cudaFreeAsync(mem, st);
+    if (rc) return rc;
+    SGR_CUDA(ef);
     return SGR_OK;
 }
 

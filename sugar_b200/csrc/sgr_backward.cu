@@ -199,15 +199,16 @@ __device__ __forceinline__ void chunk_flush(uint32_t cb, int nf, float blk_x0, f
 // dL_dfeat[H,W] in, dL/dvalues into dval[P]; the FEAT = false instantiations ignore the last four arguments.
 template <bool packed, bool FEAT>
 __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
-    const uint32_t *__restrict__ tile_order, const uint32_t *__restrict__ tile_start, const uint32_t *__restrict__ plist,
-    const float4 *__restrict__ rec, int W, int H, int gx, const float *__restrict__ bg,
+    const uint32_t *__restrict__ tile_order, const uint32_t *__restrict__ tile_start, const uint32_t *__restrict__ tile_end,
+    const uint32_t *__restrict__ plist, const float4 *__restrict__ rec, int W, int H, int gx, const float *__restrict__ bg,
     const float *__restrict__ final_Ts, const uint32_t *__restrict__ n_contrib, const float *__restrict__ dL_dpixels,
     float *__restrict__ gacc, float *__restrict__ dcol, const float *__restrict__ values,
     const float *__restrict__ feat_bg, const float *__restrict__ dL_dfeat, float *__restrict__ dval)
 {
     extern __shared__ __align__(16) unsigned char s_raw[];
     const int tile = (int)tile_order[blockIdx.x];
-    const uint32_t lo = tile_start[tile], hi = tile_start[tile + 1];
+    // the forward's live list of the tile; n_contrib counts positions in it
+    const uint32_t lo = tile_start[tile], hi = tile_end[tile];
     if (hi == lo) return;
     const int tile_y = tile / gx, tile_x = tile - tile_y * gx;
     const int tid = threadIdx.x;
@@ -263,10 +264,9 @@ __global__ void __launch_bounds__(256, 4) blend_backward_kernel(
     // record pipeline (threads 0..BWD_B-1 own one slot of every batch)
     const bool loader = tid < BWD_B;
     auto fetch = [&](int b0) -> uint32_t {
-        // back to front; dead instances (packed list, empty footprint) are dropped here: 0xffffffff
+        // back to front; 0xffffffff: no slot (the live list holds no dead instance: scatter left them out)
         if (!(loader && b0 + tid < n)) return 0xffffffffu;
-        const uint32_t w = plist[lo + (uint32_t)(n - 1 - (b0 + tid))];
-        return (packed && (w & 0xffu) == 0u) ? 0xffffffffu : w;
+        return plist[lo + (uint32_t)(n - 1 - (b0 + tid))];
     };
     // membership words of the batch in stage `st` from the loader threads' masks
     auto publish_members = [&](uint32_t mask, uint32_t(*set)[BWD_B / 32]) {
@@ -1349,8 +1349,8 @@ static void launch_blend_backward(const ViewConsts &v, int P, const ImageState &
     const auto kernel = feat ? (packed ? &blend_backward_kernel<true, true> : &blend_backward_kernel<false, true>)
                              : (packed ? &blend_backward_kernel<true, false> : &blend_backward_kernel<false, false>);
     kernel<<<v.gx * v.gy, 256, feat ? BWD_SMEM_BYTES_FEAT : BWD_SMEM_BYTES, st>>>(
-        img.tile_order, img.tile_start, bin.plist, geom.rec, v.W, v.H, v.gx, v.bg, img.final_T, img.n_contrib,
-        dL_dout_color, gacc, dL_dcolors, feat ? feat->values : nullptr, feat ? feat->bg : nullptr,
+        img.tile_order, img.tile_start, img.tile_cursor, bin.plist, geom.rec, v.W, v.H, v.gx, v.bg, img.final_T,
+        img.n_contrib, dL_dout_color, gacc, dL_dcolors, feat ? feat->values : nullptr, feat ? feat->bg : nullptr,
         feat ? feat->dL_dout : nullptr, feat ? feat->dL_dvalues : nullptr);
 }
 

@@ -386,7 +386,9 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
 // Also orders the tiles by decreasing instance count (counting sort on count / 8, 1024 classes): the
 // blend kernels take their tile from this list, so the hardware's in-order block dispatch starts the
 // heaviest tiles first and the tail of the grid consists of the lightest ones (longest-processing-time
-// -first; the order within a class is arbitrary and has no effect on any result).
+// -first; the order within a class is arbitrary and has no effect on any result).  The weights are the full
+// counts, dead instances included: the live counts are only known after scatter, and the order is a schedule
+// that no result depends on.
 __global__ void __launch_bounds__(1024) tile_scan_kernel(const uint32_t *__restrict__ count, uint32_t *__restrict__ start,
                                                          uint32_t *__restrict__ cursor, uint32_t *__restrict__ order,
                                                          uint32_t *__restrict__ counters, int T, uint32_t *host_mirror)
@@ -473,11 +475,18 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(const uint32_t *__restr
 }
 
 // ------------------------------------------------------------------------------------------------
-// scatter: one (depth | id [| footprint mask]) word per (Gaussian, tile) instance into its tile's segment.
-// The kernel is bound by the round trip of its returning atomics (one slot claim per instance), so the
-// arithmetic it does while they are in flight is free: this is where the exact footprint mask of every
+// scatter: one (depth | id [| footprint mask]) word per LIVE (Gaussian, tile) instance into its tile's
+// segment.  The kernel is bound by the round trip of its returning atomics (one slot claim per instance), so
+// the arithmetic it does while they are in flight is free: this is where the exact footprint mask of every
 // instance (sgr_internal.cuh, block_mask) is computed -- once, for both blend kernels.
+// An instance whose mask is 0 cannot reach any pixel of its tile (the masks are conservative), so it claims
+// no slot: the live words of tile t fill [tile_start[t], cursor[t]) and the rest of the segment, which
+// preprocess sized by the full count, stays unused.  The sorts and both blend kernels walk the live range only.
+// The plain-id format (packed = 0) carries no mask in the word but computes it all the same, to drop the dead.
+// KEEP_DEAD: every instance claims its slot (cursor[t] ends at tile_start[t + 1]): the reference's full list,
+// rebuilt by sgr_inspect_state.
 // ------------------------------------------------------------------------------------------------
+template <bool KEEP_DEAD>
 __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushort4 *__restrict__ rect,
                                                       const float *__restrict__ depth, const float4 *__restrict__ rec,
                                                       uint32_t *__restrict__ cursor,
@@ -496,10 +505,8 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushor
         rc = rect[idx];
         if (rc.z > rc.x && rc.w > rc.y) {
             dbits = __float_as_uint(depth[idx]);
-            if (packed) {
-                const float4 r0 = __ldg(rec + (size_t)idx * 3), r1 = __ldg(rec + (size_t)idx * 3 + 1);
-                eb = ellipse_bands(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y);
-            }
+            const float4 r0 = __ldg(rec + (size_t)idx * 3), r1 = __ldg(rec + (size_t)idx * 3 + 1);
+            eb = ellipse_bands(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y);
         }
     }
     // Rects of up to SMALL tiles are walked by their own thread: masks first (pure arithmetic), then all
@@ -509,9 +516,10 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushor
     static_assert(SMALL <= 8, "masks of a small rect are packed into one 64-bit register");
     const int rw = (int)rc.z - (int)rc.x, rcnt = (rc.z > rc.x && rc.w > rc.y) ? rw * ((int)rc.w - (int)rc.y) : 0;
     const uint32_t low_id = packed ? ((uint32_t)idx << 8) : (uint32_t)idx;
+    const uint32_t word_mask = packed ? 0xffu : 0u;  // the mask rides in the word only in the packed format
     if (rcnt > 0 && rcnt <= SMALL) {
         uint64_t masks = 0;
-        if (packed && !eb.dead) {
+        if (!eb.dead) {
             // the columns a band reaches do not depend on the tile column: once per tile row, then every
             // tile of the row only compares its two 8-column halves with them
             int k = 0;
@@ -548,7 +556,7 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushor
 #pragma unroll
         for (int k = 0; k < SMALL; k++) {
             if (k < rcnt) {
-                slot[k] = atomicAdd(cursor + trow + tx, 1u);
+                if (KEEP_DEAD || ((masks >> (8 * k)) & 0xffu)) slot[k] = atomicAdd(cursor + trow + tx, 1u);
                 if (++tx == rw) {
                     tx = 0;
                     trow += gx;
@@ -556,8 +564,10 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushor
             }
         }
 #pragma unroll
-        for (int k = 0; k < SMALL; k++)
-            if (k < rcnt) inst[slot[k]] = ((uint64_t)dbits << 32) | low_id | (uint32_t)((masks >> (8 * k)) & 0xffu);
+        for (int k = 0; k < SMALL; k++) {
+            const uint32_t m = (uint32_t)(masks >> (8 * k)) & 0xffu;
+            if (k < rcnt && (KEEP_DEAD || m)) inst[slot[k]] = ((uint64_t)dbits << 32) | low_id | (m & word_mask);
+        }
     }
     unsigned todo = __ballot_sync(0xffffffffu, rcnt > SMALL);
     while (todo) {
@@ -580,9 +590,10 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, int gx, const ushor
         es.dead = __shfl_sync(0xffffffffu, (int)eb.dead, src) != 0;
         for (int k = lane; k < cnt; k += 32) {
             const int ty = k / w, tx = k - ty * w;
-            const uint32_t m = packed ? block_mask(es, (rx0 + tx) * SGR_TILE, (ry0 + ty) * SGR_TILE) : 0u;
+            const uint32_t m = block_mask(es, (rx0 + tx) * SGR_TILE, (ry0 + ty) * SGR_TILE);
+            if (!KEEP_DEAD && m == 0u) continue;
             const uint32_t slot = atomicAdd(cursor + (ry0 + ty) * gx + rx0 + tx, 1u);
-            inst[slot] = ((uint64_t)db << 32) | lid | m;
+            inst[slot] = ((uint64_t)db << 32) | lid | (m & word_mask);
         }
     }
 }
@@ -596,6 +607,7 @@ constexpr int SORT_CAP = 8192;  // largest shared-memory (merge sort) class; abo
 constexpr int GSORT_T = 1024;
 
 __global__ void __launch_bounds__(GSORT_T) tile_sort_global_kernel(const uint32_t *__restrict__ tile_start,
+                                                                   const uint32_t *__restrict__ tile_end,
                                                                    const uint32_t *__restrict__ counters,
                                                                    uint64_t capacity, uint64_t *__restrict__ inst_a,
                                                                    uint64_t *__restrict__ inst_b,
@@ -610,7 +622,7 @@ __global__ void __launch_bounds__(GSORT_T) tile_sort_global_kernel(const uint32_
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const uint32_t lo = tile_start[tile];
-    const int n = (int)(tile_start[tile + 1] - lo);
+    const int n = (int)(tile_end[tile] - lo);
     if (n <= SORT_CAP) continue;
 
     uint64_t *src = inst_a + lo, *dst = inst_b + lo;
@@ -714,7 +726,8 @@ __global__ void __launch_bounds__(GSORT_T) tile_sort_global_kernel(const uint32_
 // merge-path binary search and merges 8 outputs serially.  The words are distinct (the id is part
 // of the key) so the result is the unique total order = the reference's stable sort by depth.
 // Size classes (LOWER, CAP]: each class is its own launch over all tiles with early exit, so the
-// shared-memory footprint (and occupancy) matches the tile population.
+// shared-memory footprint (and occupancy) matches the tile population.  Every sort kernel sorts the
+// words of [tile_start[t], tile_end[t]) -- the live instances scatter wrote -- and picks its class by that count.
 // ------------------------------------------------------------------------------------------------
 constexpr int SORT_VT = 8;  // words per thread in the per-tile merge sort
 
@@ -795,6 +808,7 @@ __device__ __forceinline__ void block_merge_sort(uint64_t *s_keys, const int n)
 
 template <int CAP, int LOWER>
 __global__ void __launch_bounds__(CAP / SORT_VT) tile_sort_merge_kernel(const uint32_t *__restrict__ tile_start,
+                                                                        const uint32_t *__restrict__ tile_end,
                                                                         const uint32_t *__restrict__ counters,
                                                                         uint64_t capacity,
                                                                         const uint64_t *__restrict__ inst,
@@ -806,7 +820,7 @@ __global__ void __launch_bounds__(CAP / SORT_VT) tile_sort_merge_kernel(const ui
     // grid-stride over tiles: rare size classes are launched with a small grid and skip cheaply
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const uint32_t lo = tile_start[tile];
-        const int n = (int)(tile_start[tile + 1] - lo);
+        const int n = (int)(tile_end[tile] - lo);
         if (n <= LOWER || n > CAP) continue;
         for (int i = tid; i < n; i += CAP / SORT_VT) s_keys[i] = inst[lo + i];
         __syncthreads();
@@ -830,6 +844,7 @@ __global__ void __launch_bounds__(CAP / SORT_VT) tile_sort_merge_kernel(const ui
 constexpr int BK_CAP = 2048, BK_T = 256, BK_NB = 1024, BK_LOG2NB = 10, BUCKET_MAX = 24;
 
 __global__ void __launch_bounds__(BK_T) tile_sort_bucket_kernel(const uint32_t *__restrict__ tile_start,
+                                                                 const uint32_t *__restrict__ tile_end,
                                                                  const uint32_t *__restrict__ counters, uint64_t capacity,
                                                                  const uint64_t *__restrict__ inst,
                                                                  uint32_t *__restrict__ plist, int num_tiles, int lower)
@@ -844,7 +859,7 @@ __global__ void __launch_bounds__(BK_T) tile_sort_bucket_kernel(const uint32_t *
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const uint32_t lo = tile_start[tile];
-        const int n = (int)(tile_start[tile + 1] - lo);
+        const int n = (int)(tile_end[tile] - lo);
         if (n <= lower || n > BK_CAP) continue;
         if (tid == 0) {
             s_red[0] = 0xffffffffu;
@@ -933,13 +948,14 @@ __global__ void __launch_bounds__(BK_T) tile_sort_bucket_kernel(const uint32_t *
 
 // ------------------------------------------------------------------------------------------------
 // forward blend: one CTA per 16x16 tile, one thread per pixel, one warp per 8x4 pixel block
-// (block w = band * 2 + half, sgr_internal.cuh).  The records of a batch of the tile's list are
-// gathered once into shared memory -- only those whose footprint mask is not empty: a third of the
-// instances are dead in their tile -- and each warp walks only the splats whose mask has its block's
+// (block w = band * 2 + half, sgr_internal.cuh).  The records of a batch of the tile's live list
+// [tile_start, tile_end) are gathered once into shared memory -- the dead instances (empty footprint mask, a
+// third of them) never entered the list -- and each warp walks only the splats whose mask has its block's
 // bit (clz over a bit-reversed per-block membership word).  power / alpha / T / C follow the reference's rounding
-// exactly (forward.cu:261-374), so final_T, n_contrib and the image are bit-identical to the
-// reference; the masks and the `power < tau` test only skip pairs the exact alpha test would reject.
-// Tiles are taken heaviest first (tile_order).
+// exactly (forward.cu:261-374), so final_T and the image are bit-identical to the reference; the masks and the
+// `power < tau` test only skip pairs the exact alpha test would reject.  n_contrib is the last contributor's
+// position + 1 in the LIVE list (the backward bounds its walk by it; sgr_inspect_state maps it back to the
+// reference's count over the full list).  Tiles are taken heaviest first (tile_order).
 // ------------------------------------------------------------------------------------------------
 constexpr int BLEND_T = 256;
 
@@ -965,6 +981,7 @@ __device__ __forceinline__ uint32_t low_mask(uint32_t n)
 template <bool packed, bool FEAT>
 __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *__restrict__ tile_order,
                                                                 const uint32_t *__restrict__ tile_start,
+                                                                const uint32_t *__restrict__ tile_end,
                                                                 const uint32_t *__restrict__ plist,
                                                                 const float4 *__restrict__ rec,
                                                                 const uint32_t *__restrict__ counters, uint64_t capacity,
@@ -993,7 +1010,7 @@ __global__ void __launch_bounds__(BLEND_T) blend_forward_kernel(const uint32_t *
     const uint32_t pxi = tx0 + (wid & 1u) * 8 + (lane & 7u), pyi = ty0 + (wid >> 1) * 4 + (lane >> 3);
     const bool inside = pxi < (uint32_t)W && pyi < (uint32_t)H;
     const float pxf = (float)pxi, pyf = (float)pyi;
-    const uint32_t lo = tile_start[tile], hi = tile_start[tile + 1];
+    const uint32_t lo = tile_start[tile], hi = tile_end[tile];  // the tile's live list (scatter)
     uint32_t done = inside ? 0u : 1u;  // 32-bit flag: a bool makes nvcc shuffle bytes (PRMT) in the hot loop
     float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, C3 = 0.f;
     uint32_t last = 0;
@@ -1201,36 +1218,63 @@ static void launch_blend_forward(const ViewConsts &v, int P, const GeomState &ge
     const bool packed = ids_packed(P);
     const auto kernel = feat ? (packed ? &blend_forward_kernel<true, true> : &blend_forward_kernel<false, true>)
                              : (packed ? &blend_forward_kernel<true, false> : &blend_forward_kernel<false, false>);
-    kernel<<<v.gx * v.gy, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, bin.plist, geom.rec, img.counters, capacity,
-                                            v.W, v.H, v.gx, v.bg, img.final_T, img.n_contrib, out_color,
-                                            feat ? feat->values : nullptr, feat ? feat->bg : nullptr,
+    kernel<<<v.gx * v.gy, BLEND_T, 0, st>>>(img.tile_order, img.tile_start, img.tile_cursor, bin.plist, geom.rec,
+                                            img.counters, capacity, v.W, v.H, v.gx, v.bg, img.final_T, img.n_contrib,
+                                            out_color, feat ? feat->values : nullptr, feat ? feat->bg : nullptr,
                                             feat ? feat->out : nullptr);
+}
+
+// scatter (into bin.inst_a, advancing `cursor` from tile_start) and the per-tile sorts of [tile_start, cursor)
+// into bin.plist.  KEEP_DEAD: the full list of the reference instead of the live one.
+template <bool KEEP_DEAD>
+static int launch_scatter_and_sorts(int P, int gx, int T, const GeomState &geom, const uint32_t *tile_start,
+                                    uint32_t *cursor, const uint32_t *counters, const BinState &bin, uint64_t capacity,
+                                    cudaStream_t st)
+{
+    SGR_LAUNCH(K_SCATTER, st,
+               scatter_kernel<KEEP_DEAD><<<(P + 255) / 256, 256, 0, st>>>(P, gx, geom.rect, geom.depth, geom.rec, cursor,
+                                                                          counters, capacity, ids_packed(P) ? 1 : 0,
+                                                                          bin.inst_a));
+    sgr::prof_begin(K_SORT_SMEM, st);  // one timing bracket around the three size classes ...
+    sgr::note_launches(2);             // ... but three launches
+    const int slots = 2 * device_sm_count();
+    const int small_grid = T < slots ? T : slots;  // 2 CTAs per SM, grid-stride over tiles
+    tile_sort_merge_kernel<512, 0><<<T, 512 / SORT_VT, 512 * 8, st>>>(tile_start, cursor, counters, capacity, bin.inst_a,
+                                                                      bin.plist, T);
+    tile_sort_bucket_kernel<<<T, BK_T, 0, st>>>(tile_start, cursor, counters, capacity, bin.inst_a, bin.plist, T, 512);
+    tile_sort_merge_kernel<8192, 2048><<<small_grid, 8192 / SORT_VT, 8192 * 8, st>>>(tile_start, cursor, counters,
+                                                                                     capacity, bin.inst_a, bin.plist, T);
+    sgr::prof_end(st);
+    SGR_LAUNCH(K_SORT_GLOBAL, st,
+               tile_sort_global_kernel<<<small_grid, GSORT_T, 0, st>>>(tile_start, cursor, counters, capacity,
+                                                                       bin.inst_a, bin.inst_b, bin.plist, T));
+    SGR_CUDA(cudaGetLastError());
+    return SGR_OK;
 }
 
 static int launch_binning_and_blend(const ViewConsts &v, int P, const GeomState &geom, const ImageState &img,
                                     const BinState &bin, uint64_t capacity, float *out_color,
                                     const FeatureChannel *feat, cudaStream_t st)
 {
-    const int T = v.gx * v.gy;
-    SGR_LAUNCH(K_SCATTER, st,
-               scatter_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, v.gx, geom.rect, geom.depth, geom.rec, img.tile_cursor,
-                                                               img.counters, capacity, ids_packed(P) ? 1 : 0, bin.inst_a));
-    sgr::prof_begin(K_SORT_SMEM, st);  // one timing bracket around the three size classes ...
-    sgr::note_launches(2);             // ... but three launches
-    const int slots = 2 * device_sm_count();
-    const int small_grid = T < slots ? T : slots;  // 2 CTAs per SM, grid-stride over tiles
-    tile_sort_merge_kernel<512, 0><<<T, 512 / SORT_VT, 512 * 8, st>>>(img.tile_start, img.counters, capacity, bin.inst_a,
-                                                                      bin.plist, T);
-    tile_sort_bucket_kernel<<<T, BK_T, 0, st>>>(img.tile_start, img.counters, capacity, bin.inst_a, bin.plist, T, 512);
-    tile_sort_merge_kernel<8192, 2048><<<small_grid, 8192 / SORT_VT, 8192 * 8, st>>>(img.tile_start, img.counters,
-                                                                                     capacity, bin.inst_a, bin.plist, T);
-    sgr::prof_end(st);
-    SGR_LAUNCH(K_SORT_GLOBAL, st,
-               tile_sort_global_kernel<<<small_grid, GSORT_T, 0, st>>>(img.tile_start, img.counters, capacity,
-                                                                       bin.inst_a, bin.inst_b, bin.plist, T));
+    const int rc = launch_scatter_and_sorts<false>(P, v.gx, v.gx * v.gy, geom, img.tile_start, img.tile_cursor,
+                                                   img.counters, bin, capacity, st);
+    if (rc) return rc;
+    // the blend reads the live ends scatter left in tile_cursor (same stream, after it)
     SGR_LAUNCH(K_BLEND_FWD, st, launch_blend_forward(v, P, geom, img, bin, capacity, out_color, feat, st));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
+}
+
+// The reference's full per-tile list of a forward's state, dead instances included, into `full` (capacity
+// num_rendered): tile_start[t + 1] ends each segment, `cursor` (T words) is scratch.  sgr_inspect_state.
+int build_full_list(int P, int W, int H, const GeomState &geom, const ImageState &img, uint64_t num_rendered,
+                    const BinState &full, uint32_t *cursor, cudaStream_t st)
+{
+    int rc = once_per_device(g_forward_attributes, set_forward_attributes);
+    if (rc) return rc;
+    const int gx = (W + SGR_TILE - 1) / SGR_TILE, T = gx * ((H + SGR_TILE - 1) / SGR_TILE);
+    SGR_CUDA(cudaMemcpyAsync(cursor, img.tile_start, sizeof(uint32_t) * T, cudaMemcpyDeviceToDevice, st));
+    return launch_scatter_and_sorts<true>(P, gx, T, geom, img.tile_start, cursor, img.counters, full, num_rendered, st);
 }
 
 int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_alloc, void *geom_ctx,

@@ -55,7 +55,7 @@ struct ImageState {
     uint32_t *n_contrib;
     uint32_t *tile_count;
     uint32_t *tile_start;  // T+1
-    uint32_t *tile_cursor;
+    uint32_t *tile_cursor;  // after scatter: the end of each tile's live list [tile_start[t], tile_cursor[t])
     uint32_t *tile_order;  // tiles by decreasing instance count: launch order of the blend kernels
     uint32_t *counters;    // [0] = num_rendered, [1] = overflow flag
     static size_t bytes(size_t W, size_t H)
@@ -552,5 +552,8 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
                     const float *dL_dout_color, float *dL_dmeans2D, float *dL_dcolors, float *dL_dopacity,
                     float *dL_dmeans3D, float *dL_dcov3D, float *dL_dsh, float *dL_dscales, float *dL_drotations,
                     void *grad_scratch, cudaStream_t stream, const SgrBackwardPlan *plan, const FeatureChannel *feat);
+// The reference's full per-tile list (dead instances included) of a forward's state, into `full`; `cursor`: T words
+int build_full_list(int P, int W, int H, const GeomState &geom, const ImageState &img, uint64_t num_rendered,
+                    const BinState &full, uint32_t *cursor, cudaStream_t stream);
 
 }  // namespace sgr
