@@ -510,6 +510,35 @@ SGR_API int sgr_texture_bake_view(int32_t V, int32_t F, int32_t n_uv, int32_t T,
                                   const float *image, const float *zbuf, const int64_t *pix_to_face, float *tex_sum,
                                   int32_t *tex_count, int32_t *owner, int32_t *pix_texel, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Marching-cubes mesh of the coarse model (the use_marching_cubes branch of coarse_mesh.py:623-714).
+ * sgr_density_grid: SuGaR.compute_density (sugar_model.py:1345-1368) at every point (x_axis[i], y_axis[j], z_axis[k])
+ * of a torch.meshgrid ('ij'): the exact K nearest Gaussian centres by squared distance (sgr_knn's set and order), summed
+ * with sgr_field_forward's arithmetic and order, so a voxel equals sgr_field_forward over sgr_knn's neighbours of the
+ * same point.  Voxels strictly inside the box (-e, e)^3, e = exclude_extent compared in float32, are 0 without a search
+ * (coarse_mesh.py:698); e <= 0 excludes nothing.
+ *   points f32[P,3], scaling f32[P,3] (activated), quaternions f32[P,4] (w first, 16-byte aligned), strengths f32[P],
+ *   x_axis f32[Rx], y_axis f32[Ry], z_axis f32[Rz], density f32[Rx,Ry,Rz] fully written.
+ *   Limits: 0 < K <= min(P, 64), Rx*Ry*Rz <= 2^30.  `workspace`: sgr_density_grid_workspace_bytes(P) bytes.
+ * sgr_mcubes_count / sgr_mcubes_emit: marching cubes at `level` (a corner is inside when (double)value > level) with
+ * the generated case table of sgr_mcubes_table.h.  One vertex per grid edge whose ends are on different sides, at
+ * lower corner + t along the edge, t = (level - f1) / (f2 - f1) in double, in index space; vertices ordered by the
+ * edge's lower voxel (C order), then axis x, y, z; triangles (int64 vertex ids) ordered by cube, then table order.
+ * count classifies and scans into `scratch` and returns the totals (one stream synchronisation; more than 2^32 - 1 of
+ * either is an error); emit, on the same scratch, volume and level, writes verts f32[n_verts,3] and faces i64[n_faces,3].
+ *   volume f32[Rx,Ry,Rz] (C order), Rx*Ry*Rz <= 2^30.  `scratch`: sgr_mcubes_scratch_bytes(Rx, Ry, Rz) bytes.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API size_t sgr_density_grid_workspace_bytes(int32_t P);
+SGR_API int sgr_density_grid(int32_t P, const float *points, const float *scaling, const float *quaternions,
+                             const float *strengths, int32_t K, float density_factor, int32_t Rx, int32_t Ry,
+                             int32_t Rz, const float *x_axis, const float *y_axis, const float *z_axis,
+                             float exclude_extent, float *density, void *workspace, void *stream);
+SGR_API size_t sgr_mcubes_scratch_bytes(int32_t Rx, int32_t Ry, int32_t Rz);
+SGR_API int sgr_mcubes_count(int32_t Rx, int32_t Ry, int32_t Rz, const float *volume, double level, int64_t *n_verts,
+                             int64_t *n_faces, void *scratch, void *stream);
+SGR_API int sgr_mcubes_emit(int32_t Rx, int32_t Ry, int32_t Rz, const float *volume, double level, int64_t n_verts,
+                            int64_t n_faces, float *verts, int64_t *faces, void *scratch, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */

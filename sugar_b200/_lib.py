@@ -123,6 +123,12 @@ PROTOTYPES = {
     "sgr_texture_init": (C.c_int, [C.c_int32] * 5 + [C.c_void_p] * 8),
     "sgr_texture_bake_view": (C.c_int, [C.c_int32] * 4 + [C.c_void_p] * 6 + [C.c_int32, C.c_int32] +
                               [C.c_void_p] * 8),
+    "sgr_density_grid_workspace_bytes": (C.c_size_t, [C.c_int32]),
+    "sgr_density_grid": (C.c_int, [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32, C.c_float] + [C.c_int32] * 3 +
+                         [C.c_void_p] * 3 + [C.c_float] + [C.c_void_p] * 3),
+    "sgr_mcubes_scratch_bytes": (C.c_size_t, [C.c_int32] * 3),
+    "sgr_mcubes_count": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double] + [C.c_void_p] * 4),
+    "sgr_mcubes_emit": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double, C.c_int64, C.c_int64] + [C.c_void_p] * 4),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),

@@ -10,11 +10,10 @@
 // (sample, neighbour) pair, gathers a 48-byte packed Gaussian record, and the K partial
 // opacities are summed with shuffles.  Backward recomputes the pair and scatters with
 // 16-byte vector reductions into a packed per-Gaussian gradient record.
-#include "sgr_internal.cuh"
+#include "sgr_field.cuh"
 
 namespace sgr {
 
-// packed per-Gaussian record, 12 floats:  mu.xyz sig | q.rijk | inv_s.xyz s_min
 __global__ void __launch_bounds__(256) field_pack_kernel(int P, const float *__restrict__ points,
                                                          const float *__restrict__ scaling,
                                                          const float *__restrict__ quats,
@@ -28,28 +27,6 @@ __global__ void __launch_bounds__(256) field_pack_kernel(int P, const float *__r
     // 1 / scaling.clamp(min=1e-8)   (sugar_model.py:732-733)
     rec[(size_t)i * 3 + 2] =
         make_float4(1.0f / fmaxf(s0, 1e-8f), 1.0f / fmaxf(s1, 1e-8f), 1.0f / fmaxf(s2, 1e-8f), fminf(s0, fminf(s1, s2)));
-}
-
-struct Rot {
-    float m[3][3];  // row-major R[row][col]
-    float ts;       // two_s = 2 / |q|^2
-};
-__device__ __forceinline__ Rot quat_to_rot(float4 q)
-{
-    const float r = q.x, i = q.y, j = q.z, k = q.w;
-    Rot o;
-    o.ts = 2.0f / (r * r + i * i + j * j + k * k);
-    const float ts = o.ts;
-    o.m[0][0] = 1 - ts * (j * j + k * k);
-    o.m[0][1] = ts * (i * j - k * r);
-    o.m[0][2] = ts * (i * k + j * r);
-    o.m[1][0] = ts * (i * j + k * r);
-    o.m[1][1] = 1 - ts * (i * i + k * k);
-    o.m[1][2] = ts * (j * k - i * r);
-    o.m[2][0] = ts * (i * k - j * r);
-    o.m[2][1] = ts * (j * k + i * r);
-    o.m[2][2] = 1 - ts * (i * i + j * j);
-    return o;
 }
 
 template <int G>
@@ -100,13 +77,7 @@ __global__ void __launch_bounds__(256) field_forward_kernel(const FieldArgs a, f
         for (int k = l; k < a.K; k += G) {
             const int64_t id = a.idx[(size_t)nrow * a.K + k];
             const float4 r0 = __ldg(a.rec + id * 3), r1 = __ldg(a.rec + id * 3 + 1), r2 = __ldg(a.rec + id * 3 + 2);
-            const Rot R = quat_to_rot(r1);
-            const float sh0 = x0 - r0.x, sh1 = x1 - r0.y, sh2 = x2 - r0.z;
-            const float w0 = (R.m[0][0] * sh0 + R.m[1][0] * sh1 + R.m[2][0] * sh2) * r2.x;
-            const float w1 = (R.m[0][1] * sh0 + R.m[1][1] * sh1 + R.m[2][1] * sh2) * r2.y;
-            const float w2 = (R.m[0][2] * sh0 + R.m[1][2] * sh1 + R.m[2][2] * sh2) * r2.z;
-            const float d2 = fminf(fmaxf(w0 * w0 + w1 * w1 + w2 * w2, 0.f), 1e8f);
-            const float o = a.density_factor * r0.w * expf(-0.5f * d2);
+            const float o = field_term(x0, x1, x2, r0, r1, r2, a.density_factor);
             if (nbr_opacity) nbr_opacity[(size_t)n * a.K + k] = o;
             dens += o;
             bsum += r2.w;
@@ -265,11 +236,10 @@ __global__ void __launch_bounds__(256) field_unpack_kernel(int P, const float4 *
     if (g_scaling) g_scaling[3 * i] = c.x, g_scaling[3 * i + 1] = c.y, g_scaling[3 * i + 2] = c.z;
 }
 
-static int group_width(int K)
+void field_pack(int kind, int P, const float *points, const float *scaling, const float *quats, const float *strengths,
+                float4 *rec, cudaStream_t st)
 {
-    int G = 1;
-    while (G < K && G < 32) G <<= 1;
-    return G;
+    SGR_LAUNCH(kind, st, field_pack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quats, strengths, rec));
 }
 
 }  // namespace sgr
@@ -321,8 +291,7 @@ int sgr_field_forward(const SgrFieldParams *p, const float *x, const int64_t *nb
     if (p->N == 0) return SGR_OK;
     cudaStream_t st = (cudaStream_t)stream;
     float4 *rec = (float4 *)align_up((size_t)scratch);
-    SGR_LAUNCH(K_FIELD_PACK, st,
-               field_pack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, points, scaling, quaternions, strengths, rec));
+    field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
     const FieldArgs a = make_args(p, x, nbr_idx, rec);
     const int G = group_width(p->K);
     const int blocks = (p->N + 256 / G - 1) / (256 / G);
@@ -353,8 +322,7 @@ int sgr_field_backward(const SgrFieldParams *p, const float *x, const int64_t *n
     float *grec = (float *)((char *)rec + align_up((size_t)p->P * 48));
     SGR_CUDA(cudaMemsetAsync(grec, 0, (size_t)p->P * 48, st));
     if (p->N > 0) {
-        SGR_LAUNCH(K_FIELD_PACK, st,
-                   field_pack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, points, scaling, quaternions, strengths, rec));
+        field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
         const FieldArgs a = make_args(p, x, nbr_idx, rec);
         const int G = group_width(p->K);
         const int blocks = (p->N + 256 / G - 1) / (256 / G);

@@ -16,16 +16,9 @@
 // size) stays on the device: no host synchronisation.
 #include <math.h>
 
-#include "sgr_internal.cuh"
+#include "sgr_knn.cuh"
 
 namespace sgr {
-
-struct KnnGrid {
-    float lo[3];
-    float inv_h;  // cells per unit length (cubic cells)
-    float h;      // cell edge
-    int n[3];     // cells per axis, n[0] * n[1] * n[2] <= the budget N^3
-};
 
 __device__ __forceinline__ int float_flip(float f)
 {  // order-preserving float -> int map for atomicMin/Max
@@ -123,12 +116,6 @@ __global__ void knn_grid_setup_kernel(const int *bb, int n, int P, KnnGrid *g)
     for (int a = 0; a < 3; a++) g->n[a] = c[a];
 }
 
-__device__ __forceinline__ int cell_coord(float v, float lo, float inv_h, int n)
-{
-    const int c = (int)floorf((v - lo) * inv_h);
-    return min(max(c, 0), n - 1);
-}
-
 __global__ void __launch_bounds__(256) knn_count_kernel(int P, const float *__restrict__ pts, const KnnGrid *__restrict__ gp,
                                                         uint32_t *__restrict__ cell_of, uint32_t *__restrict__ counts)
 {
@@ -143,7 +130,8 @@ __global__ void __launch_bounds__(256) knn_count_kernel(int P, const float *__re
     atomicAdd(&counts[c], 1u);
 }
 
-// three-kernel exclusive scan over the cell counts (block = 1024 threads x 4 cells)
+// three-kernel exclusive scan over the cell counts (block = 1024 threads x 4 cells); in place is safe: a thread loads
+// its four counts before the block barrier and stores their offsets after it
 __global__ void __launch_bounds__(1024) knn_scan_blocks_kernel(int ncell, const uint32_t *__restrict__ counts,
                                                                uint32_t *__restrict__ starts, uint32_t *__restrict__ block_sums)
 {
@@ -244,8 +232,6 @@ __global__ void __launch_bounds__(256) knn_scatter_kernel(int P, const float *__
     sorted[slot] = make_float4(pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], __int_as_float(i));
 }
 
-constexpr int KNN_MAXK = 64;
-
 __global__ void __launch_bounds__(128) knn_query_kernel(int Q, int K, int P, const float *__restrict__ qs,
                                                         const KnnGrid *__restrict__ gp, const uint32_t *__restrict__ starts,
                                                         const float4 *__restrict__ sorted, int64_t *__restrict__ idx_out,
@@ -323,13 +309,7 @@ static int knn_axis_cells(int P)
     return n;
 }
 
-}  // namespace sgr
-
-using namespace sgr;
-
-extern "C" {
-
-size_t sgr_knn_workspace_bytes(int32_t P)
+size_t knn_cells_bytes(int P)
 {
     const size_t n = (size_t)knn_axis_cells(P < 1 ? 1 : P), ncell = n * n * n;
     const size_t nblocks = (ncell + 4095) / 4096;
@@ -337,16 +317,17 @@ size_t sgr_knn_workspace_bytes(int32_t P)
            align_up((nblocks + 1) * 4) + align_up((size_t)P * 16) + SGR_ALIGN;
 }
 
-int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int32_t K, int64_t *idx, float *dist2,
-            void *workspace, void *stream)
+void exclusive_scan_u32(int kind, int n, const uint32_t *counts, uint32_t *starts, uint32_t *block_sums,
+                        uint32_t *cursor, cudaStream_t st)
 {
-    if (P <= 0 || Q < 0 || K <= 0 || K > KNN_MAXK || K > P || !points || (Q > 0 && (!queries || !idx || !dist2)) ||
-        !workspace) {
-        set_error("sgr_knn: need 0 < K <= min(P, %d), non-null pointers (P=%d Q=%d K=%d)", KNN_MAXK, P, Q, K);
-        return SGR_EINVAL;
-    }
-    if (Q == 0) return SGR_OK;
-    cudaStream_t st = (cudaStream_t)stream;
+    const int nblocks = (int)(((size_t)n + 4095) / 4096);
+    SGR_LAUNCH(kind, st, knn_scan_blocks_kernel<<<(unsigned)nblocks, 1024, 0, st>>>(n, counts, starts, block_sums));
+    SGR_LAUNCH(kind, st, knn_scan_sums_kernel<<<1, 1024, 0, st>>>(nblocks, block_sums));
+    SGR_LAUNCH(kind, st, knn_scan_add_kernel<<<(unsigned)nblocks, 1024, 0, st>>>(n, starts, block_sums, cursor));
+}
+
+int knn_build_cells(int P, const float *points, void *workspace, cudaStream_t st, KnnCells *out)
+{
     const int n = knn_axis_cells(P);
     const size_t ncell = (size_t)n * n * n, nblocks = (ncell + 4095) / 4096;
     char *p = (char *)align_up((size_t)workspace);
@@ -362,12 +343,38 @@ int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int
     SGR_LAUNCH(K_KNN, st, knn_grid_setup_kernel<<<1, 32, 0, st>>>(bb, n, P, grid));
     SGR_CUDA(cudaMemsetAsync(cursor, 0, ncell * 4, st));  // cursor doubles as the count array first
     SGR_LAUNCH(K_KNN, st, knn_count_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, grid, cell_of, cursor));
-    SGR_LAUNCH(K_KNN, st, knn_scan_blocks_kernel<<<(unsigned)nblocks, 1024, 0, st>>>((int)ncell, cursor, starts, bsums));
-    SGR_LAUNCH(K_KNN, st, knn_scan_sums_kernel<<<1, 1024, 0, st>>>((int)nblocks, bsums));
-    SGR_LAUNCH(K_KNN, st, knn_scan_add_kernel<<<(unsigned)nblocks, 1024, 0, st>>>((int)ncell, starts, bsums, cursor));
+    exclusive_scan_u32(K_KNN, (int)ncell, cursor, starts, bsums, cursor, st);
     SGR_LAUNCH(K_KNN, st, knn_scatter_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, cell_of, cursor, sorted));
+    out->grid = grid;
+    out->starts = starts;
+    out->sorted = sorted;
+    return SGR_OK;
+}
+
+}  // namespace sgr
+
+using namespace sgr;
+
+extern "C" {
+
+size_t sgr_knn_workspace_bytes(int32_t P) { return knn_cells_bytes(P); }
+
+int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int32_t K, int64_t *idx, float *dist2,
+            void *workspace, void *stream)
+{
+    if (P <= 0 || Q < 0 || K <= 0 || K > KNN_MAXK || K > P || !points || (Q > 0 && (!queries || !idx || !dist2)) ||
+        !workspace) {
+        set_error("sgr_knn: need 0 < K <= min(P, %d), non-null pointers (P=%d Q=%d K=%d)", KNN_MAXK, P, Q, K);
+        return SGR_EINVAL;
+    }
+    if (Q == 0) return SGR_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    KnnCells cells;
+    int rc = knn_build_cells(P, points, workspace, st, &cells);
+    if (rc) return rc;
     SGR_LAUNCH(K_KNN_QUERY, st,
-               knn_query_kernel<<<(Q + 127) / 128, 128, 0, st>>>(Q, K, P, queries, grid, starts, sorted, idx, dist2));
+               knn_query_kernel<<<(Q + 127) / 128, 128, 0, st>>>(Q, K, P, queries, cells.grid, cells.starts,
+                                                                 cells.sorted, idx, dist2));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }
