@@ -297,6 +297,27 @@ def rel_err(a, b):
     return d / max(np.abs(b).max() if b.size else 0.0, 1e-30)
 
 
+def row_errors(got, want, bound, rows=None):
+    """Row-wise comparison of [P, C] arrays (one row per Gaussian): per row the largest |got - want| / bound over its
+    components (a nonzero difference against a zero bound, and any non-finite `got` or difference, count as
+    infinite, so a NaN fails the check).  rows: bool [P], the rows compared (default all).  Returns
+    dict(ratio_rows [P] (0 outside `rows`), ratio (the largest), worst_row, worst_col, n_over (rows with ratio > 1)).
+    Unlike rel_err, a row far below the tensor's largest is held to its own bound."""
+    got = np.asarray(got, np.float64).reshape(len(got), -1)
+    want = np.asarray(want, np.float64).reshape(got.shape)
+    bound = np.asarray(bound, np.float64).reshape(got.shape)
+    d = np.abs(got - want)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        r = np.where(d == 0, 0.0, d / bound)
+    r[~np.isfinite(got) | ~np.isfinite(r)] = np.inf
+    if rows is not None:
+        r[~np.asarray(rows, bool)] = 0.0
+    per_row = r.max(1) if r.size else np.zeros(len(got))
+    worst = int(np.argmax(per_row)) if per_row.size else 0
+    return dict(ratio_rows=per_row, ratio=float(per_row[worst]) if per_row.size else 0.0, worst_row=worst,
+                worst_col=int(np.argmax(r[worst])) if r.size else 0, n_over=int((per_row > 1.0).sum()))
+
+
 def grad_sensitivity(sc, bg, dL, eps=1e-6, **opts):
     """Conditioning probe for the per-Gaussian backward chain (CPU oracle): relative change (|.|_inf / |g|_inf)
     of each returned gradient when the blend accumulators dL_dmeans2D / dL_dconic are perturbed by `eps`
