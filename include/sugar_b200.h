@@ -539,6 +539,23 @@ SGR_API int sgr_mcubes_count(int32_t Rx, int32_t Ry, int32_t Rz, const float *vo
 SGR_API int sgr_mcubes_emit(int32_t Rx, int32_t Ry, int32_t Rz, const float *volume, double level, int64_t n_verts,
                             int64_t n_faces, float *verts, int64_t *faces, void *scratch, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Quadric edge-collapse decimation (open3d's simplify_quadric_decimation with maximum_error = inf and
+ * boundary_weight = 1, as coarse_mesh.py:433-463 and :716-744 call it), restated in oracle/decimate_oracle.py:
+ * rounds of independent collapses until the face count is at most `target` or no edge can be collapsed.  The
+ * result equals decimate_rounds of the oracle array for array.  Everything runs on `stream`; one host read per round.
+ *   verts f32[V,3], faces i64[F,3] (ids in [0, V), no face repeats a vertex; checked on the device before any other
+ *   work), colors / normals f32[V,3] or NULL (each goes with its output).  Outputs are caller-sized: verts_out
+ *   f32[V,3], faces_out i64[F,3], colors_out / normals_out f32[V,3]; the first V' and F' rows are written: the faces
+ *   that survive in their order, and the vertices they reference in theirs.
+ *   result i64[4] <- V', F', rounds, faces removed by the collapse that reached the target (0 if it was not reached).
+ *   Limits: V <= 2^30, F <= 2^29.  `scratch`: sgr_decimate_scratch_bytes(V, F) bytes.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API size_t sgr_decimate_scratch_bytes(int32_t V, int32_t F);
+SGR_API int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *verts, const int64_t *faces,
+                         const float *colors, const float *normals, float *verts_out, int64_t *faces_out,
+                         float *colors_out, float *normals_out, int64_t *result, void *scratch, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */

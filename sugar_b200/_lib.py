@@ -129,6 +129,8 @@ PROTOTYPES = {
     "sgr_mcubes_scratch_bytes": (C.c_size_t, [C.c_int32] * 3),
     "sgr_mcubes_count": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double] + [C.c_void_p] * 4),
     "sgr_mcubes_emit": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double, C.c_int64, C.c_int64] + [C.c_void_p] * 4),
+    "sgr_decimate_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
+    "sgr_decimate": (C.c_int, [C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 11),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),
