@@ -16,7 +16,7 @@ from typing import Tuple
 import torch
 
 from . import _lib
-from ._lib import SgrGaussians, SgrView, check, lib
+from ._lib import SgrGaussians, SgrView, check, f32_ptr, lib, require_cuda, stream
 
 
 class Context:
@@ -61,17 +61,6 @@ def use_context(ctx: Context):
         yield ctx
     finally:
         _tls.ctx = prev
-
-
-def _ptr(t: torch.Tensor, name: str):
-    """Device pointer of an optional tensor: empty tensor == absent == NULL (forward.cu:205,241)."""
-    if t is None or t.numel() == 0:
-        return None
-    if t.dtype != torch.float32:
-        raise TypeError(f"{name} must be float32, got {t.dtype}")
-    if not t.is_cuda:
-        raise _lib.SgrError(f"{name} must be a CUDA tensor (sugar_b200 has no CPU path)")
-    return t.data_ptr()
 
 
 _ROUND = 64 << 20  # arena sizes are rounded up to 64 MiB so the caching allocator sees few distinct sizes
@@ -128,12 +117,12 @@ def _view_struct(bg, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy,
     v = SgrView()
     v.image_height, v.image_width = int(H), int(W)
     v.tanfovx, v.tanfovy = float(tan_fovx), float(tan_fovy)
-    v.bg = _ptr(bg, "bg")
+    v.bg = f32_ptr(bg, "bg")
     v.scale_modifier = float(scale_modifier)
-    v.viewmatrix = _ptr(viewmatrix, "viewmatrix")
-    v.projmatrix = _ptr(projmatrix, "projmatrix")
+    v.viewmatrix = f32_ptr(viewmatrix, "viewmatrix")
+    v.projmatrix = f32_ptr(projmatrix, "projmatrix")
     v.sh_degree = int(degree)
-    v.campos = _ptr(campos, "campos")
+    v.campos = f32_ptr(campos, "campos")
     v.prefiltered, v.debug = int(bool(prefiltered)), int(bool(debug))
     return v
 
@@ -141,15 +130,15 @@ def _view_struct(bg, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy,
 def _gauss_struct(P, M, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp, sh_rest=None) -> SgrGaussians:
     g = SgrGaussians()
     g.activations = 1 if sh_rest is not None else 0   # SGR_ACT_RAW: raw SuGaR parameters, (dc, rest) SH arrays
-    g.sh_rest = _ptr(sh_rest, "sh_rest") if sh_rest is not None else None
+    g.sh_rest = f32_ptr(sh_rest, "sh_rest") if sh_rest is not None else None
     g.P, g.M = int(P), int(M)
-    g.means3D = _ptr(means3D, "means3D")
-    g.opacities = _ptr(opacity, "opacity")
-    g.shs = _ptr(sh, "sh")
-    g.colors_precomp = _ptr(colors, "colors")
-    g.scales = _ptr(scales, "scales")
-    g.rotations = _ptr(rotations, "rotations")
-    g.cov3D_precomp = _ptr(cov3D_precomp, "cov3D_precomp")
+    g.means3D = f32_ptr(means3D, "means3D")
+    g.opacities = f32_ptr(opacity, "opacity")
+    g.shs = f32_ptr(sh, "sh")
+    g.colors_precomp = f32_ptr(colors, "colors")
+    g.scales = f32_ptr(scales, "scales")
+    g.rotations = f32_ptr(rotations, "rotations")
+    g.cov3D_precomp = f32_ptr(cov3D_precomp, "cov3D_precomp")
     return g
 
 
@@ -179,8 +168,7 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         _no_exchange(context)
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
-    if not means3D.is_cuda:
-        raise _lib.SgrError("sugar_b200 needs CUDA tensors: there is no CPU fallback")
+    require_cuda("diff_gaussian_rasterization", means3D)
     dev = means3D.device
     P, H, W = means3D.size(0), int(image_height), int(image_width)
     if feature and (values.numel() != P or feature_bg.numel() != 1):
@@ -208,12 +196,11 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
                             campos, prefiltered, debug)
         g = _gauss_struct(P, M, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp, sh_rest)
         rendered = C.c_int64(0)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         allocs = (arena.cbs["geom"], None, arena.cbs["binning"], None, arena.cbs["img"], None)
-        tail = (radii.data_ptr() if P else None, hint, C.byref(rendered), stream)
+        tail = (radii.data_ptr() if P else None, hint, C.byref(rendered), stream(dev))
         if feature:
             status = lib.sgr_rasterize_forward_feature(
-                C.byref(view), C.byref(g), *allocs, _ptr(values, "values"), _ptr(feature_bg, "feature_bg"),
+                C.byref(view), C.byref(g), *allocs, f32_ptr(values, "values"), f32_ptr(feature_bg, "feature_bg"),
                 out_color.data_ptr(), out_feature.data_ptr(), *tail)
         else:
             status = lib.sgr_rasterize_forward(C.byref(view), C.byref(g), *allocs, out_color.data_ptr(), *tail)
@@ -303,11 +290,11 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                 campos, False, debug)
             # opacities are not an input of the reference's backward; the forward stored them
             g = _gauss_struct(P, M, means3D, None, sh, colors, scales, rotations, cov3D_precomp, sh_rest)
-            stream = torch.cuda.current_stream(dev).cuda_stream
+            st = stream(dev)
             # the SH exchange rebuilds the summed dL_dsh from the views' colour gradients: the pass does not write it
             dsh = b["sh"].data_ptr() if (M and not (ex is not None and ex.sh_factors)) else None
             inputs = (C.byref(view), C.byref(g), radii.data_ptr(), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
-                      imageBuffer.data_ptr(), int(R), _ptr(dL_dout_color, "dL_dout_color"))
+                      imageBuffer.data_ptr(), int(R), f32_ptr(dL_dout_color, "dL_dout_color"))
 
             def grads(dL_dcolors, dL_dsh):   # the eight gradient arrays in the C argument order
                 return (b["means2D"].data_ptr(), dL_dcolors, b["opacity"].data_ptr(), b["means3D"].data_ptr(),
@@ -317,13 +304,13 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                 """Enqueue sgr_rasterize_backward_staged under `plan` (None: no stages); the view-parallel peer
                 exchange points the two outputs it sums itself into its own buffers."""
                 check(lib.sgr_rasterize_backward_staged(*inputs, *grads(dL_dcolors, dL_dsh), b["scratch"].data_ptr(),
-                                                        stream, None if plan is None else C.byref(plan)))
+                                                        st, None if plan is None else C.byref(plan)))
 
             if feature:
                 check(lib.sgr_rasterize_backward_feature(
-                    *inputs, _ptr(values, "values"), _ptr(feature_bg, "feature_bg"),
-                    _ptr(dL_dout_feature, "dL_dout_feature"), *grads(b["colors"].data_ptr(), dsh),
-                    dL_dvalues.data_ptr(), b["scratch"].data_ptr(), stream))
+                    *inputs, f32_ptr(values, "values"), f32_ptr(feature_bg, "feature_bg"),
+                    f32_ptr(dL_dout_feature, "dL_dout_feature"), *grads(b["colors"].data_ptr(), dsh),
+                    dL_dvalues.data_ptr(), b["scratch"].data_ptr(), st))
             elif ex is not None:
                 ex.run_backward(launch, b, P, M, int(degree), means3D, campos, has_cov_precomp=has_cov)
             elif raw:   # the plan carries the second SH gradient array
@@ -342,9 +329,9 @@ def mark_visible(means3D, viewmatrix, projmatrix) -> torch.Tensor:
     if P != 0:
         with torch.cuda.device(means3D.device):
             means3D, viewmatrix, projmatrix = map(_c, (means3D, viewmatrix, projmatrix))
-            check(lib.sgr_mark_visible(P, _ptr(means3D, "means3D"), _ptr(viewmatrix, "viewmatrix"),
-                                       _ptr(projmatrix, "projmatrix"), present.data_ptr(),
-                                       torch.cuda.current_stream(means3D.device).cuda_stream))
+            check(lib.sgr_mark_visible(P, f32_ptr(means3D, "means3D"), f32_ptr(viewmatrix, "viewmatrix"),
+                                       f32_ptr(projmatrix, "projmatrix"), present.data_ptr(),
+                                       stream(means3D.device)))
     return present
 
 
@@ -367,8 +354,7 @@ def inspect_state(P, W, H, R, geomBuffer, binningBuffer, imageBuffer):
                                     out["conic_opacity"].data_ptr(), out["rgb"].data_ptr(), out["clamped"].data_ptr(),
                                     out["tiles_touched"].data_ptr(), out["keys"].data_ptr(),
                                     out["point_list"].data_ptr(), out["ranges"].data_ptr(), out["final_T"].data_ptr(),
-                                    out["n_contrib"].data_ptr(), out["footprint"].data_ptr(),
-                                    torch.cuda.current_stream(dev).cuda_stream))
+                                    out["n_contrib"].data_ptr(), out["footprint"].data_ptr(), stream(dev)))
     out["keys"] = out["keys"][:R]
     out["point_list"] = out["point_list"][:R]
     out["footprint"] = out["footprint"][:R]

@@ -6,6 +6,8 @@ call raises on a non-zero status with the library's own message.
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SGR_LIB_PATH", os.path.join(_HERE, "lib", "libsugar_b200.so"))  # override: the stats build (scripts/blend_stats.py)
 
@@ -166,6 +168,75 @@ for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams,
 def check(status: int) -> None:
     if status != 0:
         raise SgrError(lib.sgr_last_error().decode(errors="replace") or f"libsugar_b200 error {status}")
+
+
+# How the op wrappers pass tensors to the library.  Argument checks run first, so that they work on CPU tensors too.
+
+def ptr(t):
+    """Device pointer of an optional tensor: None or an empty tensor gives NULL."""
+    return None if t is None or t.numel() == 0 else t.data_ptr()
+
+
+def f32_ptr(t, name: str):
+    """ptr() of an optional float32 CUDA tensor, checked (the rasterizer's arguments)."""
+    if t is None or t.numel() == 0:
+        return None
+    if t.dtype != torch.float32:
+        raise TypeError(f"{name} must be float32, got {t.dtype}")
+    if not t.is_cuda:
+        raise SgrError(f"{name} must be a CUDA tensor (sugar_b200 has no CPU path)")
+    return t.data_ptr()
+
+
+def stream(dev):
+    """The current CUDA stream of `dev` as the library takes it."""
+    return torch.cuda.current_stream(dev).cuda_stream
+
+
+def scratch(nbytes: int, dev) -> torch.Tensor:
+    """Device scratch of `nbytes`, the answer of one of the library's size queries."""
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev)
+
+
+def require_cuda(module: str, *ts) -> None:
+    for t in ts:
+        if t is not None and not (torch.is_tensor(t) and t.is_cuda):
+            raise SgrError(f"sugar_b200.{module} needs CUDA tensors: there is no CPU fallback")
+
+
+def tensor(t, name: str, dtype, shape, device=None, ref: str = "verts", align: int = 0):
+    """-> `t` as the kernel may read it: contiguous, and copied when `align` (bytes) is given and not met.
+    Raises ValueError unless `t` is a `dtype` tensor of `shape` on `device` (when given; `ref` names the argument
+    that fixed it).  `shape` entries are sizes, or names of free dimensions (str)."""
+    want = ",".join(str(s) for s in shape)
+    if not torch.is_tensor(t) or t.dtype != dtype or t.dim() != len(shape) or \
+            any(isinstance(s, int) and t.shape[i] != s for i, s in enumerate(shape)):
+        got = f"{t.dtype} {tuple(t.shape)}" if torch.is_tensor(t) else type(t).__name__
+        raise ValueError(f"{name} must be {str(dtype).replace('torch.', '')} [{want}], got {got}")
+    if device is not None and t.device != device:
+        raise ValueError(f"{name} on {t.device}, {ref} on {device}")
+    t = t.contiguous()
+    if align and t.data_ptr() % align:
+        t = t.clone()
+    return t
+
+
+def same_device(dev, ref: str = "verts", **ts) -> None:
+    for name, t in ts.items():
+        if t is not None and t.device != dev:
+            raise ValueError(f"{name} on {t.device}, {ref} on {dev}")
+
+
+def check_ids(*checks) -> None:
+    """checks: (ids, lo, hi, what).  Raises ValueError naming each check with ids outside [lo, hi), after one host
+    read for all of them."""
+    checks = [c for c in checks if c[0].numel()]
+    if not checks:
+        return
+    counts = torch.stack([((ids < lo) | (ids >= hi)).sum() for ids, lo, hi, _ in checks]).tolist()
+    for n, (_, lo, hi, what) in zip(counts, checks):
+        if n:
+            raise ValueError(f"{n} {what} outside [{lo}, {hi})")
 
 
 def profile(on: bool) -> None:

@@ -103,6 +103,9 @@ void prof_end(cudaStream_t st)
     g_prof_n++;
 }
 
+// the 16-bit tile rect bounds the image at 65535 tiles per side
+static bool image_size_ok(int W, int H) { return W > 0 && H > 0 && W <= 65535 * 16 && H <= 65535 * 16; }
+
 static int validate(const SgrView *view, const SgrGaussians *g, bool forward)
 {
     if (!view || !g) {
@@ -113,7 +116,7 @@ static int validate(const SgrView *view, const SgrGaussians *g, bool forward)
         set_error("bad sizes P=%d W=%d H=%d", g->P, view->image_width, view->image_height);
         return SGR_EINVAL;
     }
-    if (view->image_width > 65535 * 16 || view->image_height > 65535 * 16) {
+    if (!image_size_ok(view->image_width, view->image_height)) {
         set_error("image too large for the 16-bit tile rect");
         return SGR_EINVAL;
     }
@@ -396,10 +399,13 @@ SGR_API int sgr_debug_blend_stats(unsigned long long *out16, int reset)
 #endif
 const char *sgr_version(void) { return "sugar_b200 0.1 (sm_90a)"; }
 
-size_t sgr_geometry_bytes(int32_t P) { return GeomState::bytes((size_t)(P < 0 ? 0 : P)); }
-size_t sgr_binning_bytes(int64_t capacity) { return BinState::bytes((size_t)(capacity < 0 ? 0 : capacity)); }
-size_t sgr_image_bytes(int32_t width, int32_t height) { return ImageState::bytes((size_t)width, (size_t)height); }
-size_t sgr_backward_scratch_bytes(int32_t P) { return align_up((size_t)(P < 0 ? 0 : P) * 32) + SGR_ALIGN; }
+size_t sgr_geometry_bytes(int32_t P) { return P < 0 ? 0 : layout_bytes([&](Layout &l) { GeomState::carve(l, P); }); }
+size_t sgr_binning_bytes(int64_t C) { return C < 0 ? 0 : layout_bytes([&](Layout &l) { BinState::carve(l, C); }); }
+size_t sgr_image_bytes(int32_t W, int32_t H)
+{
+    return image_size_ok(W, H) ? layout_bytes([&](Layout &l) { ImageState::carve(l, W, H); }) : 0;
+}
+size_t sgr_backward_scratch_bytes(int32_t P) { return P < 0 ? 0 : layout_bytes([&](Layout &l) { carve_grad_acc(l, P); }); }
 
 int sgr_rasterize_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_alloc, void *geom_ctx,
                           SgrAlloc binning_alloc, void *binning_ctx, SgrAlloc image_alloc, void *image_ctx,
@@ -482,8 +488,9 @@ int sgr_inspect_state(int32_t P, int32_t width, int32_t height, int64_t num_rend
         set_error("bad arguments to sgr_inspect_state");
         return SGR_EINVAL;
     }
-    GeomState geom = GeomState::carve((void *)geom_buffer, P);
-    ImageState img = ImageState::carve((void *)image_buffer, width, height);
+    Layout geom_l(geom_buffer), img_l(image_buffer);
+    GeomState geom = GeomState::carve(geom_l, P);
+    ImageState img = ImageState::carve(img_l, width, height);
     const int T = ((width + 15) / 16) * ((height + 15) / 16);
     inspect_geom_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, geom, nullptr, depths, means2D, conic_opacity, rgb, clamped,
                                                          tiles_touched);
@@ -505,12 +512,14 @@ int sgr_inspect_state(int32_t P, int32_t width, int32_t height, int64_t num_rend
     // The forward kept only the live instances; the reference's list (dead ones included, with their masks) is
     // rebuilt here in scratch of its own by the forward's scatter and sorts.  A diagnostic path: it allocates.
     const int gx = (width + 15) / 16;
-    const size_t R = (size_t)num_rendered, cursor_bytes = align_up((size_t)T * 4);
+    const size_t R = (size_t)num_rendered;
+    uint32_t *cursor = nullptr;  // the tile cursors, then a binning layout
+    const auto full_list = [&](Layout &l) { return cursor = l.take<uint32_t>(T), BinState::carve(l, R); };
     void *mem = nullptr;
-    SGR_CUDA(cudaMallocAsync(&mem, cursor_bytes + BinState::bytes(R) + SGR_ALIGN, st));
-    uint32_t *cursor = (uint32_t *)align_up((size_t)mem);
-    const BinState full = BinState::carve((char *)cursor + cursor_bytes, R);
-    const BinState live = BinState::carve((void *)binning_buffer, R);
+    SGR_CUDA(cudaMallocAsync(&mem, layout_bytes(full_list), st));
+    Layout mem_l(mem), live_l(binning_buffer);
+    const BinState full = full_list(mem_l);
+    const BinState live = BinState::carve(live_l, R);
     const int packed = ids_packed(P) ? 1 : 0;
     int rc = build_full_list(P, width, height, geom, img, R, full, cursor, st);
     if (rc == SGR_OK) {

@@ -1361,10 +1361,11 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
                     void *grad_scratch, cudaStream_t st, const SgrBackwardPlan *plan, const FeatureChannel *feat)
 {
     const int P = g->P, W = view->image_width, H = view->image_height;
-    GeomState geom = GeomState::carve((void *)geom_buffer, P);
-    ImageState img = ImageState::carve((void *)image_buffer, W, H);
-    BinState bin = BinState::carve((void *)binning_buffer, (size_t)num_rendered);
-    float *gacc = (float *)align_up((size_t)grad_scratch);
+    Layout geom_l(geom_buffer), img_l(image_buffer), bin_l(binning_buffer), scratch_l(grad_scratch);
+    GeomState geom = GeomState::carve(geom_l, P);
+    ImageState img = ImageState::carve(img_l, W, H);
+    BinState bin = BinState::carve(bin_l, (size_t)num_rendered);
+    float *gacc = carve_grad_acc(scratch_l, P);
     const SgrStageHook hook = plan ? plan->hook : nullptr;
     void *hook_ctx = plan ? plan->hook_ctx : nullptr;
     float *rec11 = plan ? plan->reduce_records : nullptr;

@@ -579,42 +579,39 @@ struct DecScratch {
     PassRec *list;
 };
 
-// carves the scratch from `base` (0: only the size) and returns its size in bytes
-size_t dec_scratch(size_t base, size_t V, size_t F, DecScratch *s)
+DecScratch dec_scratch(Layout &l, size_t V, size_t F)
 {
     const size_t n = (V > F ? V : F) + 1;
-    size_t p = align_up(base);
-    auto take = [&](size_t bytes) {
-        const size_t at = p;
-        p += align_up(bytes);
-        return at;
-    };
     DecScratch t;
-    t.ctr = (unsigned long long *)take(64);
-    t.pos = (double *)take(V * 24);
-    t.Q = (double *)take(V * 80);
-    t.col = (double *)take(V * 24);
-    t.nrm = (double *)take(V * 24);
-    t.vbar = (double *)take(V * 24);
-    t.fc[0] = (int *)take(F * 12);
-    t.fc[1] = (int *)take(F * 12);
-    t.blk[0] = (uint8_t *)take(F);
-    t.blk[1] = (uint8_t *)take(F);
-    t.state = (uint8_t *)take(V);
-    t.vcnt = (uint32_t *)take((V + 1) * 4);
-    t.vstart = (uint32_t *)take((V + 1) * 4);
-    t.csr = (uint32_t *)take(F * 12);
-    t.fflag = (uint32_t *)take(n * 4);
-    t.bsums = (uint32_t *)take(((n + 4095) / 4096 + 1) * 4);
-    t.removed = (uint32_t *)take(V * 4);
-    t.partner = (uint32_t *)take(V * 4);
-    t.slotc = (unsigned long long *)take(F * 24);
-    t.vmin = (DKey *)take(V * sizeof(DKey));
-    t.rmin = (DKey *)take(V * sizeof(DKey));
-    t.fmin = (DKey *)take(F * sizeof(DKey));
-    t.list = (PassRec *)take(V * sizeof(PassRec));
-    if (s) *s = t;
-    return p - base + SGR_ALIGN;
+    t.ctr = l.take<unsigned long long>(8);
+    t.pos = l.take<double>(3 * V);
+    t.Q = l.take<double>(10 * V);
+    t.col = l.take<double>(3 * V);
+    t.nrm = l.take<double>(3 * V);
+    t.vbar = l.take<double>(3 * V);
+    t.fc[0] = l.take<int>(3 * F);
+    t.fc[1] = l.take<int>(3 * F);
+    t.blk[0] = l.take<uint8_t>(F);
+    t.blk[1] = l.take<uint8_t>(F);
+    t.state = l.take<uint8_t>(V);
+    t.vcnt = l.take<uint32_t>(V + 1);
+    t.vstart = l.take<uint32_t>(V + 1);
+    t.csr = l.take<uint32_t>(3 * F);
+    t.fflag = l.take<uint32_t>(n);
+    t.bsums = l.take<uint32_t>(scan_block_sums(n));
+    t.removed = l.take<uint32_t>(V);
+    t.partner = l.take<uint32_t>(V);
+    t.slotc = l.take<unsigned long long>(3 * F);
+    t.vmin = l.take<DKey>(V);
+    t.rmin = l.take<DKey>(V);
+    t.fmin = l.take<DKey>(F);
+    t.list = l.take<PassRec>(V);
+    return t;
+}
+
+static bool dec_sizes_ok(int32_t V, int32_t F)
+{
+    return V >= 0 && F >= 0 && V <= (1 << 30) && F <= (1 << 29) && !(F > 0 && V == 0);
 }
 
 static unsigned grid(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
@@ -647,14 +644,14 @@ extern "C" {
 
 size_t sgr_decimate_scratch_bytes(int32_t V, int32_t F)
 {
-    return dec_scratch(0, (size_t)(V > 0 ? V : 0), (size_t)(F > 0 ? F : 0), nullptr);
+    return dec_sizes_ok(V, F) ? layout_bytes([&](Layout &l) { dec_scratch(l, V, F); }) : 0;
 }
 
 int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *verts, const int64_t *faces, const float *colors,
                  const float *normals, float *verts_out, int64_t *faces_out, float *colors_out, float *normals_out,
                  int64_t *result, void *scratch, void *stream)
 {
-    if (V < 0 || F < 0 || target < 0 || V > (1 << 30) || F > (1 << 29) || (F > 0 && V == 0)) {
+    if (!dec_sizes_ok(V, F) || target < 0) {
         set_error("sgr_decimate: need 0 <= V <= 2^30, 0 <= F <= 2^29 (F > 0 only with V > 0) and target >= 0 "
                   "(V=%d F=%d target=%lld)", V, F, (long long)target);
         return SGR_EINVAL;
@@ -667,8 +664,8 @@ int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *verts, const
     result[0] = result[1] = result[2] = result[3] = 0;
     if (V == 0) return SGR_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    DecScratch s;
-    dec_scratch((size_t)scratch, (size_t)V, (size_t)F, &s);
+    Layout l(scratch);
+    const DecScratch s = dec_scratch(l, V, F);
     double *col = colors ? s.col : nullptr, *nrm = normals ? s.nrm : nullptr;
     unsigned long long ctr[8];
     SGR_CUDA(cudaMemsetAsync(s.ctr, 0, 64, st));

@@ -242,13 +242,21 @@ void field_pack(int kind, int P, const float *points, const float *scaling, cons
     SGR_LAUNCH(kind, st, field_pack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quats, strengths, rec));
 }
 
+// the packed records, then the backward's per-Gaussian gradient records
+struct FieldScratch {
+    float4 *rec;
+    float *grec;
+};
+
+static FieldScratch field_scratch(Layout &l, size_t P) { return {l.take<float4>(3 * P), l.take<float>(12 * P)}; }
+
 }  // namespace sgr
 
 using namespace sgr;
 
 extern "C" {
 
-size_t sgr_field_scratch_bytes(int32_t P) { return align_up((size_t)(P < 0 ? 0 : P) * 48) * 2 + SGR_ALIGN; }
+size_t sgr_field_scratch_bytes(int32_t P) { return P > 0 ? layout_bytes([&](Layout &l) { field_scratch(l, P); }) : 0; }
 
 static int field_check(const SgrFieldParams *p, const void *x, const void *idx, const void *a, const void *b,
                        const void *c, const void *d, const void *scratch)
@@ -290,7 +298,8 @@ int sgr_field_forward(const SgrFieldParams *p, const float *x, const int64_t *nb
     if (rc) return rc;
     if (p->N == 0) return SGR_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    float4 *rec = (float4 *)align_up((size_t)scratch);
+    Layout l(scratch);
+    float4 *rec = field_scratch(l, p->P).rec;
     field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
     const FieldArgs a = make_args(p, x, nbr_idx, rec);
     const int G = group_width(p->K);
@@ -318,8 +327,8 @@ int sgr_field_backward(const SgrFieldParams *p, const float *x, const int64_t *n
     int rc = field_check(p, x, nbr_idx, points, scaling, quaternions, strengths, scratch);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    float4 *rec = (float4 *)align_up((size_t)scratch);
-    float *grec = (float *)((char *)rec + align_up((size_t)p->P * 48));
+    Layout l(scratch);
+    const auto [rec, grec] = field_scratch(l, p->P);
     SGR_CUDA(cudaMemsetAsync(grec, 0, (size_t)p->P * 48, st));
     if (p->N > 0) {
         field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);

@@ -1295,14 +1295,15 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
     const ViewConsts v = view_consts(view, g->M);
     const int T = v.gx * v.gy;
 
-    void *geom_mem = geom_alloc(geom_ctx, GeomState::bytes(P));
-    void *img_mem = image_alloc(image_ctx, ImageState::bytes(W, H));
+    void *geom_mem = geom_alloc(geom_ctx, sgr_geometry_bytes(P));
+    void *img_mem = image_alloc(image_ctx, sgr_image_bytes(W, H));
     if (!geom_mem || !img_mem) {
         set_error("scratch allocator returned NULL");
         return SGR_ENOMEM;
     }
-    GeomState geom = GeomState::carve(geom_mem, P);
-    ImageState img = ImageState::carve(img_mem, W, H);
+    Layout geom_l(geom_mem), img_l(img_mem);
+    GeomState geom = GeomState::carve(geom_l, P);
+    ImageState img = ImageState::carve(img_l, W, H);
 
     SGR_CUDA(cudaMemsetAsync(img.tile_count, 0, sizeof(uint32_t) * T, st));
 
@@ -1350,12 +1351,13 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
     BinState bin;
     if (capacity_hint > 0) {
         capacity = (uint64_t)capacity_hint;
-        void *bin_mem = binning_alloc(binning_ctx, BinState::bytes(capacity));
+        void *bin_mem = binning_alloc(binning_ctx, sgr_binning_bytes((int64_t)capacity));
         if (!bin_mem) {
             set_error("binning allocator returned NULL");
             return SGR_ENOMEM;
         }
-        bin = BinState::carve(bin_mem, capacity);
+        Layout bin_l(bin_mem);
+        bin = BinState::carve(bin_l, capacity);
         rc = launch_binning_and_blend(v, P, geom, img, bin, capacity, out_color, feat, st);
         if (rc) return rc;
         launched = true;
@@ -1364,12 +1366,13 @@ int launch_forward(const SgrView *view, const SgrGaussians *g, SgrAlloc geom_all
     const uint64_t R = *slot->pinned;
     if (!launched || R > capacity) {
         capacity = R;
-        void *bin_mem = binning_alloc(binning_ctx, BinState::bytes(capacity));
+        void *bin_mem = binning_alloc(binning_ctx, sgr_binning_bytes((int64_t)capacity));
         if (!bin_mem) {
             set_error("binning allocator returned NULL");
             return SGR_ENOMEM;
         }
-        bin = BinState::carve(bin_mem, capacity);
+        Layout bin_l(bin_mem);
+        bin = BinState::carve(bin_l, capacity);
         if (launched) {  // cursors were not advanced by the guarded attempt, but be explicit
             SGR_CUDA(cudaMemcpyAsync(img.tile_cursor, img.tile_start, sizeof(uint32_t) * T, cudaMemcpyDeviceToDevice, st));
         }

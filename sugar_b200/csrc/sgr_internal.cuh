@@ -29,23 +29,45 @@ namespace sgr {
 
 static inline size_t align_up(size_t v, size_t a = SGR_ALIGN) { return (v + a - 1) / a * a; }
 
+// Walks one buffer's layout.  Started at the buffer's base it hands out the arrays in order, each SGR_ALIGN-aligned;
+// started at null it only measures.  Every layout is one function over a Layout, called both to size the buffer and
+// to carve it, so the size a caller allocates and the arrays the kernels write cannot disagree.
+class Layout {
+  public:
+    explicit Layout(const void *base = nullptr) : start_(align_up((size_t)base)), at_(start_) {}
+    template <class T> T *take(size_t n)
+    {
+        T *p = (T *)at_;
+        at_ += align_up(n * sizeof(T));
+        return p;
+    }
+    // the bytes to allocate: what the walk consumed, plus the slack that aligns an unaligned base
+    size_t bytes() const { return at_ - start_ + SGR_ALIGN; }
+
+  private:
+    size_t start_, at_;
+};
+
+// the size of the layout `walk` takes from a Layout
+template <class Walk> size_t layout_bytes(Walk walk)
+{
+    Layout l;
+    walk(l);
+    return l.bytes();
+}
+
 struct GeomState {
     float4 *rec;
     ushort4 *rect;
     float *depth;
     float *sh_jac;  // [P][9] (dRGB/dx, dRGB/dy, dRGB/dz) of the SH colour; zero rows for culled Gaussians
-    static size_t bytes(size_t P)
+    static GeomState carve(Layout &l, size_t P)
     {
-        return align_up(P * 48) + align_up(P * 8) + align_up(P * 4) + align_up(P * 36) + SGR_ALIGN;
-    }
-    static GeomState carve(void *base, size_t P)
-    {
-        char *p = (char *)align_up((size_t)base);
         GeomState s;
-        s.rec = (float4 *)p; p += align_up(P * 48);
-        s.rect = (ushort4 *)p; p += align_up(P * 8);
-        s.depth = (float *)p; p += align_up(P * 4);
-        s.sh_jac = (float *)p;
+        s.rec = l.take<float4>(3 * P);
+        s.rect = l.take<ushort4>(P);
+        s.depth = l.take<float>(P);
+        s.sh_jac = l.take<float>(9 * P);
         return s;
     }
 };
@@ -58,23 +80,17 @@ struct ImageState {
     uint32_t *tile_cursor;  // after scatter: the end of each tile's live list [tile_start[t], tile_cursor[t])
     uint32_t *tile_order;  // tiles by decreasing instance count: launch order of the blend kernels
     uint32_t *counters;    // [0] = num_rendered, [1] = overflow flag
-    static size_t bytes(size_t W, size_t H)
+    static ImageState carve(Layout &l, size_t W, size_t H)
     {
-        size_t T = ((W + 15) / 16) * ((H + 15) / 16);
-        return 2 * align_up(W * H * 4) + 3 * align_up(T * 4) + align_up((T + 1) * 4) + align_up(64) + SGR_ALIGN;
-    }
-    static ImageState carve(void *base, size_t W, size_t H)
-    {
-        size_t T = ((W + 15) / 16) * ((H + 15) / 16);
-        char *p = (char *)align_up((size_t)base);
+        const size_t T = ((W + 15) / 16) * ((H + 15) / 16);
         ImageState s;
-        s.final_T = (float *)p; p += align_up(W * H * 4);
-        s.n_contrib = (uint32_t *)p; p += align_up(W * H * 4);
-        s.tile_count = (uint32_t *)p; p += align_up(T * 4);
-        s.tile_start = (uint32_t *)p; p += align_up((T + 1) * 4);
-        s.tile_cursor = (uint32_t *)p; p += align_up(T * 4);
-        s.tile_order = (uint32_t *)p; p += align_up(T * 4);
-        s.counters = (uint32_t *)p;
+        s.final_T = l.take<float>(W * H);
+        s.n_contrib = l.take<uint32_t>(W * H);
+        s.tile_count = l.take<uint32_t>(T);
+        s.tile_start = l.take<uint32_t>(T + 1);
+        s.tile_cursor = l.take<uint32_t>(T);
+        s.tile_order = l.take<uint32_t>(T);
+        s.counters = l.take<uint32_t>(16);
         return s;
     }
 };
@@ -85,22 +101,19 @@ struct BinState {
     uint32_t *plist;
     uint64_t *inst_a;
     uint64_t *inst_b;
-    static size_t bytes(size_t C)
+    static BinState carve(Layout &l, size_t C)
     {
         if (C == 0) C = 1;
-        return 2 * align_up(C * 8) + align_up(C * 4) + SGR_ALIGN;
-    }
-    static BinState carve(void *base, size_t C)
-    {
-        if (C == 0) C = 1;
-        char *p = (char *)align_up((size_t)base);
         BinState s;
-        s.plist = (uint32_t *)p; p += align_up(C * 4);
-        s.inst_a = (uint64_t *)p; p += align_up(C * 8);
-        s.inst_b = (uint64_t *)p;
+        s.plist = l.take<uint32_t>(C);
+        s.inst_a = l.take<uint64_t>(C);
+        s.inst_b = l.take<uint64_t>(C);
         return s;
     }
 };
+
+// the backward's blend accumulators, 32 B per Gaussian
+static inline float *carve_grad_acc(Layout &l, size_t P) { return l.take<float>(8 * P); }
 
 // Per-view constants passed by value (constant bank).  The matrices, camera position and background stay device
 // pointers, as in the reference API: kernels load them through the read-only path (16+16+3+3 floats, L1-resident).

@@ -309,12 +309,18 @@ static int knn_axis_cells(int P)
     return n;
 }
 
-size_t knn_cells_bytes(int P)
+KnnCellsScratch knn_cells_scratch(Layout &l, int P)
 {
-    const size_t n = (size_t)knn_axis_cells(P < 1 ? 1 : P), ncell = n * n * n;
-    const size_t nblocks = (ncell + 4095) / 4096;
-    return align_up(64) + align_up(sizeof(KnnGrid)) + align_up((size_t)P * 4) + 2 * align_up((ncell + 1) * 4) +
-           align_up((nblocks + 1) * 4) + align_up((size_t)P * 16) + SGR_ALIGN;
+    const size_t n = (size_t)knn_axis_cells(P), ncell = n * n * n;
+    KnnCellsScratch s;
+    s.bbox = l.take<int>(16);
+    s.grid = l.take<KnnGrid>(1);
+    s.cell_of = l.take<uint32_t>(P);
+    s.starts = l.take<uint32_t>(ncell + 1);
+    s.cursor = l.take<uint32_t>(ncell + 1);
+    s.bsums = l.take<uint32_t>(scan_block_sums(ncell));
+    s.sorted = l.take<float4>(P);
+    return s;
 }
 
 void exclusive_scan_u32(int kind, int n, const uint32_t *counts, uint32_t *starts, uint32_t *block_sums,
@@ -326,28 +332,20 @@ void exclusive_scan_u32(int kind, int n, const uint32_t *counts, uint32_t *start
     SGR_LAUNCH(kind, st, knn_scan_add_kernel<<<(unsigned)nblocks, 1024, 0, st>>>(n, starts, block_sums, cursor));
 }
 
-int knn_build_cells(int P, const float *points, void *workspace, cudaStream_t st, KnnCells *out)
+int knn_build_cells(int P, const float *points, const KnnCellsScratch &ws, cudaStream_t st, KnnCells *out)
 {
     const int n = knn_axis_cells(P);
-    const size_t ncell = (size_t)n * n * n, nblocks = (ncell + 4095) / 4096;
-    char *p = (char *)align_up((size_t)workspace);
-    int *bb = (int *)p; p += align_up(64);
-    KnnGrid *grid = (KnnGrid *)p; p += align_up(sizeof(KnnGrid));
-    uint32_t *cell_of = (uint32_t *)p; p += align_up((size_t)P * 4);
-    uint32_t *starts = (uint32_t *)p; p += align_up((ncell + 1) * 4);
-    uint32_t *cursor = (uint32_t *)p; p += align_up((ncell + 1) * 4);
-    uint32_t *bsums = (uint32_t *)p; p += align_up((nblocks + 1) * 4);
-    float4 *sorted = (float4 *)p;
-    SGR_LAUNCH(K_KNN, st, knn_bbox_init_kernel<<<1, 32, 0, st>>>(bb));
-    SGR_LAUNCH(K_KNN, st, knn_bbox_kernel<<<device_sm_count() * 4, 256, 0, st>>>(P, points, bb));
-    SGR_LAUNCH(K_KNN, st, knn_grid_setup_kernel<<<1, 32, 0, st>>>(bb, n, P, grid));
-    SGR_CUDA(cudaMemsetAsync(cursor, 0, ncell * 4, st));  // cursor doubles as the count array first
-    SGR_LAUNCH(K_KNN, st, knn_count_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, grid, cell_of, cursor));
-    exclusive_scan_u32(K_KNN, (int)ncell, cursor, starts, bsums, cursor, st);
-    SGR_LAUNCH(K_KNN, st, knn_scatter_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, cell_of, cursor, sorted));
-    out->grid = grid;
-    out->starts = starts;
-    out->sorted = sorted;
+    const size_t ncell = (size_t)n * n * n;
+    SGR_LAUNCH(K_KNN, st, knn_bbox_init_kernel<<<1, 32, 0, st>>>(ws.bbox));
+    SGR_LAUNCH(K_KNN, st, knn_bbox_kernel<<<device_sm_count() * 4, 256, 0, st>>>(P, points, ws.bbox));
+    SGR_LAUNCH(K_KNN, st, knn_grid_setup_kernel<<<1, 32, 0, st>>>(ws.bbox, n, P, ws.grid));
+    SGR_CUDA(cudaMemsetAsync(ws.cursor, 0, ncell * 4, st));  // cursor doubles as the count array first
+    SGR_LAUNCH(K_KNN, st, knn_count_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, ws.grid, ws.cell_of, ws.cursor));
+    exclusive_scan_u32(K_KNN, (int)ncell, ws.cursor, ws.starts, ws.bsums, ws.cursor, st);
+    SGR_LAUNCH(K_KNN, st, knn_scatter_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, ws.cell_of, ws.cursor, ws.sorted));
+    out->grid = ws.grid;
+    out->starts = ws.starts;
+    out->sorted = ws.sorted;
     return SGR_OK;
 }
 
@@ -357,7 +355,7 @@ using namespace sgr;
 
 extern "C" {
 
-size_t sgr_knn_workspace_bytes(int32_t P) { return knn_cells_bytes(P); }
+size_t sgr_knn_workspace_bytes(int32_t P) { return P > 0 ? layout_bytes([&](Layout &l) { knn_cells_scratch(l, P); }) : 0; }
 
 int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int32_t K, int64_t *idx, float *dist2,
             void *workspace, void *stream)
@@ -369,8 +367,9 @@ int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int
     }
     if (Q == 0) return SGR_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    Layout l(workspace);
     KnnCells cells;
-    int rc = knn_build_cells(P, points, workspace, st, &cells);
+    int rc = knn_build_cells(P, points, knn_cells_scratch(l, P), st, &cells);
     if (rc) return rc;
     SGR_LAUNCH(K_KNN_QUERY, st,
                knn_query_kernel<<<(Q + 127) / 128, 128, 0, st>>>(Q, K, P, queries, cells.grid, cells.starts,

@@ -29,11 +29,21 @@ struct KnnCells {
     const float4 *sorted;
 };
 
-size_t knn_cells_bytes(int P);  // workspace of knn_build_cells
-int knn_build_cells(int P, const float *points, void *workspace, cudaStream_t st, KnnCells *out);
+// knn_build_cells' workspace
+struct KnnCellsScratch {
+    int *bbox;
+    KnnGrid *grid;
+    uint32_t *cell_of, *starts, *cursor, *bsums;
+    float4 *sorted;
+};
+KnnCellsScratch knn_cells_scratch(Layout &l, int P);
+int knn_build_cells(int P, const float *points, const KnnCellsScratch &ws, cudaStream_t st, KnnCells *out);
+
+// The block sums exclusive_scan_u32 needs for n counts.
+static inline size_t scan_block_sums(size_t n) { return (n + 4095) / 4096 + 1; }
 
 // Exclusive scan of n uint32 counts into starts (counts == starts is allowed), written to cursor as well;
-// block_sums holds (n + 4095) / 4096 + 1 entries.  Three launches under `kind`.
+// block_sums holds scan_block_sums(n) entries.  Three launches under `kind`.
 void exclusive_scan_u32(int kind, int n, const uint32_t *counts, uint32_t *starts, uint32_t *block_sums,
                         uint32_t *cursor, cudaStream_t st);
 

@@ -264,6 +264,12 @@ static int loss_check(const SgrSsimParams *p, LossGrid &g, const char *who)
     return SGR_OK;
 }
 
+// the forward's per-(block, channel) partial sums, one per tile of every plane
+static double2 *loss_partials(Layout &l, const LossGrid &g)
+{
+    return l.take<double2>((size_t)g.grid.x * g.grid.y * g.grid.z);
+}
+
 static LossConsts loss_consts(const SgrSsimParams *p)
 {
     LossConsts k;
@@ -284,9 +290,11 @@ extern "C" {
 
 size_t sgr_l1_ssim_scratch_bytes(int32_t B, int32_t C, int32_t H, int32_t W)
 {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return 0;
-    const size_t tiles = (size_t)((W + LT_X - 1) / LT_X) * ((H + LT_Y - 1) / LT_Y);
-    return align_up((size_t)B * C * tiles * sizeof(double2)) + SGR_ALIGN;
+    SgrSsimParams p = {};
+    p.B = B, p.C = C, p.H = H, p.W = W;
+    LossGrid g;
+    if (loss_check(&p, g, "sgr_l1_ssim_scratch_bytes")) return 0;
+    return layout_bytes([&](Layout &l) { loss_partials(l, g); });
 }
 
 int sgr_l1_ssim_forward(const SgrSsimParams *p, const float *img1, const float *img2, float *partial_maps,
@@ -301,7 +309,8 @@ int sgr_l1_ssim_forward(const SgrSsimParams *p, const float *img1, const float *
     }
     cudaStream_t st = (cudaStream_t)stream;
     const LossConsts k = loss_consts(p);
-    double2 *partials = (double2 *)align_up((size_t)scratch);
+    Layout l(scratch);
+    double2 *partials = loss_partials(l, g);
     static DeviceOnce attributes;
     rc = once_per_device(attributes, []() -> int {
         SGR_CUDA(cudaFuncSetAttribute(loss_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,

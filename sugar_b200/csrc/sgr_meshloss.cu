@@ -174,6 +174,10 @@ __global__ void __launch_bounds__(NC_THREADS) mesh_nc_vertex_sum_kernel(int V, c
 
 static int nc_blocks(int n) { return (n + NC_THREADS - 1) / NC_THREADS; }
 
+// the forward's per-block partial sums; the backward's per-pair gradients (four vertices x 3 floats)
+static double *nc_partials(Layout &l, int Q) { return l.take<double>(nc_blocks(Q)); }
+static float4 *nc_pair_grads(Layout &l, int Q) { return l.take<float4>(3 * (size_t)Q); }
+
 static bool nc_sizes_ok(int32_t Q, int32_t V, const char *who)
 {
     if (Q < 0 || V < 0 || Q > INT32_MAX / 4) {
@@ -205,16 +209,15 @@ extern "C" void mesh_nc_host(int Q, const float *verts, const int *pairs, double
 #else
 extern "C" {
 
+// Q == 0 needs no scratch
 size_t sgr_mesh_nc_forward_scratch_bytes(int32_t Q)
 {
-    if (Q <= 0) return 0;
-    return align_up((size_t)nc_blocks(Q) * sizeof(double)) + SGR_ALIGN;
+    return Q > 0 && Q <= INT32_MAX / 4 ? layout_bytes([&](Layout &l) { nc_partials(l, Q); }) : 0;
 }
 
 size_t sgr_mesh_nc_backward_scratch_bytes(int32_t Q)
 {
-    if (Q <= 0 || Q > INT32_MAX / 4) return 0;
-    return align_up((size_t)Q * 12 * sizeof(float)) + SGR_ALIGN;
+    return Q > 0 && Q <= INT32_MAX / 4 ? layout_bytes([&](Layout &l) { nc_pair_grads(l, Q); }) : 0;
 }
 
 int sgr_mesh_nc_forward(int32_t Q, int32_t V, const float *verts, const int32_t *pairs, float *loss, void *scratch,
@@ -230,7 +233,8 @@ int sgr_mesh_nc_forward(int32_t Q, int32_t V, const float *verts, const int32_t 
         SGR_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), st));
         return SGR_OK;
     }
-    double *partials = (double *)align_up((size_t)scratch);
+    Layout l(scratch);
+    double *partials = nc_partials(l, Q);
     const int nb = nc_blocks(Q);
     SGR_LAUNCH(K_MESH_NC_FWD, st,
                mesh_nc_forward_kernel<<<nb, NC_THREADS, 0, st>>>(Q, verts, (const int4 *)pairs, partials));
@@ -253,7 +257,8 @@ int sgr_mesh_nc_backward(int32_t Q, int32_t V, const float *verts, const int32_t
         if (V > 0) SGR_CUDA(cudaMemsetAsync(g_verts, 0, sizeof(float) * 3 * (size_t)V, st));
         return SGR_OK;
     }
-    float4 *pair_grads = (float4 *)align_up((size_t)scratch);
+    Layout l(scratch);
+    float4 *pair_grads = nc_pair_grads(l, Q);
     SGR_LAUNCH(K_MESH_NC_BWD, st,
                mesh_nc_pair_grad_kernel<<<nc_blocks(Q), NC_THREADS, 0, st>>>(Q, verts, (const int4 *)pairs, g_loss,
                                                                              1.0 / (double)Q, pair_grads));

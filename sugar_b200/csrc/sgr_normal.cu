@@ -219,13 +219,21 @@ static int group_width_n(int K)
     return G;
 }
 
+// the packed records, then the backward's per-Gaussian normal gradients
+struct NormalScratch {
+    float4 *rec;
+    float *dnrm;
+};
+
+static NormalScratch normal_scratch(Layout &l, size_t P) { return {l.take<float4>(2 * P), l.take<float>(4 * P)}; }
+
 }  // namespace sgr
 
 using namespace sgr;
 
 extern "C" {
 
-size_t sgr_normal_scratch_bytes(int32_t P) { return align_up((size_t)(P < 0 ? 0 : P) * 32) + align_up((size_t)(P < 0 ? 0 : P) * 16) + SGR_ALIGN; }
+size_t sgr_normal_scratch_bytes(int32_t P) { return P > 0 ? layout_bytes([&](Layout &l) { normal_scratch(l, P); }) : 0; }
 
 static int normal_check(int N, int K, int P, const void *x, const void *own, const void *idx, const void *a,
                         const void *b, const void *c, const void *d, const void *e, const void *scratch)
@@ -249,7 +257,8 @@ int sgr_normal_loss_forward(int32_t N, int32_t K, int32_t P, const float *x, con
     if (rc) return rc;
     if (N == 0) return SGR_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    float4 *rec = (float4 *)align_up((size_t)scratch);
+    Layout l(scratch);
+    float4 *rec = normal_scratch(l, P).rec;
     SGR_LAUNCH(K_FIELD_PACK, st, normal_pack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec));
     NormalArgs a{N, K, x, own_idx, nbr_idx, rec, nbr_opacity};
     const int G = group_width_n(K), blocks = (N + 256 / G - 1) / (256 / G);
@@ -279,8 +288,8 @@ int sgr_normal_loss_backward(int32_t N, int32_t K, int32_t P, const float *x, co
         return SGR_EINVAL;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    float4 *rec = (float4 *)align_up((size_t)scratch);
-    float *dnrm = (float *)((char *)rec + align_up((size_t)P * 32));
+    Layout l(scratch);
+    const auto [rec, dnrm] = normal_scratch(l, P);
     SGR_CUDA(cudaMemsetAsync(dnrm, 0, (size_t)P * 16, st));
     if (N > 0) {
         SGR_LAUNCH(K_FIELD_PACK, st, normal_pack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec));

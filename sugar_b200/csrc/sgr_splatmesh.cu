@@ -320,23 +320,23 @@ struct RasterScratch {
     unsigned *npieces;
     unsigned long long *off, *block_sums, *keys;
     static int scan_blocks(int F) { return (F + SCAN_BLOCK - 1) / SCAN_BLOCK; }
-    static size_t bytes(int F, int W, int H)
+    static RasterScratch carve(Layout &l, int F, int W, int H)
     {
-        return align_up((size_t)F * sizeof(FaceSetup)) + align_up((size_t)F * 4) + align_up(((size_t)F + 1) * 8) +
-               align_up((size_t)scan_blocks(F) * 8 + 8) + align_up((size_t)W * H * 8) + SGR_ALIGN;
-    }
-    static RasterScratch carve(void *base, int F, int W, int H)
-    {
-        char *p = (char *)align_up((size_t)base);
         RasterScratch s;
-        s.rec = (FaceSetup *)p; p += align_up((size_t)F * sizeof(FaceSetup));
-        s.npieces = (unsigned *)p; p += align_up((size_t)F * 4);
-        s.off = (unsigned long long *)p; p += align_up(((size_t)F + 1) * 8);
-        s.block_sums = (unsigned long long *)p; p += align_up((size_t)scan_blocks(F) * 8 + 8);
-        s.keys = (unsigned long long *)p;
+        s.rec = l.take<FaceSetup>(F);
+        s.npieces = l.take<unsigned>(F);
+        s.off = l.take<unsigned long long>((size_t)F + 1);
+        s.block_sums = l.take<unsigned long long>((size_t)scan_blocks(F) + 1);
+        s.keys = l.take<unsigned long long>((size_t)W * H);
         return s;
     }
 };
+
+// the packed key keeps the face id in 32 bits: F <= 2^31 - 1 by its type, so ~0 never names a face
+static bool raster_sizes_ok(int F, int W, int H)
+{
+    return F >= 0 && W >= 0 && H >= 0 && W <= 65535 && H <= 65535 && (long long)W * H <= INT32_MAX;
+}
 
 }  // namespace sgr
 
@@ -371,16 +371,14 @@ int sgr_splat_mesh(int32_t P, const float *points, const float *scaling, const f
 
 size_t sgr_mesh_raster_scratch_bytes(int32_t F, int32_t W, int32_t H)
 {
-    if (F < 0 || W < 0 || H < 0) return 0;
-    return RasterScratch::bytes(F, W, H);
+    return raster_sizes_ok(F, W, H) ? layout_bytes([&](Layout &l) { RasterScratch::carve(l, F, W, H); }) : 0;
 }
 
 int sgr_mesh_raster(int32_t V, int32_t F, const float *verts, const int64_t *faces, const float *viewmatrix,
                     const float *projmatrix, int32_t W, int32_t H, float *zbuf, int64_t *pix_to_face, void *scratch,
                     void *stream)
 {
-    // the packed key keeps the face id in 32 bits: F <= 2^31 - 1 by its type, so ~0 never names a face
-    if (V < 0 || F < 0 || W < 0 || H < 0 || W > 65535 || H > 65535 || (long long)W * H > INT32_MAX) {
+    if (V < 0 || !raster_sizes_ok(F, W, H)) {
         set_error("sgr_mesh_raster: bad sizes V=%d F=%d W=%d H=%d (W, H <= 65535, W*H <= 2^31 - 1)", V, F, W, H);
         return SGR_EINVAL;
     }
@@ -391,7 +389,8 @@ int sgr_mesh_raster(int32_t V, int32_t F, const float *verts, const int64_t *fac
         return SGR_EINVAL;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    RasterScratch s = RasterScratch::carve(scratch, F, W, H);
+    Layout l(scratch);
+    const RasterScratch s = RasterScratch::carve(l, F, W, H);
     SGR_CUDA(cudaMemsetAsync(s.keys, 0xff, (size_t)n_pix * 8, st));
     if (F > 0) {
         // pytorch3d drops |area| <= 1e-8 in its NDC units, 2 / min(W, H) per pixel

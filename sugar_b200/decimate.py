@@ -22,16 +22,7 @@ colours and normals are averaged in float64; the non-manifold pass visits edges 
 import numpy as np
 import torch
 
-from ._lib import check, lib
-from .splatmesh import _stream
-
-
-def _vec3(t, name, n, dev):
-    if t is None:
-        return None
-    if not torch.is_tensor(t) or t.dtype != torch.float32 or tuple(t.shape) != (n, 3) or t.device != dev:
-        raise ValueError(f"{name} must be a float32 tensor [{n},3] on {dev}")
-    return t.contiguous()
+from ._lib import check, lib, ptr, require_cuda, scratch, stream, tensor
 
 
 def simplify_quadric_decimation(verts, faces, target, colors=None, normals=None):
@@ -40,29 +31,24 @@ def simplify_quadric_decimation(verts, faces, target, colors=None, normals=None)
     [V,3].  -> {"verts" f32 [V',3], "faces" i64 [F',3], "colors", "normals" (None when not given), "rounds": int,
     "last_removed": faces removed by the collapse that reached the target (0 if it was not reached)}.
     F' <= target unless no edge can be collapsed; the vertices are those the faces reference, in their order."""
-    if not torch.is_tensor(verts) or not verts.is_cuda:
-        raise RuntimeError("sugar_b200.decimate needs CUDA tensors: there is no CPU fallback")
+    require_cuda("decimate", verts)
     dev = verts.device
-    if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
-        raise ValueError(f"verts must be float32 [V,3], got {verts.dtype} {tuple(verts.shape)}")
-    if not torch.is_tensor(faces) or faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3 or \
-            faces.device != dev:
-        raise ValueError(f"faces must be an int64 tensor [F,3] on {dev}")
+    verts = tensor(verts, "verts", torch.float32, ("V", 3))
+    faces = tensor(faces, "faces", torch.int64, ("F", 3), dev)
     target = int(target)
     if target < 0:
         raise ValueError(f"target = {target}: must be >= 0")
     V, F = verts.shape[0], faces.shape[0]
-    verts, faces = verts.contiguous(), faces.contiguous()
-    colors, normals = _vec3(colors, "colors", V, dev), _vec3(normals, "normals", V, dev)
-    ptr = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()
+    colors = None if colors is None else tensor(colors, "colors", torch.float32, (V, 3), dev)
+    normals = None if normals is None else tensor(normals, "normals", torch.float32, (V, 3), dev)
     with torch.cuda.device(dev):
-        scratch = torch.empty(lib.sgr_decimate_scratch_bytes(V, F), dtype=torch.uint8, device=dev)
+        ws = scratch(lib.sgr_decimate_scratch_bytes(V, F), dev)
         vo, fo = torch.empty_like(verts), torch.empty_like(faces)
         co = None if colors is None else torch.empty_like(colors)
         no = None if normals is None else torch.empty_like(normals)
         res = np.zeros(4, np.int64)
         check(lib.sgr_decimate(V, F, target, ptr(verts), ptr(faces), ptr(colors), ptr(normals), ptr(vo), ptr(fo),
-                               ptr(co), ptr(no), res.ctypes.data, scratch.data_ptr(), _stream(dev)))
+                               ptr(co), ptr(no), res.ctypes.data, ws.data_ptr(), stream(dev)))
     nv, nf = int(res[0]), int(res[1])
     cut = lambda t, n: None if t is None else t[:n].clone()
     return {"verts": cut(vo, nv), "faces": cut(fo, nf), "colors": cut(co, nv), "normals": cut(no, nv),

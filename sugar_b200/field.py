@@ -18,7 +18,7 @@ import ctypes as C
 
 import torch
 
-from ._lib import SgrFieldParams, check, lib
+from ._lib import SgrFieldParams, check, lib, ptr, require_cuda, scratch, stream, tensor
 
 
 def _params(N, K, P, density_factor, density_threshold, opacity_min_clamp, group=1):
@@ -31,8 +31,12 @@ def _params(N, K, P, density_factor, density_threshold, opacity_min_clamp, group
     return p
 
 
-def _ptr(t):
-    return None if t is None else t.data_ptr()
+def _gaussians(dev, points, scaling, quaternions):
+    """The Gaussians' float32 [P,3] centres, [P,3] scales and [P,4] quaternions on the samples' device."""
+    points = tensor(points.float(), "points", torch.float32, ("P", 3), dev, "x")
+    P = points.shape[0]
+    return (points, tensor(scaling.float(), "scaling", torch.float32, (P, 3), dev, "x"),
+            tensor(quaternions.float(), "quaternions", torch.float32, (P, 4), dev, "x"))
 
 
 class _Field(torch.autograd.Function):
@@ -41,26 +45,30 @@ class _Field(torch.autograd.Function):
                 opacity_min_clamp, group=1, outputs=7):
         """outputs: bit 0 nbr_opacity, bit 1 beta, bit 2 sdf -- unrequested ones are neither allocated nor
         written (they come back as empty tensors)."""
-        if not x.is_cuda:
-            raise RuntimeError("sugar_b200.field needs CUDA tensors: there is no CPU fallback")
-        x, points, scaling, quaternions = (t.contiguous().float() for t in (x, points, scaling, quaternions))
-        strengths = strengths.contiguous().float()
-        nbr_idx = nbr_idx.contiguous().long()
-        N, K, P = x.shape[0], nbr_idx.shape[1], points.shape[0]
+        dev = x.device
+        x = tensor(x.float(), "x", torch.float32, ("N", 3))
+        points, scaling, quaternions = _gaussians(dev, points, scaling, quaternions)
+        N, P = x.shape[0], points.shape[0]
+        strengths = strengths.float()
+        if tuple(strengths.shape) not in ((P,), (P, 1)):
+            raise ValueError(f"strengths must be float32 [{P}] or [{P},1], got {tuple(strengths.shape)}")
+        strengths = tensor(strengths, "strengths", torch.float32, strengths.shape, dev, "x")
+        nbr_idx = tensor(nbr_idx.long(), "closest_gaussians_idx", torch.int64, ("M", "K"), dev, "x")
+        K = nbr_idx.shape[1]
         if nbr_idx.shape[0] * group < N:
             raise RuntimeError("closest_gaussians_idx has too few rows for the samples")
-        dev = x.device
+        require_cuda("field", x)
         with torch.cuda.device(dev):
             density = torch.empty(N, device=dev)
             nbr = torch.empty((N, K) if outputs & 1 else (0, K), device=dev)
             beta = torch.empty(N if outputs & 2 else 0, device=dev)
             sdf = torch.empty(N if outputs & 4 else 0, device=dev)
-            scratch = torch.empty(lib.sgr_field_scratch_bytes(P), dtype=torch.uint8, device=dev)
+            ws = scratch(lib.sgr_field_scratch_bytes(P), dev)
             p = _params(N, K, P, density_factor, density_threshold, opacity_min_clamp, group)
-            check(lib.sgr_field_forward(C.byref(p), _ptr(x), _ptr(nbr_idx), _ptr(points), _ptr(scaling),
-                                        _ptr(quaternions), _ptr(strengths), _ptr(density),
-                                        _ptr(nbr) if outputs & 1 else None, _ptr(beta) if outputs & 2 else None,
-                                        _ptr(sdf) if outputs & 4 else None, _ptr(scratch), torch.cuda.current_stream(dev).cuda_stream))
+            check(lib.sgr_field_forward(C.byref(p), ptr(x), ptr(nbr_idx), ptr(points), ptr(scaling), ptr(quaternions),
+                                        ptr(strengths), ptr(density), ptr(nbr) if outputs & 1 else None,
+                                        ptr(beta) if outputs & 2 else None, ptr(sdf) if outputs & 4 else None,
+                                        ptr(ws), stream(dev)))
         ctx.save_for_backward(x, nbr_idx, points, scaling, quaternions, strengths)
         ctx.cfg = (density_factor, density_threshold, opacity_min_clamp, strengths.shape, group, outputs)
         ctx.mark_non_differentiable(nbr_idx)
@@ -81,31 +89,34 @@ class _Field(torch.autograd.Function):
             g_scaling = torch.empty_like(scaling)
             g_quat = torch.empty_like(quaternions)
             g_str = torch.empty(P, device=dev)
-            scratch = torch.empty(lib.sgr_field_scratch_bytes(P), dtype=torch.uint8, device=dev)
+            ws = scratch(lib.sgr_field_scratch_bytes(P), dev)
             p = _params(N, K, P, density_factor, density_threshold, opacity_min_clamp, group)
-            check(lib.sgr_field_backward(C.byref(p), _ptr(x), _ptr(nbr_idx), _ptr(points), _ptr(scaling),
-                                         _ptr(quaternions), _ptr(strengths), _ptr(g_density), _ptr(g_nbr), _ptr(g_beta),
-                                         _ptr(g_sdf), _ptr(g_x), _ptr(g_points), _ptr(g_scaling), _ptr(g_quat),
-                                         _ptr(g_str), _ptr(scratch), torch.cuda.current_stream(dev).cuda_stream))
+            check(lib.sgr_field_backward(C.byref(p), ptr(x), ptr(nbr_idx), ptr(points), ptr(scaling),
+                                         ptr(quaternions), ptr(strengths), ptr(g_density), ptr(g_nbr), ptr(g_beta),
+                                         ptr(g_sdf), ptr(g_x), ptr(g_points), ptr(g_scaling), ptr(g_quat),
+                                         ptr(g_str), ptr(ws), stream(dev)))
         return g_x, None, g_points, g_scaling, g_quat, g_str.view(s_shape), None, None, None, None, None
 
 
 class _NormalLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gaussian_idx, nbr_idx, points, scaling, quaternions, nbr_opacity):
-        if not x.is_cuda:
-            raise RuntimeError("sugar_b200.field needs CUDA tensors: there is no CPU fallback")
-        x, points, scaling, quaternions, nbr_opacity = (t.detach().contiguous().float()
-                                                        for t in (x, points, scaling, quaternions, nbr_opacity))
-        gaussian_idx, nbr_idx = gaussian_idx.contiguous().long(), nbr_idx.contiguous().long()
-        N, K, P = x.shape[0], nbr_idx.shape[1], points.shape[0]
         dev = x.device
+        x = tensor(x.detach().float(), "x", torch.float32, ("N", 3))
+        points, scaling, quaternions = _gaussians(dev, points.detach(), scaling.detach(), quaternions.detach())
+        N, P = x.shape[0], points.shape[0]
+        gaussian_idx = tensor(gaussian_idx.long(), "gaussian_idx", torch.int64, (N,), dev, "x")
+        nbr_idx = tensor(nbr_idx.long(), "closest_gaussians_idx", torch.int64, (N, "K"), dev, "x")
+        K = nbr_idx.shape[1]
+        nbr_opacity = tensor(nbr_opacity.detach().float(), "closest_gaussian_opacities", torch.float32, (N, K), dev,
+                             "x")
+        require_cuda("field", x)
         with torch.cuda.device(dev):
             loss = torch.empty(N, device=dev)
-            scratch = torch.empty(lib.sgr_normal_scratch_bytes(P), dtype=torch.uint8, device=dev)
-            check(lib.sgr_normal_loss_forward(N, K, P, _ptr(x), _ptr(gaussian_idx), _ptr(nbr_idx), _ptr(points),
-                                              _ptr(scaling), _ptr(quaternions), _ptr(nbr_opacity), _ptr(loss),
-                                              _ptr(scratch), torch.cuda.current_stream(dev).cuda_stream))
+            ws = scratch(lib.sgr_normal_scratch_bytes(P), dev)
+            check(lib.sgr_normal_loss_forward(N, K, P, ptr(x), ptr(gaussian_idx), ptr(nbr_idx), ptr(points),
+                                              ptr(scaling), ptr(quaternions), ptr(nbr_opacity), ptr(loss), ptr(ws),
+                                              stream(dev)))
         ctx.save_for_backward(x, gaussian_idx, nbr_idx, points, scaling, quaternions, nbr_opacity)
         return loss
 
@@ -116,11 +127,10 @@ class _NormalLoss(torch.autograd.Function):
         dev = x.device
         with torch.cuda.device(dev):
             g_quat = torch.empty_like(quaternions)
-            scratch = torch.empty(lib.sgr_normal_scratch_bytes(P), dtype=torch.uint8, device=dev)
-            check(lib.sgr_normal_loss_backward(N, K, P, _ptr(x), _ptr(gaussian_idx), _ptr(nbr_idx), _ptr(points),
-                                               _ptr(scaling), _ptr(quaternions), _ptr(nbr_opacity),
-                                               _ptr(g_loss.contiguous().float()), _ptr(g_quat), _ptr(scratch),
-                                               torch.cuda.current_stream(dev).cuda_stream))
+            ws = scratch(lib.sgr_normal_scratch_bytes(P), dev)
+            check(lib.sgr_normal_loss_backward(N, K, P, ptr(x), ptr(gaussian_idx), ptr(nbr_idx), ptr(points),
+                                               ptr(scaling), ptr(quaternions), ptr(nbr_opacity),
+                                               ptr(g_loss.contiguous().float()), ptr(g_quat), ptr(ws), stream(dev)))
         return None, None, None, None, None, g_quat, None
 
 
@@ -134,7 +144,8 @@ def better_normal_loss(x, gaussian_idx, closest_gaussians_idx, points, scaling, 
     Normals are SuGaR.get_normals(estimate_from_points=False) of an unbound model, i.e. the smallest
     axis of each Gaussian (sugar_model.py:930-968).  Only the trainers' setting
     sdf_better_normal_gradient_through_normal_only=True (coarse_sdf.py:144) is implemented: gradients
-    flow to `quaternions` alone."""
+    flow to `quaternions` alone.  Shapes, dtypes and devices are checked (ValueError); index ranges are not, which
+    would cost a host synchronisation per step."""
     if not gradient_through_normal_only:
         raise NotImplementedError("only sdf_better_normal_gradient_through_normal_only=True (the reference "
                                   "trainers' fixed setting, coarse_sdf.py:144) is implemented")
@@ -152,7 +163,8 @@ def field_values(x, closest_gaussians_idx, points, scaling, quaternions, strengt
     mode every trainer and extractor of the reference constructs its model with; 'learnable' / 'weighted_average'
     raise.  `return_sdf_grad` adds fields['sdf_grad'] (:1307-1314) as a VALUE (detached, clamped to
     +-sdf_grad_max_value): it is beta / (rho sqrt(-2 ln rho)) times minus the density's spatial gradient, which the
-    fused backward kernel delivers; no caller of the reference differentiates through it."""
+    fused backward kernel delivers; no caller of the reference differentiates through it.  Shapes, dtypes and devices
+    are checked (ValueError); index ranges are not, which would cost a host synchronisation per step."""
     if beta_mode != "average":
         raise NotImplementedError(f"beta_mode={beta_mode!r}: only 'average' is implemented (sugar_model.py:1192-1195)")
     density, nbr, beta, sdf = _Field.apply(x, closest_gaussians_idx, points, scaling, quaternions, strengths,

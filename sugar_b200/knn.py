@@ -6,23 +6,29 @@ SuGaR uses it (sugar_scene/sugar_model.py:1013-1030 reset_neighbors, :1335-1343)
 """
 import torch
 
-from ._lib import check, lib
+from ._lib import check, lib, ptr, require_cuda, scratch, stream, tensor
+
+
+def _cloud(p, name, dev=None):
+    """[N,3] or pytorch3d's batched [1,N,3] -> float32 [N,3]."""
+    p = p.float()
+    return tensor(p[0] if p.dim() == 3 and p.shape[0] == 1 else p, name, torch.float32, ("N", 3), dev, "p1")
 
 
 def knn_points(p1: torch.Tensor, p2: torch.Tensor, K: int):
-    """K nearest points of p2 for every point of p1.  Accepts [N,3] or pytorch3d's batched [1,N,3]."""
+    """K nearest points of p2 for every point of p1.  Accepts [N,3] or pytorch3d's batched [1,N,3].  Shapes and
+    devices are checked (ValueError)."""
     batched = p1.dim() == 3
-    q = (p1[0] if batched else p1).contiguous().float()
-    r = (p2[0] if p2.dim() == 3 else p2).contiguous().float()
-    if not q.is_cuda or not r.is_cuda:
-        raise RuntimeError("sugar_b200.knn needs CUDA tensors: there is no CPU fallback")
-    Q, P, dev = q.shape[0], r.shape[0], q.device
+    q = _cloud(p1, "p1")
+    dev = q.device
+    r = _cloud(p2, "p2", dev)
+    require_cuda("knn", q, r)
+    Q, P = q.shape[0], r.shape[0]
     with torch.cuda.device(dev):
         idx = torch.empty((Q, K), dtype=torch.int64, device=dev)
         d2 = torch.empty((Q, K), dtype=torch.float32, device=dev)
-        ws = torch.empty(lib.sgr_knn_workspace_bytes(P), dtype=torch.uint8, device=dev)
-        check(lib.sgr_knn(P, r.data_ptr(), Q, q.data_ptr() if Q else None, K, idx.data_ptr() if Q else None,
-                          d2.data_ptr() if Q else None, ws.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+        ws = scratch(lib.sgr_knn_workspace_bytes(P), dev)
+        check(lib.sgr_knn(P, r.data_ptr(), Q, ptr(q), K, ptr(idx), ptr(d2), ptr(ws), stream(dev)))
     return (d2[None], idx[None]) if batched else (d2, idx)
 
 

@@ -15,7 +15,7 @@ import math
 
 import torch
 
-from ._lib import SgrSsimParams, check, lib
+from ._lib import SgrSsimParams, check, lib, require_cuda, scratch, stream
 
 C1 = 0.01 ** 2
 C2 = 0.03 ** 2
@@ -42,10 +42,6 @@ def _params(B, Cc, H, W):
     return p
 
 
-def _ptr(t):
-    return t.data_ptr()
-
-
 class _L1Ssim(torch.autograd.Function):
     """(img1 [B,C,H,W], img2 [B,C,H,W]) -> (per-image mean |img1 - img2| [B], per-image mean SSIM [B])."""
 
@@ -57,10 +53,10 @@ class _L1Ssim(torch.autograd.Function):
         with torch.cuda.device(dev):
             maps = torch.empty((3,) + img1.shape, device=dev)
             out = torch.empty(B, 2, device=dev)
-            scratch = torch.empty(lib.sgr_l1_ssim_scratch_bytes(B, Cc, H, W), dtype=torch.uint8, device=dev)
+            ws = scratch(lib.sgr_l1_ssim_scratch_bytes(B, Cc, H, W), dev)
             p = _params(B, Cc, H, W)
-            check(lib.sgr_l1_ssim_forward(C.byref(p), _ptr(img1), _ptr(img2), _ptr(maps), _ptr(out), _ptr(scratch),
-                                          torch.cuda.current_stream(dev).cuda_stream))
+            check(lib.sgr_l1_ssim_forward(C.byref(p), img1.data_ptr(), img2.data_ptr(), maps.data_ptr(),
+                                          out.data_ptr(), ws.data_ptr(), stream(dev)))
         ctx.save_for_backward(img1, img2, maps)
         return out[:, 0], out[:, 1]
 
@@ -74,8 +70,8 @@ class _L1Ssim(torch.autograd.Function):
             g_l1, g_ssim = g(g_l1), g(g_ssim)
             grad = torch.empty_like(img1)
             p = _params(B, Cc, H, W)
-            check(lib.sgr_l1_ssim_backward(C.byref(p), _ptr(img1), _ptr(img2), _ptr(maps), _ptr(g_l1), _ptr(g_ssim),
-                                           _ptr(grad), torch.cuda.current_stream(dev).cuda_stream))
+            check(lib.sgr_l1_ssim_backward(C.byref(p), img1.data_ptr(), img2.data_ptr(), maps.data_ptr(),
+                                           g_l1.data_ptr(), g_ssim.data_ptr(), grad.data_ptr(), stream(dev)))
         return grad, None
 
 
@@ -84,8 +80,7 @@ def l1_ssim_per_image(img1, img2, window_size=11):
     [C,H,W] inputs count as one image.  Differentiable with respect to img1 only."""
     if window_size != 11:
         raise NotImplementedError(f"window_size={window_size}: only the reference's 11x11 window is implemented")
-    if not (img1.is_cuda and img2.is_cuda):
-        raise RuntimeError("sugar_b200.loss needs CUDA tensors: there is no CPU fallback")
+    require_cuda("loss", img1, img2)
     if img2.requires_grad:
         raise RuntimeError("sugar_b200.loss differentiates the first image only: the second (the target) must not "
                            "require grad")

@@ -19,7 +19,7 @@ from types import SimpleNamespace
 
 import torch
 
-from ._lib import check, lib
+from ._lib import check, lib, require_cuda, stream, tensor
 
 
 def bary_coords(n_gaussians_per_surface_triangle: int, device=None) -> torch.Tensor:
@@ -35,24 +35,28 @@ def bary_coords(n_gaussians_per_surface_triangle: int, device=None) -> torch.Ten
 class _MeshBind(torch.autograd.Function):
     @staticmethod
     def forward(ctx, verts, faces, bary, scales_raw, complex_raw, thickness):
-        if not verts.is_cuda:
-            raise RuntimeError("sugar_b200.meshbind needs CUDA tensors: there is no CPU fallback")
-        verts, scales_raw, complex_raw = (t.contiguous().float() for t in (verts, scales_raw, complex_raw))
-        faces = faces.contiguous().long()
-        bary = bary.reshape(-1, 3).contiguous().float()
+        dev = verts.device
+        verts = tensor(verts.float(), "verts", torch.float32, ("V", 3))
+        faces = tensor(faces.long(), "faces", torch.int64, ("F", 3), dev)
+        bary = bary.float()
+        if bary.dim() == 3 and bary.shape[2] == 1:      # the reference's [n,3,1]
+            bary = bary[..., 0]
+        bary = tensor(bary, "bary", torch.float32, ("n", 3), dev)
         F, n, V = faces.shape[0], bary.shape[0], verts.shape[0]
         P = F * n
+        scales_raw, complex_raw = scales_raw.float(), complex_raw.float()
         if scales_raw.shape != (P, 2) or complex_raw.shape != (P, 2):
             raise RuntimeError(f"_scales / _quaternions of a mesh-bound model must be [{P}, 2]")
-        dev = verts.device
+        scales_raw = tensor(scales_raw, "scales_raw", torch.float32, (P, 2), dev)
+        complex_raw = tensor(complex_raw, "complex_raw", torch.float32, (P, 2), dev)
+        require_cuda("meshbind", verts)
         with torch.cuda.device(dev):
             points = torch.empty((P, 3), device=dev)
             scaling = torch.empty((P, 3), device=dev)
             quats = torch.empty((P, 4), device=dev)
             check(lib.sgr_meshbind_forward(F, n, V, verts.data_ptr(), faces.data_ptr(), bary.data_ptr(),
                                            scales_raw.data_ptr(), complex_raw.data_ptr(), float(thickness),
-                                           points.data_ptr(), scaling.data_ptr(), quats.data_ptr(),
-                                           torch.cuda.current_stream(dev).cuda_stream))
+                                           points.data_ptr(), scaling.data_ptr(), quats.data_ptr(), stream(dev)))
         ctx.save_for_backward(verts, faces, bary, scales_raw, complex_raw)
         ctx.mark_non_differentiable(faces)
         return points, scaling, quats
@@ -73,13 +77,14 @@ class _MeshBind(torch.autograd.Function):
             check(lib.sgr_meshbind_backward(F, n, V, verts.data_ptr(), faces.data_ptr(), bary.data_ptr(),
                                             scales_raw.data_ptr(), complex_raw.data_ptr(), g_points.data_ptr(),
                                             g_scaling.data_ptr(), g_quats.data_ptr(), g_verts.data_ptr(), g_s.data_ptr(),
-                                            g_c.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+                                            g_c.data_ptr(), stream(dev)))
         return g_verts, None, None, g_s, g_c, None
 
 
 def bind_to_mesh(verts, faces, bary, scales_raw, complex_raw, thickness):
     """verts [V,3] (SuGaR._points of a bound model), faces [F,3] int64 (_surface_mesh_faces), bary [n,3] or the
     reference's [n,3,1], scales_raw [F*n,2] (_scales), complex_raw [F*n,2] (_quaternions), thickness (float:
-    surface_mesh_thickness).  Returns namespace(points, scaling, quaternions)."""
+    surface_mesh_thickness).  Returns namespace(points, scaling, quaternions).  Shapes, dtypes and devices are checked
+    (ValueError); face ids are not range-checked, which would cost a host synchronisation per step."""
     points, scaling, quats = _MeshBind.apply(verts, faces, bary, scales_raw, complex_raw, float(thickness))
     return SimpleNamespace(points=points, scaling=scaling, quaternions=quats)

@@ -19,7 +19,7 @@ from typing import NamedTuple
 
 import torch
 
-from ._lib import check, lib
+from ._lib import check, lib, ptr, require_cuda, scratch, stream, tensor
 
 INT32_MAX = 2 ** 31 - 1
 
@@ -43,8 +43,7 @@ def mesh_topology(faces: torch.Tensor, n_verts: int) -> MeshTopology:
 
     Sort / unique / scan on the device with one host read (the pair count, together with the count of face ids
     outside [0, n_verts), which raise ValueError).  The caller keeps the result for as long as the faces stay."""
-    if not faces.is_cuda:
-        raise RuntimeError("sugar_b200.meshloss needs CUDA tensors: there is no CPU fallback")
+    require_cuda("meshloss", faces)
     if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
         raise ValueError(f"faces must be an integer [F,3] tensor, got {faces.dtype} {tuple(faces.shape)}")
     with torch.cuda.device(faces.device):
@@ -93,9 +92,8 @@ class _MeshNormalConsistency(torch.autograd.Function):
         Q, V, dev = pairs.shape[0], verts.shape[0], verts.device
         with torch.cuda.device(dev):
             out = torch.empty((), device=dev)
-            scratch = torch.empty(lib.sgr_mesh_nc_forward_scratch_bytes(Q), dtype=torch.uint8, device=dev)
-            check(lib.sgr_mesh_nc_forward(Q, V, verts.data_ptr(), pairs.data_ptr(), out.data_ptr(), scratch.data_ptr(),
-                                          torch.cuda.current_stream(dev).cuda_stream))
+            ws = scratch(lib.sgr_mesh_nc_forward_scratch_bytes(Q), dev)
+            check(lib.sgr_mesh_nc_forward(Q, V, ptr(verts), ptr(pairs), out.data_ptr(), ptr(ws), stream(dev)))
         ctx.save_for_backward(verts, pairs, vert_ptr, vert_inc)
         return out
 
@@ -106,10 +104,9 @@ class _MeshNormalConsistency(torch.autograd.Function):
         with torch.cuda.device(dev):
             g = g.detach().float().contiguous()
             g_verts = torch.empty_like(verts)
-            scratch = torch.empty(lib.sgr_mesh_nc_backward_scratch_bytes(Q), dtype=torch.uint8, device=dev)
-            check(lib.sgr_mesh_nc_backward(Q, V, verts.data_ptr(), pairs.data_ptr(), vert_ptr.data_ptr(),
-                                           vert_inc.data_ptr(), g.data_ptr(), g_verts.data_ptr(), scratch.data_ptr(),
-                                           torch.cuda.current_stream(dev).cuda_stream))
+            ws = scratch(lib.sgr_mesh_nc_backward_scratch_bytes(Q), dev)
+            check(lib.sgr_mesh_nc_backward(Q, V, ptr(verts), ptr(pairs), ptr(vert_ptr), ptr(vert_inc), g.data_ptr(),
+                                           ptr(g_verts), ptr(ws), stream(dev)))
         return g_verts, None, None, None
 
 
@@ -118,10 +115,8 @@ def mesh_normal_consistency(verts, faces=None, topology=None):
     the pairs of faces sharing an edge of 1 - cos(n_a, -n_b).  Pass `topology` (from `mesh_topology`) to skip the
     per-call table build (`faces` is then not read); without it one is built from `faces` on the device.
     -> 0-dim tensor."""
-    if not verts.is_cuda:
-        raise RuntimeError("sugar_b200.meshloss needs CUDA tensors: there is no CPU fallback")
-    if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
-        raise ValueError(f"verts must be float32 [V,3], got {verts.dtype} {tuple(verts.shape)}")
+    require_cuda("meshloss", verts)
+    tensor(verts, "verts", torch.float32, ("V", 3))
     if topology is None:
         if faces is None:
             raise ValueError("mesh_normal_consistency needs `faces` or a `topology`")

@@ -428,15 +428,14 @@ class ViewParallel:
 def sh_grad_from_factors(means3D: torch.Tensor, campos_all: torch.Tensor, dRGB_all: torch.Tensor, M: int,
                          sh_degree: int, out: torch.Tensor = None) -> torch.Tensor:
     """dL_dsh [P,M,3] = sum_v basis(normalize(means3D - campos_all[v])) (x) dRGB_all[v]  (CUDA kernel)."""
-    from ._lib import check, lib
+    from ._lib import check, lib, stream
     P, V = means3D.shape[0], campos_all.shape[0]
     if out is None:
         out = torch.empty((P, M, 3), dtype=torch.float32, device=means3D.device)
     assert out.is_contiguous() and out.numel() == P * M * 3 and dRGB_all.is_contiguous() and campos_all.is_contiguous()
     with torch.cuda.device(means3D.device):
         check(lib.sgr_sh_grad_from_factors(P, M, sh_degree, V, means3D.contiguous().data_ptr(), campos_all.data_ptr(),
-                                           dRGB_all.data_ptr(), out.data_ptr(),
-                                           torch.cuda.current_stream(means3D.device).cuda_stream))
+                                           dRGB_all.data_ptr(), out.data_ptr(), stream(means3D.device)))
     return out
 
 

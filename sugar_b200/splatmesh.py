@@ -15,35 +15,15 @@ both run on the GPU only.
 """
 import torch
 
-from ._lib import check, lib
+from ._lib import check, check_ids, lib, require_cuda, scratch, stream, tensor
 
 INT32_MAX = 2 ** 31 - 1
 TRIANGLES = ((0, 2, 1), (0, 3, 2))   # the two faces of a diamond (sugar_model.py:254-256)
 
 
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
-
-
-def _require_cuda(*ts):
-    for t in ts:
-        if not t.is_cuda:
-            raise RuntimeError("sugar_b200.splatmesh needs CUDA tensors: there is no CPU fallback")
-
-
-def _cam_matrix(m, dev, name):
-    if not torch.is_tensor(m) or m.shape != (4, 4) or m.dtype != torch.float32:
-        raise ValueError(f"cam.{name} must be a float32 [4,4] tensor")
-    if m.device != dev:
-        raise ValueError(f"cam.{name} on {m.device}, the mesh on {dev}")
-    return m.contiguous()
-
-
-def _vec3(t, name, n=None):
-    if t.dtype != torch.float32 or t.dim() != 2 or t.shape[1] != 3 or (n is not None and t.shape[0] != n):
-        want = f"[{n},3]" if n is not None else "[N,3]"
-        raise ValueError(f"{name} must be float32 {want}, got {t.dtype} {tuple(t.shape)}")
-    return t.contiguous()
+def cam_matrix(cam, name, dev):
+    """cam.viewmatrix / cam.projmatrix checked as a float32 [4,4] tensor on `dev`."""
+    return tensor(getattr(cam, name), f"cam.{name}", torch.float32, (4, 4), dev, "the mesh")
 
 
 def splat_mesh(points, scaling, quaternions, cam, triangle_scale=2.0):
@@ -52,20 +32,16 @@ def splat_mesh(points, scaling, quaternions, cam, triangle_scale=2.0):
     points, scaling (activated) float32 [P,3], quaternions float32 [P,4] (normalised, w first) on one CUDA device.
     -> verts float32 [4P,3] (every vertex moved along its view ray onto the plane through the Gaussian's centre
     perpendicular to the centre's ray), faces int64 [2P,3] = 4g + (0, 2, 1), 4g + (0, 3, 2)."""
-    P, dev = points.shape[0], points.device
-    points = _vec3(points, "points")
-    scaling = _vec3(scaling, "scaling", P)
-    if quaternions.dtype != torch.float32 or quaternions.shape != (P, 4):
-        raise ValueError(f"quaternions must be float32 [{P},4], got {quaternions.dtype} {tuple(quaternions.shape)}")
-    if scaling.device != dev or quaternions.device != dev:
-        raise ValueError("points, scaling and quaternions must be on one device")
+    dev = points.device
+    points = tensor(points, "points", torch.float32, ("N", 3))
+    P = points.shape[0]
+    scaling = tensor(scaling, "scaling", torch.float32, (P, 3), dev, "points")
+    # the kernel loads one float4 per Gaussian
+    quaternions = tensor(quaternions, "quaternions", torch.float32, (P, 4), dev, "points", align=16)
     if 4 * P > INT32_MAX:
         raise ValueError(f"{P} Gaussians: at most (2^31 - 1) / 4")
-    view = _cam_matrix(cam.viewmatrix, dev, "viewmatrix")
-    _require_cuda(points, scaling, quaternions)
-    quaternions = quaternions.contiguous()
-    if quaternions.data_ptr() % 16:                  # the kernel loads one float4 per Gaussian
-        quaternions = quaternions.clone()
+    view = cam_matrix(cam, "viewmatrix", dev)
+    require_cuda("splatmesh", points, scaling, quaternions)
     with torch.no_grad(), torch.cuda.device(dev):
         verts = torch.empty((4 * P, 3), dtype=torch.float32, device=dev)
         faces = (4 * torch.arange(P, device=dev)[:, None, None] +
@@ -73,7 +49,7 @@ def splat_mesh(points, scaling, quaternions, cam, triangle_scale=2.0):
         if P:
             view_inv = torch.linalg.inv(view.double()).float().contiguous()
             check(lib.sgr_splat_mesh(P, points.data_ptr(), scaling.data_ptr(), quaternions.data_ptr(), view.data_ptr(),
-                                     view_inv.data_ptr(), float(triangle_scale), verts.data_ptr(), _stream(dev)))
+                                     view_inv.data_ptr(), float(triangle_scale), verts.data_ptr(), stream(dev)))
     return verts, faces
 
 
@@ -85,30 +61,24 @@ def rasterize_mesh(verts, faces, cam):
     -> zbuf float32 [H,W] (view-space depth of the nearest covering face, -1 where none), pix_to_face int64 [H,W]
     (its index, -1 where none; equal depths resolve to the lower index), identical from run to run."""
     dev = verts.device
-    verts = _vec3(verts, "verts")
-    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
-        raise ValueError(f"faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
-    if faces.device != dev:
-        raise ValueError(f"faces on {faces.device}, verts on {dev}")
+    verts = tensor(verts, "verts", torch.float32, ("N", 3))
+    faces = tensor(faces, "faces", torch.int64, ("F", 3), dev)
     V, F = verts.shape[0], faces.shape[0]
     if V > INT32_MAX or F > INT32_MAX:
         raise ValueError(f"{V} vertices / {F} faces: at most 2^31 - 1 each (the face id is packed in 32 bits)")
     H, W = int(cam.height), int(cam.width)
     if not (0 < W <= 65535 and 0 < H <= 65535 and W * H <= INT32_MAX):
         raise ValueError(f"image {W}x{H}: need 0 < W, H <= 65535 and W*H <= 2^31 - 1")
-    view = _cam_matrix(cam.viewmatrix, dev, "viewmatrix")
-    proj = _cam_matrix(cam.projmatrix, dev, "projmatrix")
-    faces = faces.contiguous()
-    n_bad = int(((faces < 0) | (faces >= V)).sum()) if F else 0             # the one host read
-    if n_bad:
-        raise ValueError(f"{n_bad} face vertex ids outside [0, {V})")
-    _require_cuda(verts, faces)
+    view = cam_matrix(cam, "viewmatrix", dev)
+    proj = cam_matrix(cam, "projmatrix", dev)
+    check_ids((faces, 0, V, "face vertex ids"))
+    require_cuda("splatmesh", verts, faces)
     with torch.no_grad(), torch.cuda.device(dev):
         if F == 0:
             return (torch.full((H, W), -1.0, device=dev), torch.full((H, W), -1, dtype=torch.int64, device=dev))
         zbuf = torch.empty((H, W), dtype=torch.float32, device=dev)
         pix_to_face = torch.empty((H, W), dtype=torch.int64, device=dev)
-        scratch = torch.empty(lib.sgr_mesh_raster_scratch_bytes(F, W, H), dtype=torch.uint8, device=dev)
+        ws = scratch(lib.sgr_mesh_raster_scratch_bytes(F, W, H), dev)
         check(lib.sgr_mesh_raster(V, F, verts.data_ptr(), faces.data_ptr(), view.data_ptr(), proj.data_ptr(), W, H,
-                                  zbuf.data_ptr(), pix_to_face.data_ptr(), scratch.data_ptr(), _stream(dev)))
+                                  zbuf.data_ptr(), pix_to_face.data_ptr(), ws.data_ptr(), stream(dev)))
     return zbuf, pix_to_face

@@ -39,8 +39,8 @@ from types import SimpleNamespace
 
 import torch
 
-from ._lib import check, lib
-from .splatmesh import _cam_matrix, _require_cuda, _stream, _vec3
+from ._lib import check, check_ids, lib, require_cuda, same_device, stream, tensor
+from .splatmesh import cam_matrix
 
 INT32_MAX = 2 ** 31 - 1
 SH_C0 = 0.28209479177387814
@@ -76,25 +76,11 @@ def uv_layout(n_faces, square_size=10, device=None):
     return verts_uv.to(device), faces_uv.to(device), T
 
 
-def _faces(faces, V):
-    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
-        raise ValueError(f"faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
+def _faces(faces):
+    faces = tensor(faces, "faces", torch.int64, ("F", 3))
     if faces.shape[0] > INT32_MAX // 3:
         raise ValueError(f"{faces.shape[0]} faces: at most (2^31 - 1) / 3")
-    return faces.contiguous()
-
-
-def _same_device(dev, **ts):
-    for name, t in ts.items():
-        if t.device != dev:
-            raise ValueError(f"{name} on {t.device}, verts on {dev}")
-
-
-def _n_bad(*conds):
-    """Counts of the given bool tensors with one host read."""
-    if not conds:
-        return []
-    return torch.stack([c.sum() for c in conds]).tolist()
+    return faces
 
 
 def initial_texture(verts, faces, points, scaling, quaternions, sh_dc, square_size=10):
@@ -105,15 +91,15 @@ def initial_texture(verts, faces, points, scaling, quaternions, sh_dc, square_si
     if square_size < 3:
         raise ValueError("square_size must be >= 3")
     dev = verts.device
-    verts = _vec3(verts, "verts")
+    verts = tensor(verts, "verts", torch.float32, ("N", 3))
     V = verts.shape[0]
-    faces = _faces(faces, V)
+    faces = _faces(faces)
     F = faces.shape[0]
+    points = tensor(points, "points", torch.float32, ("N", 3))
     P = points.shape[0]
-    points = _vec3(points, "points")
-    scaling = _vec3(scaling, "scaling", P)
-    if quaternions.dtype != torch.float32 or quaternions.shape != (P, 4):
-        raise ValueError(f"quaternions must be float32 [{P},4], got {quaternions.dtype} {tuple(quaternions.shape)}")
+    scaling = tensor(scaling, "scaling", torch.float32, (P, 3))
+    # the kernel loads one float4 per Gaussian
+    quaternions = tensor(quaternions, "quaternions", torch.float32, (P, 4), align=16)
     if sh_dc.dtype != torch.float32 or tuple(sh_dc.shape) not in ((P, 3), (P, 1, 3)):
         raise ValueError(f"sh_dc must be float32 [{P},3] or [{P},1,3], got {sh_dc.dtype} {tuple(sh_dc.shape)}")
     if (F == 0 and P != 0) or (F > 0 and (P == 0 or P % F)):
@@ -121,23 +107,18 @@ def initial_texture(verts, faces, points, scaling, quaternions, sh_dc, square_si
     if P > INT32_MAX:
         raise ValueError(f"{P} Gaussians: at most 2^31 - 1")
     n = P // F if F else 1
-    _same_device(dev, faces=faces, points=points, scaling=scaling, quaternions=quaternions, sh_dc=sh_dc)
+    same_device(dev, faces=faces, points=points, scaling=scaling, quaternions=quaternions, sh_dc=sh_dc)
     T = texture_size(F, square_size)
     if T * T > INT32_MAX:
         raise ValueError(f"{F} faces at square size {square_size}: texture {T}x{T} has more than 2^31 - 1 texels")
-    (bad,) = _n_bad((faces < 0) | (faces >= V)) if F else [0]
-    if bad:
-        raise ValueError(f"{bad} face vertex ids outside [0, {V})")
-    _require_cuda(verts, faces, points, scaling, quaternions, sh_dc)
-    quaternions = quaternions.contiguous()
-    if quaternions.data_ptr() % 16:                  # the kernel loads one float4 per Gaussian
-        quaternions = quaternions.clone()
+    check_ids((faces, 0, V, "face vertex ids"))
+    require_cuda("texture", verts, faces, points, scaling, quaternions, sh_dc)
     sh_dc = sh_dc.reshape(P, 3).contiguous()
     with torch.no_grad(), torch.cuda.device(dev):
         tex = torch.empty((T, T, 3), dtype=torch.float32, device=dev)
         check(lib.sgr_texture_init(F, n, V, square_size, T, verts.data_ptr(), faces.data_ptr(), points.data_ptr(),
                                    scaling.data_ptr(), quaternions.data_ptr(), sh_dc.data_ptr(), tex.data_ptr(),
-                                   _stream(dev)))
+                                   stream(dev)))
     return tex
 
 
@@ -147,7 +128,7 @@ def new_bake_state(init_texture):
     if init_texture.dtype != torch.float32 or init_texture.dim() != 3 or init_texture.shape[2] != 3 or \
             init_texture.shape[0] != init_texture.shape[1]:
         raise ValueError(f"init_texture must be float32 [T,T,3], got {init_texture.dtype} {tuple(init_texture.shape)}")
-    _require_cuda(init_texture)
+    require_cuda("texture", init_texture)
     T, dev = init_texture.shape[0], init_texture.device
     return SimpleNamespace(sum=torch.zeros((T, T, 3), dtype=torch.float32, device=dev),
                            count=torch.zeros((T, T), dtype=torch.int32, device=dev),
@@ -156,40 +137,31 @@ def new_bake_state(init_texture):
 
 def _check_view(state, verts, faces, verts_uv, faces_uv, cam, image, zbuf, pix_to_face):
     dev = verts.device
-    verts = _vec3(verts, "verts")
-    faces = _faces(faces, verts.shape[0])
-    if verts_uv.dtype != torch.float32 or verts_uv.dim() != 2 or verts_uv.shape[1] != 2:
-        raise ValueError(f"verts_uv must be float32 [N,2], got {verts_uv.dtype} {tuple(verts_uv.shape)}")
+    verts = tensor(verts, "verts", torch.float32, ("N", 3))
+    faces = _faces(faces)
+    tensor(verts_uv, "verts_uv", torch.float32, ("N", 2))
     F = faces.shape[0]
-    if faces_uv.dtype != torch.int64 or faces_uv.shape != (F, 3):
-        raise ValueError(f"faces_uv must be int64 [{F},3], got {faces_uv.dtype} {tuple(faces_uv.shape)}")
+    tensor(faces_uv, "faces_uv", torch.int64, (F, 3))
     H, W = int(cam.height), int(cam.width)
     if not (0 < W and 0 < H and W * H <= INT32_MAX):
         raise ValueError(f"image {W}x{H}: need 0 < W, H and W*H <= 2^31 - 1")
-    if image.dtype != torch.float32 or image.shape != (3, H, W):
-        raise ValueError(f"image must be float32 [3,{H},{W}], got {image.dtype} {tuple(image.shape)}")
-    if zbuf.dtype != torch.float32 or zbuf.shape != (H, W):
-        raise ValueError(f"zbuf must be float32 [{H},{W}], got {zbuf.dtype} {tuple(zbuf.shape)}")
-    if pix_to_face.dtype != torch.int64 or pix_to_face.shape != (H, W):
-        raise ValueError(f"pix_to_face must be int64 [{H},{W}], got {pix_to_face.dtype} {tuple(pix_to_face.shape)}")
+    tensor(image, "image", torch.float32, (3, H, W))
+    tensor(zbuf, "zbuf", torch.float32, (H, W))
+    tensor(pix_to_face, "pix_to_face", torch.int64, (H, W))
     T = state.sum.shape[0]
     if state.sum.shape != (T, T, 3) or state.count.shape != (T, T) or state.owner.shape != (T, T) or \
             state.count.dtype != torch.int32 or state.owner.dtype != torch.int32:
         raise ValueError("state must come from new_bake_state")
-    _same_device(dev, faces=faces, verts_uv=verts_uv, faces_uv=faces_uv, image=image, zbuf=zbuf,
-                 pix_to_face=pix_to_face, state=state.sum)
-    _cam_matrix(cam.viewmatrix, dev, "viewmatrix")
-    _cam_matrix(cam.projmatrix, dev, "projmatrix")
+    same_device(dev, faces=faces, verts_uv=verts_uv, faces_uv=faces_uv, image=image, zbuf=zbuf,
+                pix_to_face=pix_to_face, state=state.sum)
+    cam_matrix(cam, "viewmatrix", dev)
+    cam_matrix(cam, "projmatrix", dev)
     V, n_uv = verts.shape[0], verts_uv.shape[0]
     if V > INT32_MAX or n_uv > INT32_MAX:
         raise ValueError(f"{V} vertices / {n_uv} UV vertices: at most 2^31 - 1 each")
-    bad = _n_bad((faces < 0) | (faces >= V), (faces_uv < 0) | (faces_uv >= n_uv),
-                 (pix_to_face < -1) | (pix_to_face >= F))
-    for count, what in zip(bad, (f"face vertex ids outside [0, {V})", f"faces_uv ids outside [0, {n_uv})",
-                                 f"pix_to_face values outside [-1, {F})")):
-        if count:
-            raise ValueError(f"{count} {what}")
-    _require_cuda(verts, faces, verts_uv, faces_uv, image, zbuf, pix_to_face, state.sum)
+    check_ids((faces, 0, V, "face vertex ids"), (faces_uv, 0, n_uv, "faces_uv ids"),
+              (pix_to_face, -1, F, "pix_to_face values"))
+    require_cuda("texture", verts, faces, verts_uv, faces_uv, image, zbuf, pix_to_face, state.sum)
 
 
 def _bake(state, verts, faces, verts_uv, faces_uv, cam, image, zbuf, pix_to_face):
@@ -207,7 +179,7 @@ def _bake(state, verts, faces, verts_uv, faces_uv, cam, image, zbuf, pix_to_face
                                         faces.data_ptr(), verts_uv.data_ptr(), faces_uv.data_ptr(), view.data_ptr(),
                                         proj.data_ptr(), W, H, image.data_ptr(), zbuf.data_ptr(),
                                         pix_to_face.data_ptr(), state.sum.data_ptr(), state.count.data_ptr(),
-                                        state.owner.data_ptr(), pix_texel.data_ptr(), _stream(dev)))
+                                        state.owner.data_ptr(), pix_texel.data_ptr(), stream(dev)))
 
 
 def bake_view(state, verts, faces, verts_uv, faces_uv, cam, image, zbuf, pix_to_face):
@@ -238,7 +210,7 @@ def extract_texture_image_and_uv_from_gaussians(verts, faces, points, scaling, q
     P = points.shape[0]
     if strengths.dtype != torch.float32 or tuple(strengths.shape) not in ((P,), (P, 1)):
         raise ValueError(f"strengths must be float32 [{P}] or [{P},1], got {strengths.dtype} {tuple(strengths.shape)}")
-    _same_device(dev, strengths=strengths)
+    same_device(dev, strengths=strengths)
     with torch.no_grad():
         init = initial_texture(verts, faces, points, scaling, quaternions, sh_dc, square_size)
         verts_uv, faces_uv, _ = uv_layout(faces.shape[0], square_size, dev)
