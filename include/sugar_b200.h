@@ -556,6 +556,56 @@ SGR_API int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *vert
                          const float *colors, const float *normals, float *verts_out, int64_t *faces_out,
                          float *colors_out, float *normals_out, int64_t *result, void *scratch, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Densification and pruning of the coarse model (SuGaRDensifier, sugar_densifier.py), restated in
+ * oracle/densify_oracle.py; sugar_b200/densify.py is the caller.  P original rows, float32 raw parameters.
+ * sgr_densify_stats: update_densification_stats for rows with visibility[i] != 0: max_radii = max(max_radii,
+ *   float(radii)), accum += sqrtf(gx*gx + gy*gy) (each square rounded: torch's vector_norm over two floats),
+ *   denom += 1.  grad_means2D f32 rows of grad_stride >= 2 floats (gx, gy first), radii i32[P], visibility u8[P],
+ *   accum / denom / max_radii f32[P].  No host synchronisation.
+ * sgr_densify_classify: flags u8[4,P] fully written: row 0 keep (an original row that is not split and not pruned),
+ *   row 1 clone_kept, row 2 split, row 3 children_kept (both children of a split row share one fate), from accum /
+ *   denom f32[P], scales (log) f32[P,3], densities (logit) f32[P] and the float32 gates below.
+ * sgr_densify_emit: the P' = n_keep + n_clone + 2 n_child output rows of every column, in the order kept originals,
+ *   kept clones, kept children of copy 0, kept children of copy 1 (each in parent order).  scan i32[4,P] is the
+ *   inclusive scan of the four flag rows along P, and n_keep, n_clone, S, n_child its totals.  cols: a HOST array of
+ *   n_cols <= SGR_DENSIFY_MAX_COLUMNS columns, src f32[P,width] -> dst f32[P',width].  Clone and child rows copy src
+ *   except in SGR_DENSIFY_ZERO_NEW columns (zeros: Adam moments); a child's SGR_DENSIFY_POINTS value is
+ *   R(q / |q|) (normal * exp(scale)) + point with normals f32[2S,3] (copy k of the split row of rank r reads row
+ *   k*S + r; R as pytorch3d's quaternion_to_matrix) and its SGR_DENSIFY_SCALES value log(exp(scale) * inv_split).
+ *   points / scales f32[P,3] and quaternions f32[P,4] (16-byte aligned) are the parents'.  src_row i32[P'] scratch.
+ *   Pruning by a mask is the same call with only the keep row set.
+ * ------------------------------------------------------------------------------------------ */
+#define SGR_DENSIFY_MAX_COLUMNS 24
+#define SGR_DENSIFY_COPY 0      /* new rows copy the parent */
+#define SGR_DENSIFY_ZERO_NEW 1  /* new rows are zero */
+#define SGR_DENSIFY_POINTS 2    /* children compute their position */
+#define SGR_DENSIFY_SCALES 3    /* children compute their log-scale */
+typedef struct SgrDensifyColumn {
+    const float *src;
+    float *dst;
+    int32_t width;  /* floats per row */
+    int32_t kind;   /* SGR_DENSIFY_* */
+} SgrDensifyColumn;
+/* Thresholds as float32 (torch compares a float32 tensor with a Python float rounded to float32). */
+typedef struct SgrDensifyGates {
+    float max_grad;     /* clone / split when the mean gradient >= max_grad */
+    float clone_scale;  /* percent_dense * extent: clone when max(scale) <= it, split when > */
+    float big_scale;    /* 0.1 * extent */
+    float min_opacity;  /* prune when sigmoid(density) < min_opacity */
+    float screen_size;  /* max_screen_size: compared with max_radii2D, all zeros after the appends */
+    float inv_split;    /* 1 / (0.8 * 2) as the float reciprocal torch multiplies by */
+    int32_t use_screen; /* max_screen_size is truthy: the screen and world-size clauses apply */
+} SgrDensifyGates;
+SGR_API int sgr_densify_stats(int32_t P, const float *grad_means2D, int32_t grad_stride, const int32_t *radii,
+                              const uint8_t *visibility, float *accum, float *denom, float *max_radii, void *stream);
+SGR_API int sgr_densify_classify(int32_t P, const float *accum, const float *denom, const float *scales,
+                                 const float *densities, const SgrDensifyGates *gates, uint8_t *flags, void *stream);
+SGR_API int sgr_densify_emit(int32_t P, int32_t n_keep, int32_t n_clone, int32_t S, int32_t n_child,
+                             const int32_t *scan, int32_t n_cols, const SgrDensifyColumn *cols, const float *points,
+                             const float *scales, const float *quaternions, const float *normals, float inv_split,
+                             int32_t *src_row, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */
@@ -567,7 +617,7 @@ SGR_API int sgr_profile_read(float *total_ms, int *counts);
 SGR_API int sgr_profile_timeline(int max_records, int *kinds, float *t_begin_ms, float *t_end_ms);
 
 /* sizeof of an ABI struct as the library was compiled (0 SgrView, 1 SgrGaussians, 2 SgrBackwardPlan, 3 SgrFieldParams,
- * 4 SgrSsimParams; else 0): lets a foreign-language binding check its own struct layout. */
+ * 4 SgrSsimParams, 5 SgrDensifyGates, 6 SgrDensifyColumn; else 0): lets a foreign-language binding check its own struct layout. */
 SGR_API size_t sgr_struct_bytes(int32_t which);
 SGR_API const char *sgr_last_error(void);
 SGR_API const char *sgr_version(void);

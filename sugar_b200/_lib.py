@@ -46,6 +46,16 @@ class SgrSsimParams(C.Structure):
                 ("c2", C.c_float), ("window", C.c_float * 11)]
 
 
+class SgrDensifyGates(C.Structure):
+    _fields_ = [("max_grad", C.c_float), ("clone_scale", C.c_float), ("big_scale", C.c_float),
+                ("min_opacity", C.c_float), ("screen_size", C.c_float), ("inv_split", C.c_float),
+                ("use_screen", C.c_int32)]
+
+
+class SgrDensifyColumn(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("width", C.c_int32), ("kind", C.c_int32)]
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 STAGE_HOOK = C.CFUNCTYPE(None, C.c_void_p, C.c_int32)
 
@@ -133,6 +143,11 @@ PROTOTYPES = {
     "sgr_mcubes_emit": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double, C.c_int64, C.c_int64] + [C.c_void_p] * 4),
     "sgr_decimate_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "sgr_decimate": (C.c_int, [C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 11),
+    "sgr_densify_stats": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 6),
+    "sgr_densify_classify": (C.c_int, [C.c_int32] + [C.c_void_p] * 4 + [C.POINTER(SgrDensifyGates)] +
+                             [C.c_void_p] * 2),
+    "sgr_densify_emit": (C.c_int, [C.c_int32] * 5 + [C.c_void_p, C.c_int32, C.POINTER(SgrDensifyColumn)] +
+                         [C.c_void_p] * 4 + [C.c_float, C.c_void_p, C.c_void_p]),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),
@@ -159,7 +174,8 @@ def _load():
 
 
 lib = _load()
-for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams, SgrSsimParams)):
+for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams, SgrSsimParams, SgrDensifyGates,
+                          SgrDensifyColumn)):
     if lib.sgr_struct_bytes(_i) != C.sizeof(_t):   # a stale library or a binding edited without the header
         raise SgrError(f"{LIB_PATH}: struct {_t.__name__} is {lib.sgr_struct_bytes(_i)} bytes in the library, "
                        f"{C.sizeof(_t)} in this binding -- rebuild with `python sugar_b200/build.py`")

@@ -334,6 +334,8 @@ size_t sgr_struct_bytes(int32_t which)
         case 2: return sizeof(SgrBackwardPlan);
         case 3: return sizeof(SgrFieldParams);
         case 4: return sizeof(SgrSsimParams);
+        case 5: return sizeof(SgrDensifyGates);
+        case 6: return sizeof(SgrDensifyColumn);
         default: return 0;
     }
 }

@@ -23,7 +23,8 @@ implementations:
     normalize / cat of SuGaR's raw parameters) just backpropagates the summed gradient: inputs need not be
     leaves, and several backwards per step (several views per rank) each do their own exchange.
   * dL_dmeans2D and radii are per-view densification statistics (sugar_scene/sugar_densifier.py:156-164) and
-    are NOT summed.
+    are NOT summed here: each rank accumulates them locally, and densify.Densifier(group=...) reduces them and
+    shares the split's normals when it densifies, so the replicated parameters stay replicas.
   * Losses that reach the parameters without going through the rasterizer (density / SDF regularisation,
     evaluated per view on its rank) are summed with `reduce_grad(tensor)`: identity in the forward, all-reduce of
     the incoming gradient in the backward.
