@@ -32,6 +32,7 @@ WORKLOADS = {
 
 def reference_ops(torch, ref_mod):
     """The reference's building blocks behind the `ops` interface of sugar_b200/steps.py."""
+    from oracle import densest_oracle as deo
     from oracle import field_oracle as fo
     from oracle import meshbind_oracle as mo
     from oracle import meshloss_oracle as mlo
@@ -46,6 +47,7 @@ def reference_ops(torch, ref_mod):
         field_values=lambda x, nbr, points, scaling, quats, strengths, density_factor=1.0, density_threshold=1.0, **_:
             fo.field_values_torch(x, nbr, points, scaling, quats, strengths, density_factor, density_threshold),
         better_normal_loss=fo.better_normal_loss_torch, bind_to_mesh=bind, l1_dssim=so.l1_dssim_torch,
+        density_estimation_loss=deo.density_estimation_loss_torch,
         # pytorch3d's cost: a new Meshes every call (edges rebuilt) and its Python pair loop; no cached topology
         mesh_normal_consistency=lambda verts, faces, topology=None: mlo.mesh_normal_consistency_torch(verts, faces))
 

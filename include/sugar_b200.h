@@ -356,6 +356,26 @@ SGR_API int sgr_field_backward(const SgrFieldParams *p, const float *x, const in
                        float *g_x, float *g_points, float *g_scaling, float *g_quaternions,
                        float *g_strengths, void *scratch, void *stream);
 
+/* Density estimation loss of the coarse_density trainer in projection mode
+ * (sugar_trainers/coarse_density.py:654-656, 684-691), per sample n drawn from Gaussian g = own_idx[n]:
+ *   rho  = sgr_field_forward's density at x_n (before the straight-through clamp), beta its beta
+ *   e    = <x_n - points[g], n_g>,  n_g = column argmin_j scaling[g][j] of R(quaternions[g]) (first minimum)
+ *   loss[n] = | rho - exp(-0.5 e^2 / beta^2) |
+ * Same arguments as sgr_field_forward plus own_idx i64[N]; p->samples_per_idx_row must be 0 or 1 and
+ * density_threshold / opacity_min_clamp are not used.  loss f32[N] is required, nbr_opacity f32[N,K] may be
+ * NULL and equals sgr_field_forward's.  `scratch` must hold sgr_field_scratch_bytes(P).
+ * Backward: g_loss f32[N] -> g_x, g_points, g_scaling, g_quaternions, g_strengths as in sgr_field_backward
+ * (fully written, any may be NULL); no gradient flows through the argmin. */
+SGR_API int sgr_density_estimation_forward(const SgrFieldParams *p, const float *x, const int64_t *own_idx,
+                                           const int64_t *nbr_idx, const float *points, const float *scaling,
+                                           const float *quaternions, const float *strengths, float *loss,
+                                           float *nbr_opacity, void *scratch, void *stream);
+SGR_API int sgr_density_estimation_backward(const SgrFieldParams *p, const float *x, const int64_t *own_idx,
+                                            const int64_t *nbr_idx, const float *points, const float *scaling,
+                                            const float *quaternions, const float *strengths, const float *g_loss,
+                                            float *g_x, float *g_points, float *g_scaling, float *g_quaternions,
+                                            float *g_strengths, void *scratch, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * "Better normal" regularisation of the trainers (sugar_trainers/coarse_sdf.py:688-716, with
  * SuGaR.get_normals(estimate_from_points=False) -> get_smallest_axis, sugar_model.py:930-968), in the

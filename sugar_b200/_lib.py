@@ -116,6 +116,8 @@ PROTOTYPES = {
     "sgr_normal_loss_backward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 11),
     "sgr_field_forward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 12),
     "sgr_field_backward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 17),
+    "sgr_density_estimation_forward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 11),
+    "sgr_density_estimation_backward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 15),
     "sgr_meshbind_forward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 5 + [C.c_float] + [C.c_void_p] * 4),
     "sgr_meshbind_backward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 12),
     "sgr_knn_workspace_bytes": (C.c_size_t, [C.c_int32]),

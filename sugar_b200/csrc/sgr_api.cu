@@ -64,8 +64,8 @@ int device_sm_count()
 static const char *const g_kind_names[K_NUM_KINDS] = {
     "preprocess", "tile_scan", "scatter", "tile_sort_smem", "tile_sort_global", "blend_forward", "blend_backward",
     "preprocess_backward", "field_pack", "field_forward", "field_backward", "field_unpack", "knn_build", "knn_query",
-    "misc", "view_finalize", "peer_reduce", "peer_sync", "loss_forward", "loss_backward", "mesh_nc_forward",
-    "mesh_nc_backward"};
+    "misc", "view_finalize", "peer_reduce", "peer_sync", "loss_forward", "loss_backward", "density_estimation_forward",
+    "density_estimation_backward", "mesh_nc_forward", "mesh_nc_backward"};
 struct ProfRec {
     cudaEvent_t a, b;
     int kind;

@@ -10,6 +10,8 @@
 // (sample, neighbour) pair, gathers a 48-byte packed Gaussian record, and the K partial
 // opacities are summed with shuffles.  Backward recomputes the pair and scatters with
 // 16-byte vector reductions into a packed per-Gaussian gradient record.
+// The coarse_density trainer's density estimation loss (densest_*_kernel) runs the same per-pair passes and adds the
+// sample's own Gaussian's terms.
 #include "sgr_field.cuh"
 
 namespace sgr {
@@ -102,7 +104,83 @@ __device__ __forceinline__ void red_v4(float *addr, float a, float b, float c, f
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-// gradient record per Gaussian, 12 floats: dmu.xyz dsig | dq.rijk | ds.xyz -
+// dL/dq from A = dL/dR, R = I + ts * E(q) with ts = two_s = 2 / |q|^2 (pytorch3d's quaternion_to_matrix)
+__device__ __forceinline__ float4 rot_backward(const float (&A)[3][3], float4 q, float ts)
+{
+    const float qr = q.x, qi = q.y, qj = q.z, qk = q.w;
+    const float dts = A[0][0] * -(qj * qj + qk * qk) + A[0][1] * (qi * qj - qk * qr) + A[0][2] * (qi * qk + qj * qr) +
+                      A[1][0] * (qi * qj + qk * qr) + A[1][1] * -(qi * qi + qk * qk) + A[1][2] * (qj * qk - qi * qr) +
+                      A[2][0] * (qi * qk - qj * qr) + A[2][1] * (qj * qk + qi * qr) + A[2][2] * -(qi * qi + qj * qj);
+    const float c = -ts * ts * dts;  // d ts / d q_c = -ts^2 q_c
+    const float dqr = ts * (-qk * A[0][1] + qj * A[0][2] + qk * A[1][0] - qi * A[1][2] - qj * A[2][0] + qi * A[2][1]) + c * qr;
+    const float dqi = ts * (qj * (A[0][1] + A[1][0]) + qk * (A[0][2] + A[2][0]) + qr * (A[2][1] - A[1][2]) -
+                            2.f * qi * (A[1][1] + A[2][2])) + c * qi;
+    const float dqj = ts * (qi * (A[0][1] + A[1][0]) + qr * (A[0][2] - A[2][0]) + qk * (A[1][2] + A[2][1]) -
+                            2.f * qj * (A[0][0] + A[2][2])) + c * qj;
+    const float dqk = ts * (qr * (A[1][0] - A[0][1]) + qi * (A[0][2] + A[2][0]) + qj * (A[1][2] + A[2][1]) -
+                            2.f * qk * (A[0][0] + A[1][1])) + c * qk;
+    return make_float4(dqr, dqi, dqj, dqk);
+}
+
+// Pass 2 of a field backward for one (sample x, neighbour id) pair.  Gk = dL/d(the pair's opacity) in total, gb = dL/d
+// beta of the sample.  Adds dL/dx to gx and scatters dL/d(mu, sigma, q, s) into the Gaussian's 12-float gradient record:
+// dmu.xyz dsig | dq.rijk | ds.xyz -
+__device__ __forceinline__ void field_pair_backward(float x0, float x1, float x2, int64_t id, const float4 *__restrict__ rec,
+                                                    const float *__restrict__ scaling, float density_factor, float Gk,
+                                                    float gb, int K, float *__restrict__ grec, float &gx0, float &gx1,
+                                                    float &gx2)
+{
+    const float4 r0 = __ldg(rec + id * 3), r1 = __ldg(rec + id * 3 + 1), r2 = __ldg(rec + id * 3 + 2);
+    const Rot R = quat_to_rot(r1);
+    const float sh[3] = {x0 - r0.x, x1 - r0.y, x2 - r0.z};
+    float u[3], w[3];
+#pragma unroll
+    for (int j = 0; j < 3; j++) u[j] = R.m[0][j] * sh[0] + R.m[1][j] * sh[1] + R.m[2][j] * sh[2];
+    w[0] = u[0] * r2.x;
+    w[1] = u[1] * r2.y;
+    w[2] = u[2] * r2.z;
+    const float d2raw = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
+    const float d2 = fminf(fmaxf(d2raw, 0.f), 1e8f);
+    const float e = density_factor * expf(-0.5f * d2);
+    const float o = r0.w * e;
+    const float dsig = Gk * e;
+    const float dd2 = (d2raw > 1e8f || d2raw < 0.f) ? 0.f : Gk * o * -0.5f;
+    const float invs[3] = {r2.x, r2.y, r2.z};
+    float du[3], ds[3];
+    const float *sc = scaling + id * 3;
+    int amin = 0;
+    float smin = sc[0];
+#pragma unroll
+    for (int j = 0; j < 3; j++) {
+        const float dw = dd2 * 2.0f * w[j];
+        du[j] = dw * invs[j];
+        const float sj = sc[j];
+        ds[j] = (sj >= 1e-8f) ? -(dw * u[j]) * invs[j] * invs[j] : 0.f;
+        if (j > 0 && sj < smin) {
+            smin = sj;
+            amin = j;
+        }
+    }
+    ds[amin] += gb / (float)K;
+    float dsh[3];
+#pragma unroll
+    for (int i = 0; i < 3; i++) dsh[i] = R.m[i][0] * du[0] + R.m[i][1] * du[1] + R.m[i][2] * du[2];
+    gx0 += dsh[0];
+    gx1 += dsh[1];
+    gx2 += dsh[2];
+    // dL/dR[i][j] = sh[i] * du[j]
+    float A[3][3];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) A[i][j] = sh[i] * du[j];
+    const float4 dq = rot_backward(A, r1, R.ts);
+    float *gr = grec + id * 12;
+    red_v4(gr, -dsh[0], -dsh[1], -dsh[2], dsig);
+    red_v4(gr + 4, dq.x, dq.y, dq.z, dq.w);
+    red_v4(gr + 8, ds[0], ds[1], ds[2], 0.f);
+}
+
 template <int G>
 __global__ void __launch_bounds__(256) field_backward_kernel(const FieldArgs a, const float *__restrict__ scaling,
                                                              const float *__restrict__ g_density,
@@ -152,67 +230,8 @@ __global__ void __launch_bounds__(256) field_backward_kernel(const FieldArgs a, 
     if (live)
         for (int k = l; k < a.K; k += G) {
             const int64_t id = a.idx[(size_t)nrow * a.K + k];
-            const float4 r0 = __ldg(a.rec + id * 3), r1 = __ldg(a.rec + id * 3 + 1), r2 = __ldg(a.rec + id * 3 + 2);
-            const Rot R = quat_to_rot(r1);
-            const float sh[3] = {x0 - r0.x, x1 - r0.y, x2 - r0.z};
-            float u[3], w[3];
-#pragma unroll
-            for (int j = 0; j < 3; j++) u[j] = R.m[0][j] * sh[0] + R.m[1][j] * sh[1] + R.m[2][j] * sh[2];
-            w[0] = u[0] * r2.x;
-            w[1] = u[1] * r2.y;
-            w[2] = u[2] * r2.z;
-            const float d2raw = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
-            const float d2 = fminf(fmaxf(d2raw, 0.f), 1e8f);
-            const float e = a.density_factor * expf(-0.5f * d2);
-            const float o = r0.w * e;
             const float Gk = gd + (g_nbr ? g_nbr[(size_t)n * a.K + k] : 0.f);
-            const float dsig = Gk * e;
-            const float dd2 = (d2raw > 1e8f || d2raw < 0.f) ? 0.f : Gk * o * -0.5f;
-            const float invs[3] = {r2.x, r2.y, r2.z};
-            float du[3], ds[3];
-            const float *sc = scaling + id * 3;
-            int amin = 0;
-            float smin = sc[0];
-#pragma unroll
-            for (int j = 0; j < 3; j++) {
-                const float dw = dd2 * 2.0f * w[j];
-                du[j] = dw * invs[j];
-                const float sj = sc[j];
-                ds[j] = (sj >= 1e-8f) ? -(dw * u[j]) * invs[j] * invs[j] : 0.f;
-                if (j > 0 && sj < smin) {
-                    smin = sj;
-                    amin = j;
-                }
-            }
-            ds[amin] += gb / (float)a.K;
-            float dsh[3];
-#pragma unroll
-            for (int i = 0; i < 3; i++) dsh[i] = R.m[i][0] * du[0] + R.m[i][1] * du[1] + R.m[i][2] * du[2];
-            gx0 += dsh[0];
-            gx1 += dsh[1];
-            gx2 += dsh[2];
-            // dL/dR[i][j] = sh[i] * du[j];  R = I + ts * E(q)
-            float A[3][3];
-#pragma unroll
-            for (int i = 0; i < 3; i++)
-#pragma unroll
-                for (int j = 0; j < 3; j++) A[i][j] = sh[i] * du[j];
-            const float qr = r1.x, qi = r1.y, qj = r1.z, qk = r1.w, ts = R.ts;
-            const float dts = A[0][0] * -(qj * qj + qk * qk) + A[0][1] * (qi * qj - qk * qr) + A[0][2] * (qi * qk + qj * qr) +
-                              A[1][0] * (qi * qj + qk * qr) + A[1][1] * -(qi * qi + qk * qk) + A[1][2] * (qj * qk - qi * qr) +
-                              A[2][0] * (qi * qk - qj * qr) + A[2][1] * (qj * qk + qi * qr) + A[2][2] * -(qi * qi + qj * qj);
-            const float c = -ts * ts * dts;  // d ts / d q_c = -ts^2 q_c
-            const float dqr = ts * (-qk * A[0][1] + qj * A[0][2] + qk * A[1][0] - qi * A[1][2] - qj * A[2][0] + qi * A[2][1]) + c * qr;
-            const float dqi = ts * (qj * (A[0][1] + A[1][0]) + qk * (A[0][2] + A[2][0]) + qr * (A[2][1] - A[1][2]) -
-                                    2.f * qi * (A[1][1] + A[2][2])) + c * qi;
-            const float dqj = ts * (qi * (A[0][1] + A[1][0]) + qr * (A[0][2] - A[2][0]) + qk * (A[1][2] + A[2][1]) -
-                                    2.f * qj * (A[0][0] + A[2][2])) + c * qj;
-            const float dqk = ts * (qr * (A[1][0] - A[0][1]) + qi * (A[0][2] + A[2][0]) + qj * (A[1][2] + A[2][1]) -
-                                    2.f * qk * (A[0][0] + A[1][1])) + c * qk;
-            float *gr = grec + id * 12;
-            red_v4(gr, -dsh[0], -dsh[1], -dsh[2], dsig);
-            red_v4(gr + 4, dqr, dqi, dqj, dqk);
-            red_v4(gr + 8, ds[0], ds[1], ds[2], 0.f);
+            field_pair_backward(x0, x1, x2, id, a.rec, scaling, a.density_factor, Gk, gb, a.K, grec, gx0, gx1, gx2);
         }
     gx0 = group_sum<G>(gx0);
     gx1 = group_sum<G>(gx1);
@@ -222,6 +241,152 @@ __global__ void __launch_bounds__(256) field_backward_kernel(const FieldArgs a, 
         g_x[3 * n + 1] = gx1;
         g_x[3 * n + 2] = gx2;
     }
+}
+
+// Density estimation loss of the coarse_density trainer in projection mode (coarse_density.py:654-656, 684-691):
+//   e = <x - mu_g, n_g>,  n_g = column argmin_j scaling[g][j] of R(q_g) (the first minimum, like torch.min),
+//   target = exp(-0.5 e^2 / beta^2),  loss = |rho - target|
+// with rho and beta the field's density (before the straight-through clamp) and beta at x.  The K terms are the field
+// forward's, in its lane order and butterfly, so rho and the neighbour opacities carry the field's bits.
+
+// <x - mu_g, n_g> for the sample's own Gaussian g; the column index comes from the float scaling row, so the 1e-8
+// clamp of the packed 1/s cannot change the pick
+struct OwnAxis {
+    float e, n[3], d[3];  // d = x - mu_g
+    int col;
+    float4 q;
+    float ts;  // two_s of q
+};
+
+__device__ __forceinline__ OwnAxis own_axis(float x0, float x1, float x2, int64_t g, const float4 *__restrict__ rec,
+                                            const float *__restrict__ scaling)
+{
+    OwnAxis o;
+    const float4 r0 = __ldg(rec + g * 3);
+    o.q = __ldg(rec + g * 3 + 1);
+    const float *sc = scaling + g * 3;
+    const float s0 = sc[0], s1 = sc[1], s2 = sc[2];
+    o.col = 0;
+    float smin = s0;
+    if (s1 < smin) smin = s1, o.col = 1;
+    if (s2 < smin) o.col = 2;
+    const Rot R = quat_to_rot(o.q);
+    o.ts = R.ts;
+#pragma unroll
+    for (int i = 0; i < 3; i++) o.n[i] = o.col == 0 ? R.m[i][0] : (o.col == 1 ? R.m[i][1] : R.m[i][2]);
+    o.d[0] = x0 - r0.x;
+    o.d[1] = x1 - r0.y;
+    o.d[2] = x2 - r0.z;
+    o.e = o.d[0] * o.n[0] + o.d[1] * o.n[1] + o.d[2] * o.n[2];
+    return o;
+}
+
+// exp(-0.5 * e.pow(2) / beta.pow(2)) in the reference's evaluation order
+__device__ __forceinline__ float density_target(float e, float beta) { return expf(-0.5f * (e * e) / (beta * beta)); }
+
+template <int G>
+__global__ void __launch_bounds__(256) densest_forward_kernel(const FieldArgs a, const int64_t *__restrict__ own,
+                                                              const float *__restrict__ scaling, float *__restrict__ loss,
+                                                              float *__restrict__ nbr_opacity)
+{
+    constexpr int SPB = 256 / G;
+    const int g = threadIdx.x / G, l = threadIdx.x % G;
+    const int n = blockIdx.x * SPB + g;
+    const bool live = n < a.N;
+    float x0 = 0.f, x1 = 0.f, x2 = 0.f, dens = 0.f, bsum = 0.f;
+    if (live) {
+        x0 = a.x[3 * n], x1 = a.x[3 * n + 1], x2 = a.x[3 * n + 2];
+        for (int k = l; k < a.K; k += G) {
+            const int64_t id = a.idx[(size_t)n * a.K + k];
+            const float4 r0 = __ldg(a.rec + id * 3), r1 = __ldg(a.rec + id * 3 + 1), r2 = __ldg(a.rec + id * 3 + 2);
+            const float o = field_term(x0, x1, x2, r0, r1, r2, a.density_factor);
+            if (nbr_opacity) nbr_opacity[(size_t)n * a.K + k] = o;
+            dens += o;
+            bsum += r2.w;
+        }
+    }
+    dens = group_sum<G>(dens);
+    bsum = group_sum<G>(bsum);
+    if (live && l == 0) {
+        const float b = bsum / (float)a.K;
+        const OwnAxis ax = own_axis(x0, x1, x2, own[n], a.rec, scaling);
+        loss[n] = fabsf(dens - density_target(ax.e, b));
+    }
+}
+
+template <int G>
+__global__ void __launch_bounds__(256) densest_backward_kernel(const FieldArgs a, const int64_t *__restrict__ own,
+                                                               const float *__restrict__ scaling,
+                                                               const float *__restrict__ g_loss, float *__restrict__ g_x,
+                                                               float *__restrict__ grec)
+{
+    constexpr int SPB = 256 / G;
+    const int g = threadIdx.x / G, l = threadIdx.x % G;
+    const int n = blockIdx.x * SPB + g;
+    const bool live = n < a.N;
+    float x0 = 0.f, x1 = 0.f, x2 = 0.f;
+    if (live) x0 = a.x[3 * n], x1 = a.x[3 * n + 1], x2 = a.x[3 * n + 2];
+    // pass 1: rho and beta of the sample, as the forward
+    float dens = 0.f, bsum = 0.f;
+    if (live)
+        for (int k = l; k < a.K; k += G) {
+            const int64_t id = a.idx[(size_t)n * a.K + k];
+            const float4 r0 = __ldg(a.rec + id * 3), r1 = __ldg(a.rec + id * 3 + 1), r2 = __ldg(a.rec + id * 3 + 2);
+            dens += field_term(x0, x1, x2, r0, r1, r2, a.density_factor);
+            bsum += r2.w;
+        }
+    dens = group_sum<G>(dens);
+    bsum = group_sum<G>(bsum);
+    // lane 0 of the group: dL/drho, dL/dbeta and dL/de of |rho - t|, t = exp(-e^2 / (2 beta^2))
+    float gd = 0.f, gb = 0.f, ge = 0.f;
+    if (live && l == 0) {
+        const float b = bsum / (float)a.K;
+        const OwnAxis ax = own_axis(x0, x1, x2, own[n], a.rec, scaling);
+        const float t = density_target(ax.e, b);
+        const float r = dens - t;
+        const float s = (r > 0.f ? 1.f : (r < 0.f ? -1.f : 0.f)) * g_loss[n];  // torch's abs: 0 at rho == t
+        const float ib2 = 1.0f / (b * b);
+        gd = s;
+        gb = -s * t * (ax.e * ax.e) * ib2 / b;
+        ge = s * t * ax.e * ib2;
+    }
+    const int lead = (threadIdx.x & 31) & ~(G - 1);
+    gd = __shfl_sync(0xffffffffu, gd, lead);
+    gb = __shfl_sync(0xffffffffu, gb, lead);
+    ge = __shfl_sync(0xffffffffu, ge, lead);
+    // pass 2: the field backward's per-pair scatter with dL/d opacity = dL/drho
+    float gx0 = 0.f, gx1 = 0.f, gx2 = 0.f;
+    if (live)
+        for (int k = l; k < a.K; k += G) {
+            const int64_t id = a.idx[(size_t)n * a.K + k];
+            field_pair_backward(x0, x1, x2, id, a.rec, scaling, a.density_factor, gd, gb, a.K, grec, gx0, gx1, gx2);
+        }
+    gx0 = group_sum<G>(gx0);
+    gx1 = group_sum<G>(gx1);
+    gx2 = group_sum<G>(gx2);
+    if (!live || l != 0) return;
+    // the own Gaussian's terms of e = <x - mu_g, n_g>: x, mu_g, and q_g through column `col` of R(q_g).  The axis is
+    // gathered again rather than kept live through pass 2 (fewer registers for every lane)
+    const int64_t og = own[n];
+    const OwnAxis ax = own_axis(x0, x1, x2, og, a.rec, scaling);
+    if (g_x) {
+        g_x[3 * n] = gx0 + ge * ax.n[0];
+        g_x[3 * n + 1] = gx1 + ge * ax.n[1];
+        g_x[3 * n + 2] = gx2 + ge * ax.n[2];
+    }
+    if (ge == 0.f) return;
+    float A[3][3];
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        const float dn = ge * ax.d[i];
+        A[i][0] = ax.col == 0 ? dn : 0.f;
+        A[i][1] = ax.col == 1 ? dn : 0.f;
+        A[i][2] = ax.col == 2 ? dn : 0.f;
+    }
+    const float4 dq = rot_backward(A, ax.q, ax.ts);
+    float *gr = grec + og * 12;
+    red_v4(gr, -ge * ax.n[0], -ge * ax.n[1], -ge * ax.n[2], 0.f);
+    red_v4(gr + 4, dq.x, dq.y, dq.z, dq.w);
 }
 
 __global__ void __launch_bounds__(256) field_unpack_kernel(int P, const float4 *__restrict__ grec, float *g_points,
@@ -348,6 +513,90 @@ int sgr_field_backward(const SgrFieldParams *p, const float *x, const int64_t *n
         }
         sgr::prof_end(st);
 #undef SGR_FB
+    }
+    SGR_LAUNCH(K_FIELD_UNPACK, st,
+               field_unpack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, (const float4 *)grec, g_points, g_scaling,
+                                                                       g_quaternions, g_strengths));
+    SGR_CUDA(cudaGetLastError());
+    return SGR_OK;
+}
+
+// the density estimation loss takes the field's sizes and one index row per sample
+static int densest_check(const SgrFieldParams *p, const void *own, const void *out)
+{
+    if (p && p->samples_per_idx_row > 1) {
+        set_error("bad field sizes: sgr_density_estimation_* takes one index row per sample");
+        return SGR_EINVAL;
+    }
+    if (p && p->N > 0 && (!own || !out)) {
+        set_error("null pointer passed to sgr_density_estimation_*");
+        return SGR_EINVAL;
+    }
+    return SGR_OK;
+}
+
+int sgr_density_estimation_forward(const SgrFieldParams *p, const float *x, const int64_t *own_idx,
+                                   const int64_t *nbr_idx, const float *points, const float *scaling,
+                                   const float *quaternions, const float *strengths, float *loss, float *nbr_opacity,
+                                   void *scratch, void *stream)
+{
+    int rc = field_check(p, x, nbr_idx, points, scaling, quaternions, strengths, scratch);
+    if (!rc) rc = densest_check(p, own_idx, loss);
+    if (rc) return rc;
+    if (p->N == 0) return SGR_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    Layout l(scratch);
+    float4 *rec = field_scratch(l, p->P).rec;
+    field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
+    const FieldArgs a = make_args(p, x, nbr_idx, rec);
+    const int G = group_width(p->K);
+    const int blocks = (p->N + 256 / G - 1) / (256 / G);
+#define SGR_DF(GW) densest_forward_kernel<GW><<<blocks, 256, 0, st>>>(a, own_idx, scaling, loss, nbr_opacity)
+    sgr::prof_begin(K_DENSEST_FWD, st);
+    switch (G) {
+        case 1: SGR_DF(1); break;
+        case 2: SGR_DF(2); break;
+        case 4: SGR_DF(4); break;
+        case 8: SGR_DF(8); break;
+        case 16: SGR_DF(16); break;
+        default: SGR_DF(32); break;
+    }
+    sgr::prof_end(st);
+#undef SGR_DF
+    SGR_CUDA(cudaGetLastError());
+    return SGR_OK;
+}
+
+int sgr_density_estimation_backward(const SgrFieldParams *p, const float *x, const int64_t *own_idx,
+                                    const int64_t *nbr_idx, const float *points, const float *scaling,
+                                    const float *quaternions, const float *strengths, const float *g_loss, float *g_x,
+                                    float *g_points, float *g_scaling, float *g_quaternions, float *g_strengths,
+                                    void *scratch, void *stream)
+{
+    int rc = field_check(p, x, nbr_idx, points, scaling, quaternions, strengths, scratch);
+    if (!rc) rc = densest_check(p, own_idx, g_loss);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    Layout l(scratch);
+    const auto [rec, grec] = field_scratch(l, p->P);
+    SGR_CUDA(cudaMemsetAsync(grec, 0, (size_t)p->P * 48, st));
+    if (p->N > 0) {
+        field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
+        const FieldArgs a = make_args(p, x, nbr_idx, rec);
+        const int G = group_width(p->K);
+        const int blocks = (p->N + 256 / G - 1) / (256 / G);
+#define SGR_DB(GW) densest_backward_kernel<GW><<<blocks, 256, 0, st>>>(a, own_idx, scaling, g_loss, g_x, grec)
+        sgr::prof_begin(K_DENSEST_BWD, st);
+        switch (G) {
+            case 1: SGR_DB(1); break;
+            case 2: SGR_DB(2); break;
+            case 4: SGR_DB(4); break;
+            case 8: SGR_DB(8); break;
+            case 16: SGR_DB(16); break;
+            default: SGR_DB(32); break;
+        }
+        sgr::prof_end(st);
+#undef SGR_DB
     }
     SGR_LAUNCH(K_FIELD_UNPACK, st,
                field_unpack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, (const float4 *)grec, g_points, g_scaling,

@@ -188,7 +188,7 @@ int once_per_device(DeviceOnce &once, int (*init)());
 enum KernelKind {
     K_PREPROCESS = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMEM, K_SORT_GLOBAL, K_BLEND_FWD, K_BLEND_BWD, K_PRE_BWD,
     K_FIELD_PACK, K_FIELD_FWD, K_FIELD_BWD, K_FIELD_UNPACK, K_KNN, K_KNN_QUERY, K_MISC, K_FINALIZE, K_PEER_REDUCE,
-    K_PEER_SYNC, K_LOSS_FWD, K_LOSS_BWD, K_MESH_NC_FWD, K_MESH_NC_BWD, K_NUM_KINDS
+    K_PEER_SYNC, K_LOSS_FWD, K_LOSS_BWD, K_DENSEST_FWD, K_DENSEST_BWD, K_MESH_NC_FWD, K_MESH_NC_BWD, K_NUM_KINDS
 };
 void prof_begin(int kind, cudaStream_t st);
 void prof_end(cudaStream_t st);

@@ -98,6 +98,60 @@ class _Field(torch.autograd.Function):
         return g_x, None, g_points, g_scaling, g_quat, g_str.view(s_shape), None, None, None, None, None
 
 
+class _DensityEstimation(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, gaussian_idx, nbr_idx, points, scaling, quaternions, strengths, density_factor, with_opacity):
+        dev = x.device
+        # floating inputs are taken as float32 and integer indices as int64; anything else fails tensor()'s dtype check
+        f32 = lambda t: t.float() if torch.is_tensor(t) and t.is_floating_point() else t
+        i64 = lambda t: t.long() if torch.is_tensor(t) and not t.is_floating_point() and t.dtype != torch.bool else t
+        x = tensor(f32(x), "x", torch.float32, ("N", 3))
+        points = tensor(f32(points), "points", torch.float32, ("P", 3), dev, "x")
+        N, P = x.shape[0], points.shape[0]
+        scaling = tensor(f32(scaling), "scaling", torch.float32, (P, 3), dev, "x")
+        quaternions = tensor(f32(quaternions), "quaternions", torch.float32, (P, 4), dev, "x")
+        strengths = f32(strengths)
+        one_d = torch.is_tensor(strengths) and strengths.dim() == 1
+        strengths = tensor(strengths, "strengths", torch.float32, (P,) if one_d else (P, 1), dev, "x")
+        gaussian_idx = tensor(i64(gaussian_idx), "gaussian_idx", torch.int64, (N,), dev, "x")
+        nbr_idx = tensor(i64(nbr_idx), "closest_gaussians_idx", torch.int64, (N, "K"), dev, "x")
+        K = nbr_idx.shape[1]
+        require_cuda("field", x)
+        with torch.cuda.device(dev):
+            loss = torch.empty(N, device=dev)
+            nbr = torch.empty((N, K) if with_opacity else (0, K), device=dev)
+            ws = scratch(lib.sgr_field_scratch_bytes(P), dev)
+            p = _params(N, K, P, density_factor, 1.0, 1e-16)
+            check(lib.sgr_density_estimation_forward(C.byref(p), ptr(x), ptr(gaussian_idx), ptr(nbr_idx), ptr(points),
+                                                     ptr(scaling), ptr(quaternions), ptr(strengths), ptr(loss),
+                                                     ptr(nbr), ptr(ws), stream(dev)))
+        ctx.save_for_backward(x, gaussian_idx, nbr_idx, points, scaling, quaternions, strengths)
+        ctx.cfg = (density_factor, strengths.shape)
+        ctx.mark_non_differentiable(nbr)
+        return loss, nbr
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_nbr):
+        x, gaussian_idx, nbr_idx, points, scaling, quaternions, strengths = ctx.saved_tensors
+        density_factor, s_shape = ctx.cfg
+        N, K, P = x.shape[0], nbr_idx.shape[1], points.shape[0]
+        dev = x.device
+        with torch.cuda.device(dev):
+            g_loss = g_loss.contiguous().float()
+            g_x = torch.empty_like(x)
+            g_points = torch.empty_like(points)
+            g_scaling = torch.empty_like(scaling)
+            g_quat = torch.empty_like(quaternions)
+            g_str = torch.empty(P, device=dev)
+            ws = scratch(lib.sgr_field_scratch_bytes(P), dev)
+            p = _params(N, K, P, density_factor, 1.0, 1e-16)
+            check(lib.sgr_density_estimation_backward(C.byref(p), ptr(x), ptr(gaussian_idx), ptr(nbr_idx), ptr(points),
+                                                      ptr(scaling), ptr(quaternions), ptr(strengths), ptr(g_loss),
+                                                      ptr(g_x), ptr(g_points), ptr(g_scaling), ptr(g_quat), ptr(g_str),
+                                                      ptr(ws), stream(dev)))
+        return g_x, None, None, g_points, g_scaling, g_quat, g_str.view(s_shape), None, None
+
+
 class _NormalLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gaussian_idx, nbr_idx, points, scaling, quaternions, nbr_opacity):
@@ -151,6 +205,28 @@ def better_normal_loss(x, gaussian_idx, closest_gaussians_idx, points, scaling, 
                                   "trainers' fixed setting, coarse_sdf.py:144) is implemented")
     return _NormalLoss.apply(x, gaussian_idx, closest_gaussians_idx, points, scaling, quaternions,
                              closest_gaussian_opacities)
+
+
+def density_estimation_loss(x, gaussian_idx, closest_gaussians_idx, points, scaling, quaternions, strengths,
+                            density_factor=1.0, return_closest_gaussian_opacities=False):
+    """Per-sample density estimation loss of the coarse_density trainer in projection mode
+    (sugar_trainers/coarse_density.py:642-656, 684-691): returns `sdf_estimation_loss` [N]; the caller adds
+    `factor * loss.mean()` over all samples (:691).
+
+        rho    = field_values(...)['density'] at x, before the straight-through clamp (sugar_model.py:1279)
+        beta   = mean of the K neighbours' smallest scales ('average' beta, :1192-1195)
+        e      = <x - points[gaussian_idx], n>, n the smallest axis of the sample's own Gaussian (get_normals)
+        loss   = | rho - exp(-0.5 e^2 / beta^2) |
+
+    x = sdf_samples, gaussian_idx = sdf_gaussian_idx, closest_gaussians_idx = knn_idx[gaussian_idx].  One fused
+    kernel evaluates it; the backward reaches x, points, scaling, quaternions and strengths (no gradient through
+    the argmin picking the normal's column).  With return_closest_gaussian_opacities, also returns the field's
+    [N, K] neighbour opacities (non-differentiable, for better_normal_loss), bit for bit those of field_values.
+    Shapes, dtypes and devices are checked (ValueError); index ranges are not, which would cost a host
+    synchronisation per step."""
+    loss, nbr = _DensityEstimation.apply(x, gaussian_idx, closest_gaussians_idx, points, scaling, quaternions,
+                                         strengths, density_factor, bool(return_closest_gaussian_opacities))
+    return (loss, nbr) if return_closest_gaussian_opacities else loss
 
 
 def field_values(x, closest_gaussians_idx, points, scaling, quaternions, strengths, density_factor=1.,

@@ -12,6 +12,9 @@
     7. "better normal" loss                                      :688-716
     8. one backward through all of it
 
+`coarse_density_step` is the same phase of the other coarse trainer (sugar_trainers/coarse_density.py, the
+`-r density` choice of train.py): no depth render, and the density estimation loss in place of steps 2-6.
+
 `refine_step` is the refinement loop's render (sugar_trainers/refine.py) for Gaussians bound to a mesh:
 barycentric centres, flat scales and face-normal-aligned rotations (sugar_model.py:384-398, 415-479, see
 sugar_b200/meshbind.py) followed by the RGB render and one backward.
@@ -23,6 +26,8 @@ fused kernels and over the reference's own building blocks (its CUDA rasterizer 
     ops.colors(points, sh, campos, sh_deg) -> colors_precomp or None (None: pass `shs` to the rasterizer)
     ops.field_values(x, nbr_idx, points, scaling, quaternions, strengths, **kw) -> dict
     ops.better_normal_loss(x, idx, nbr_idx, points, scaling, quaternions, nbr_opacity) -> [N]
+    ops.density_estimation_loss(x, idx, nbr_idx, points, scaling, quaternions, strengths, density_factor=,
+                                return_closest_gaussian_opacities=True) -> ([N], [N,K])   (coarse_density_step)
     ops.l1_dssim(pred, gt, dssim_factor) -> scalar   (only called with dssim_factor > 0)
     ops.mesh_normal_consistency(verts, faces, topology) -> scalar   (only called with normal_consistency_factor > 0)
     ops.rasterize_with_depth   sugar_b200.depth.rasterize_with_depth (only called with fused_depth=True; the
@@ -175,6 +180,45 @@ def coarse_sdf_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, density
     return loss.detach(), stats
 
 
+def coarse_density_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, density_factor=1.0,
+                        sdf_estimation_factor=0.2, sdf_better_normal_factor=0.2, sampling_scale_factor=1.5,
+                        generator=None, backward=True, dssim_factor=0.0):
+    """One regularised iteration of the coarse_density trainer (sugar_trainers/coarse_density.py:510-730, iteration
+    > 9000, the file's default switches: sdf_estimation_mode='density', use_projection_as_estimation=True,
+    density_factor = 1, sdf_sampling_proportional_to_volume=False):
+
+        1. RGB render of the view                                  :510-540
+        2. visible Gaussians (radii > 0): the sampling mask        :574 (projection mode samples in all of them)
+        3. n_samples inside them, uniformly per Gaussian, scale 1.5 :632-638
+        4. density estimation loss, K = 16 neighbours              :642-656, 684-691 (ops.density_estimation_loss)
+        5. "better normal" loss with the field's opacities         :702-730
+        6. one backward through all of it
+
+    Same arguments as coarse_sdf_step; no depth render.  Stats: visible and sampled_gaussians (the same Gaussians
+    in projection mode)."""
+    from .field import sample_points_in_gaussians
+    a = activate(raw)
+    dev = a.points.device
+    image, radii, _ = render(ops, a, cam, torch.zeros(3, device=dev), sh_deg=3)
+    loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
+    vis = radii > 0
+    n_vis = int(vis.sum())
+    stats = {"visible": n_vis, "sampled_gaussians": n_vis}
+    if n_vis > 0:
+        x, idx = sample_points_in_gaussians(a.points, a.scaling, a.quaternions, a.strengths, n_samples,
+                                            sampling_scale_factor=sampling_scale_factor, mask=vis,
+                                            probabilities_proportional_to_volume=False, generator=generator)
+        nbr = knn_idx[idx]
+        est, opac = ops.density_estimation_loss(x, idx, nbr, a.points, a.scaling, a.quaternions, a.strengths,
+                                                density_factor=density_factor, return_closest_gaussian_opacities=True)
+        loss = loss + sdf_estimation_factor * est.mean()
+        nl = ops.better_normal_loss(x, idx, nbr, a.points, a.scaling, a.quaternions, opac.detach())
+        loss = loss + sdf_better_normal_factor * nl.mean()
+    if backward:
+        loss.backward()
+    return loss.detach(), stats
+
+
 def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0, normal_consistency_factor=0.0):
     """One refinement iteration's render for mesh-bound Gaussians (sugar_trainers/refine.py; model properties
     sugar_model.py:384-398 points, :415-441 scaling, :443-479 quaternions).  `raw`: verts [V,3], sh_dc, sh_rest,
@@ -204,12 +248,13 @@ def camera_from_scene(sc, device):
 
 
 def ours_ops():
-    """This package's operators: in-kernel SH colours, fused field / normal-loss kernels, fused mesh binding, fused
-    L1 + D-SSIM loss, fused mesh normal consistency, colour + depth in one rasterizer call."""
+    """This package's operators: in-kernel SH colours, fused field / normal-loss / density-estimation kernels, fused
+    mesh binding, fused L1 + D-SSIM loss, fused mesh normal consistency, colour + depth in one rasterizer call."""
     from . import diff_gaussian_rasterization as dgr
     from . import depth, field, loss, meshbind, meshloss
     return SimpleNamespace(rasterizer=dgr, colors=lambda points, sh, campos, deg: None,
                            rasterize_with_depth=depth.rasterize_with_depth,
                            field_values=field.field_values, better_normal_loss=field.better_normal_loss,
+                           density_estimation_loss=field.density_estimation_loss,
                            bind_to_mesh=meshbind.bind_to_mesh, l1_dssim=loss.l1_dssim_loss,
                            mesh_normal_consistency=meshloss.mesh_normal_consistency)
