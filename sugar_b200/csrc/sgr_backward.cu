@@ -34,10 +34,6 @@ constexpr int BWD_NW = 8;   // warps per CTA (16x16 pixels)
 //   dcol   f32[P][3]  dL/dRGB, accumulated straight into the caller's dL_dcolors output.  With SH colours the
 //          channels the forward clamped (forward.cu:63-70) are masked here, so this array IS the per-view
 //          SH factor the view-parallel step exchanges, complete as soon as the blend pass ends.
-__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d)
-{
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 __device__ __forceinline__ void red_add_v2(float *addr, float a, float b)
 {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");

@@ -31,14 +31,6 @@ __global__ void __launch_bounds__(256) field_pack_kernel(int P, const float *__r
         make_float4(1.0f / fmaxf(s0, 1e-8f), 1.0f / fmaxf(s1, 1e-8f), 1.0f / fmaxf(s2, 1e-8f), fminf(s0, fminf(s1, s2)));
 }
 
-template <int G>
-__device__ __forceinline__ float group_sum(float v)
-{
-#pragma unroll
-    for (int o = G / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 struct FieldArgs {
     int N, K, P, group;
     float density_factor, sdf_offset, opacity_min_clamp;
@@ -99,29 +91,6 @@ __global__ void __launch_bounds__(256) field_forward_kernel(const FieldArgs a, f
     }
 }
 
-__device__ __forceinline__ void red_v4(float *addr, float a, float b, float c, float d)
-{
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-// dL/dq from A = dL/dR, R = I + ts * E(q) with ts = two_s = 2 / |q|^2 (pytorch3d's quaternion_to_matrix)
-__device__ __forceinline__ float4 rot_backward(const float (&A)[3][3], float4 q, float ts)
-{
-    const float qr = q.x, qi = q.y, qj = q.z, qk = q.w;
-    const float dts = A[0][0] * -(qj * qj + qk * qk) + A[0][1] * (qi * qj - qk * qr) + A[0][2] * (qi * qk + qj * qr) +
-                      A[1][0] * (qi * qj + qk * qr) + A[1][1] * -(qi * qi + qk * qk) + A[1][2] * (qj * qk - qi * qr) +
-                      A[2][0] * (qi * qk - qj * qr) + A[2][1] * (qj * qk + qi * qr) + A[2][2] * -(qi * qi + qj * qj);
-    const float c = -ts * ts * dts;  // d ts / d q_c = -ts^2 q_c
-    const float dqr = ts * (-qk * A[0][1] + qj * A[0][2] + qk * A[1][0] - qi * A[1][2] - qj * A[2][0] + qi * A[2][1]) + c * qr;
-    const float dqi = ts * (qj * (A[0][1] + A[1][0]) + qk * (A[0][2] + A[2][0]) + qr * (A[2][1] - A[1][2]) -
-                            2.f * qi * (A[1][1] + A[2][2])) + c * qi;
-    const float dqj = ts * (qi * (A[0][1] + A[1][0]) + qr * (A[0][2] - A[2][0]) + qk * (A[1][2] + A[2][1]) -
-                            2.f * qj * (A[0][0] + A[2][2])) + c * qj;
-    const float dqk = ts * (qr * (A[1][0] - A[0][1]) + qi * (A[0][2] + A[2][0]) + qj * (A[1][2] + A[2][1]) -
-                            2.f * qk * (A[0][0] + A[1][1])) + c * qk;
-    return make_float4(dqr, dqi, dqj, dqk);
-}
-
 // Pass 2 of a field backward for one (sample x, neighbour id) pair.  Gk = dL/d(the pair's opacity) in total, gb = dL/d
 // beta of the sample.  Adds dL/dx to gx and scatters dL/d(mu, sigma, q, s) into the Gaussian's 12-float gradient record:
 // dmu.xyz dsig | dq.rijk | ds.xyz -
@@ -148,20 +117,13 @@ __device__ __forceinline__ void field_pair_backward(float x0, float x1, float x2
     const float invs[3] = {r2.x, r2.y, r2.z};
     float du[3], ds[3];
     const float *sc = scaling + id * 3;
-    int amin = 0;
-    float smin = sc[0];
 #pragma unroll
     for (int j = 0; j < 3; j++) {
         const float dw = dd2 * 2.0f * w[j];
         du[j] = dw * invs[j];
-        const float sj = sc[j];
-        ds[j] = (sj >= 1e-8f) ? -(dw * u[j]) * invs[j] * invs[j] : 0.f;
-        if (j > 0 && sj < smin) {
-            smin = sj;
-            amin = j;
-        }
+        ds[j] = (sc[j] >= 1e-8f) ? -(dw * u[j]) * invs[j] * invs[j] : 0.f;
     }
-    ds[amin] += gb / (float)K;
+    ds[smallest_index(sc[0], sc[1], sc[2])] += gb / (float)K;
     float dsh[3];
 #pragma unroll
     for (int i = 0; i < 3; i++) dsh[i] = R.m[i][0] * du[0] + R.m[i][1] * du[1] + R.m[i][2] * du[2];
@@ -176,9 +138,9 @@ __device__ __forceinline__ void field_pair_backward(float x0, float x1, float x2
         for (int j = 0; j < 3; j++) A[i][j] = sh[i] * du[j];
     const float4 dq = rot_backward(A, r1, R.ts);
     float *gr = grec + id * 12;
-    red_v4(gr, -dsh[0], -dsh[1], -dsh[2], dsig);
-    red_v4(gr + 4, dq.x, dq.y, dq.z, dq.w);
-    red_v4(gr + 8, ds[0], ds[1], ds[2], 0.f);
+    red_add_v4(gr, -dsh[0], -dsh[1], -dsh[2], dsig);
+    red_add_v4(gr + 4, dq.x, dq.y, dq.z, dq.w);
+    red_add_v4(gr + 8, ds[0], ds[1], ds[2], 0.f);
 }
 
 template <int G>
@@ -249,13 +211,11 @@ __global__ void __launch_bounds__(256) field_backward_kernel(const FieldArgs a, 
 // with rho and beta the field's density (before the straight-through clamp) and beta at x.  The K terms are the field
 // forward's, in its lane order and butterfly, so rho and the neighbour opacities carry the field's bits.
 
-// <x - mu_g, n_g> for the sample's own Gaussian g; the column index comes from the float scaling row, so the 1e-8
-// clamp of the packed 1/s cannot change the pick
+// <x - mu_g, n_g> for the sample's own Gaussian g
 struct OwnAxis {
-    float e, n[3], d[3];  // d = x - mu_g
-    int col;
+    SmallestAxis ax;
     float4 q;
-    float ts;  // two_s of q
+    float e, d[3];  // d = x - mu_g
 };
 
 __device__ __forceinline__ OwnAxis own_axis(float x0, float x1, float x2, int64_t g, const float4 *__restrict__ rec,
@@ -264,20 +224,11 @@ __device__ __forceinline__ OwnAxis own_axis(float x0, float x1, float x2, int64_
     OwnAxis o;
     const float4 r0 = __ldg(rec + g * 3);
     o.q = __ldg(rec + g * 3 + 1);
-    const float *sc = scaling + g * 3;
-    const float s0 = sc[0], s1 = sc[1], s2 = sc[2];
-    o.col = 0;
-    float smin = s0;
-    if (s1 < smin) smin = s1, o.col = 1;
-    if (s2 < smin) o.col = 2;
-    const Rot R = quat_to_rot(o.q);
-    o.ts = R.ts;
-#pragma unroll
-    for (int i = 0; i < 3; i++) o.n[i] = o.col == 0 ? R.m[i][0] : (o.col == 1 ? R.m[i][1] : R.m[i][2]);
+    o.ax = smallest_axis(scaling + g * 3, o.q);
     o.d[0] = x0 - r0.x;
     o.d[1] = x1 - r0.y;
     o.d[2] = x2 - r0.z;
-    o.e = o.d[0] * o.n[0] + o.d[1] * o.n[1] + o.d[2] * o.n[2];
+    o.e = o.d[0] * o.ax.n[0] + o.d[1] * o.ax.n[1] + o.d[2] * o.ax.n[2];
     return o;
 }
 
@@ -368,25 +319,18 @@ __global__ void __launch_bounds__(256) densest_backward_kernel(const FieldArgs a
     // the own Gaussian's terms of e = <x - mu_g, n_g>: x, mu_g, and q_g through column `col` of R(q_g).  The axis is
     // gathered again rather than kept live through pass 2 (fewer registers for every lane)
     const int64_t og = own[n];
-    const OwnAxis ax = own_axis(x0, x1, x2, og, a.rec, scaling);
+    const OwnAxis o = own_axis(x0, x1, x2, og, a.rec, scaling);
     if (g_x) {
-        g_x[3 * n] = gx0 + ge * ax.n[0];
-        g_x[3 * n + 1] = gx1 + ge * ax.n[1];
-        g_x[3 * n + 2] = gx2 + ge * ax.n[2];
+        g_x[3 * n] = gx0 + ge * o.ax.n[0];
+        g_x[3 * n + 1] = gx1 + ge * o.ax.n[1];
+        g_x[3 * n + 2] = gx2 + ge * o.ax.n[2];
     }
     if (ge == 0.f) return;
-    float A[3][3];
-#pragma unroll
-    for (int i = 0; i < 3; i++) {
-        const float dn = ge * ax.d[i];
-        A[i][0] = ax.col == 0 ? dn : 0.f;
-        A[i][1] = ax.col == 1 ? dn : 0.f;
-        A[i][2] = ax.col == 2 ? dn : 0.f;
-    }
-    const float4 dq = rot_backward(A, ax.q, ax.ts);
+    const float dn[3] = {ge * o.d[0], ge * o.d[1], ge * o.d[2]};
+    const float4 dq = smallest_axis_backward(o.ax, o.q, dn);
     float *gr = grec + og * 12;
-    red_v4(gr, -ge * ax.n[0], -ge * ax.n[1], -ge * ax.n[2], 0.f);
-    red_v4(gr + 4, dq.x, dq.y, dq.z, dq.w);
+    red_add_v4(gr, -ge * o.ax.n[0], -ge * o.ax.n[1], -ge * o.ax.n[2], 0.f);
+    red_add_v4(gr + 4, dq.x, dq.y, dq.z, dq.w);
 }
 
 __global__ void __launch_bounds__(256) field_unpack_kernel(int P, const float4 *__restrict__ grec, float *g_points,
@@ -467,18 +411,9 @@ int sgr_field_forward(const SgrFieldParams *p, const float *x, const int64_t *nb
     float4 *rec = field_scratch(l, p->P).rec;
     field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
     const FieldArgs a = make_args(p, x, nbr_idx, rec);
-    const int G = group_width(p->K);
-    const int blocks = (p->N + 256 / G - 1) / (256 / G);
-    sgr::prof_begin(K_FIELD_FWD, st);
-    switch (G) {
-        case 1: field_forward_kernel<1><<<blocks, 256, 0, st>>>(a, density, nbr_opacity, beta, sdf); break;
-        case 2: field_forward_kernel<2><<<blocks, 256, 0, st>>>(a, density, nbr_opacity, beta, sdf); break;
-        case 4: field_forward_kernel<4><<<blocks, 256, 0, st>>>(a, density, nbr_opacity, beta, sdf); break;
-        case 8: field_forward_kernel<8><<<blocks, 256, 0, st>>>(a, density, nbr_opacity, beta, sdf); break;
-        case 16: field_forward_kernel<16><<<blocks, 256, 0, st>>>(a, density, nbr_opacity, beta, sdf); break;
-        default: field_forward_kernel<32><<<blocks, 256, 0, st>>>(a, density, nbr_opacity, beta, sdf); break;
-    }
-    sgr::prof_end(st);
+    SGR_LAUNCH(K_FIELD_FWD, st, with_group_width(p->K, [&](auto G) {
+                   field_forward_kernel<G><<<(a.N + 256 / G - 1) / (256 / G), 256, 0, st>>>(a, density, nbr_opacity, beta, sdf);
+               }));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }
@@ -493,29 +428,18 @@ int sgr_field_backward(const SgrFieldParams *p, const float *x, const int64_t *n
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     Layout l(scratch);
-    const auto [rec, grec] = field_scratch(l, p->P);
-    SGR_CUDA(cudaMemsetAsync(grec, 0, (size_t)p->P * 48, st));
+    const FieldScratch s = field_scratch(l, p->P);
+    SGR_CUDA(cudaMemsetAsync(s.grec, 0, (size_t)p->P * 48, st));
     if (p->N > 0) {
-        field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
-        const FieldArgs a = make_args(p, x, nbr_idx, rec);
-        const int G = group_width(p->K);
-        const int blocks = (p->N + 256 / G - 1) / (256 / G);
-#define SGR_FB(GW)                                                                                                   \
-    field_backward_kernel<GW><<<blocks, 256, 0, st>>>(a, scaling, g_density, g_nbr_opacity, g_beta, g_sdf, g_x, grec)
-        sgr::prof_begin(K_FIELD_BWD, st);
-        switch (G) {
-            case 1: SGR_FB(1); break;
-            case 2: SGR_FB(2); break;
-            case 4: SGR_FB(4); break;
-            case 8: SGR_FB(8); break;
-            case 16: SGR_FB(16); break;
-            default: SGR_FB(32); break;
-        }
-        sgr::prof_end(st);
-#undef SGR_FB
+        field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, s.rec, st);
+        const FieldArgs a = make_args(p, x, nbr_idx, s.rec);
+        SGR_LAUNCH(K_FIELD_BWD, st, with_group_width(p->K, [&](auto G) {
+                       field_backward_kernel<G><<<(a.N + 256 / G - 1) / (256 / G), 256, 0, st>>>(
+                           a, scaling, g_density, g_nbr_opacity, g_beta, g_sdf, g_x, s.grec);
+                   }));
     }
     SGR_LAUNCH(K_FIELD_UNPACK, st,
-               field_unpack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, (const float4 *)grec, g_points, g_scaling,
+               field_unpack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, (const float4 *)s.grec, g_points, g_scaling,
                                                                        g_quaternions, g_strengths));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
@@ -549,20 +473,10 @@ int sgr_density_estimation_forward(const SgrFieldParams *p, const float *x, cons
     float4 *rec = field_scratch(l, p->P).rec;
     field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
     const FieldArgs a = make_args(p, x, nbr_idx, rec);
-    const int G = group_width(p->K);
-    const int blocks = (p->N + 256 / G - 1) / (256 / G);
-#define SGR_DF(GW) densest_forward_kernel<GW><<<blocks, 256, 0, st>>>(a, own_idx, scaling, loss, nbr_opacity)
-    sgr::prof_begin(K_DENSEST_FWD, st);
-    switch (G) {
-        case 1: SGR_DF(1); break;
-        case 2: SGR_DF(2); break;
-        case 4: SGR_DF(4); break;
-        case 8: SGR_DF(8); break;
-        case 16: SGR_DF(16); break;
-        default: SGR_DF(32); break;
-    }
-    sgr::prof_end(st);
-#undef SGR_DF
+    SGR_LAUNCH(K_DENSEST_FWD, st, with_group_width(p->K, [&](auto G) {
+                   densest_forward_kernel<G><<<(a.N + 256 / G - 1) / (256 / G), 256, 0, st>>>(a, own_idx, scaling, loss,
+                                                                                              nbr_opacity);
+               }));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }
@@ -578,28 +492,18 @@ int sgr_density_estimation_backward(const SgrFieldParams *p, const float *x, con
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     Layout l(scratch);
-    const auto [rec, grec] = field_scratch(l, p->P);
-    SGR_CUDA(cudaMemsetAsync(grec, 0, (size_t)p->P * 48, st));
+    const FieldScratch s = field_scratch(l, p->P);
+    SGR_CUDA(cudaMemsetAsync(s.grec, 0, (size_t)p->P * 48, st));
     if (p->N > 0) {
-        field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, rec, st);
-        const FieldArgs a = make_args(p, x, nbr_idx, rec);
-        const int G = group_width(p->K);
-        const int blocks = (p->N + 256 / G - 1) / (256 / G);
-#define SGR_DB(GW) densest_backward_kernel<GW><<<blocks, 256, 0, st>>>(a, own_idx, scaling, g_loss, g_x, grec)
-        sgr::prof_begin(K_DENSEST_BWD, st);
-        switch (G) {
-            case 1: SGR_DB(1); break;
-            case 2: SGR_DB(2); break;
-            case 4: SGR_DB(4); break;
-            case 8: SGR_DB(8); break;
-            case 16: SGR_DB(16); break;
-            default: SGR_DB(32); break;
-        }
-        sgr::prof_end(st);
-#undef SGR_DB
+        field_pack(K_FIELD_PACK, p->P, points, scaling, quaternions, strengths, s.rec, st);
+        const FieldArgs a = make_args(p, x, nbr_idx, s.rec);
+        SGR_LAUNCH(K_DENSEST_BWD, st, with_group_width(p->K, [&](auto G) {
+                       densest_backward_kernel<G><<<(a.N + 256 / G - 1) / (256 / G), 256, 0, st>>>(a, own_idx, scaling,
+                                                                                                   g_loss, g_x, s.grec);
+                   }));
     }
     SGR_LAUNCH(K_FIELD_UNPACK, st,
-               field_unpack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, (const float4 *)grec, g_points, g_scaling,
+               field_unpack_kernel<<<(p->P + 255) / 256, 256, 0, st>>>(p->P, (const float4 *)s.grec, g_points, g_scaling,
                                                                        g_quaternions, g_strengths));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;

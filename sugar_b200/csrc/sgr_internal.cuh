@@ -439,6 +439,12 @@ __device__ __forceinline__ float warp_sum(float v)
     return v;
 }
 
+// one 16-byte vector reduction into global memory (SASS REDG.E.ADD.F32x4)
+__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d)
+{
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+
 // ---- async-copy / mbarrier primitives (sm_90+ bulk copies: SASS UBLKCP; cp.async: LDGSTS) ----
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count)

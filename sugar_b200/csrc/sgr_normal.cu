@@ -12,38 +12,11 @@
 // The reference gathers N x K x 3 normals, points and several N x K temporaries through autograd;
 // here every Gaussian's normal is packed once (32 B record), one lane owns one (sample, neighbour)
 // pair, and the backward scatters dL/dn with 16-byte vector reductions before one per-Gaussian
-// pass maps dL/dn to dL/dquaternion (pytorch3d quaternion_to_matrix, two_s = 2/|q|^2).
-#include "sgr_internal.cuh"
+// pass maps dL/dn to dL/dquaternion (pytorch3d quaternion_to_matrix, two_s = 2/|q|^2).  The normal, its quaternion
+// backward, the lane groups and their sums are the field kernels' (sgr_field.cuh).
+#include "sgr_field.cuh"
 
 namespace sgr {
-
-__device__ __forceinline__ void quat_column(float4 q, int col, float &nx, float &ny, float &nz)
-{
-    const float r = q.x, i = q.y, j = q.z, k = q.w;
-    const float ts = 2.0f / (r * r + i * i + j * j + k * k);
-    if (col == 0) {
-        nx = 1 - ts * (j * j + k * k);
-        ny = ts * (i * j + k * r);
-        nz = ts * (i * k - j * r);
-    } else if (col == 1) {
-        nx = ts * (i * j - k * r);
-        ny = 1 - ts * (i * i + k * k);
-        nz = ts * (j * k + i * r);
-    } else {
-        nx = ts * (i * k + j * r);
-        ny = ts * (j * k - i * r);
-        nz = 1 - ts * (i * i + j * j);
-    }
-}
-
-__device__ __forceinline__ int smallest_axis(const float *s, float &smin)
-{
-    int a = 0;
-    smin = s[0];
-    if (s[1] < smin) smin = s[1], a = 1;
-    if (s[2] < smin) smin = s[2], a = 2;
-    return a;  // first minimum, like torch.min(dim)
-}
 
 // per-Gaussian record, 8 floats: n.xyz, 1/max(s_min,1e-6)^2 | mu.xyz, -
 __global__ void __launch_bounds__(256) normal_pack_kernel(int P, const float *__restrict__ points,
@@ -53,21 +26,10 @@ __global__ void __launch_bounds__(256) normal_pack_kernel(int P, const float *__
     const int g = blockIdx.x * 256 + threadIdx.x;
     if (g >= P) return;
     const float s[3] = {scaling[3 * g], scaling[3 * g + 1], scaling[3 * g + 2]};
-    float smin;
-    const int col = smallest_axis(s, smin);
-    float nx, ny, nz;
-    quat_column(((const float4 *)quats)[g], col, nx, ny, nz);
-    const float c = fmaxf(smin, 1e-6f);
-    rec[(size_t)g * 2] = make_float4(nx, ny, nz, 1.0f / (c * c));
+    const SmallestAxis ax = smallest_axis(s, ((const float4 *)quats)[g]);
+    const float c = fmaxf(ax.col == 0 ? s[0] : (ax.col == 1 ? s[1] : s[2]), 1e-6f);
+    rec[(size_t)g * 2] = make_float4(ax.n[0], ax.n[1], ax.n[2], 1.0f / (c * c));
     rec[(size_t)g * 2 + 1] = make_float4(points[3 * g], points[3 * g + 1], points[3 * g + 2], 0.f);
-}
-
-template <int G>
-__device__ __forceinline__ float gsum(float v)
-{
-#pragma unroll
-    for (int o = G / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
 }
 
 struct NormalArgs {
@@ -101,10 +63,10 @@ __device__ __forceinline__ float sample_residual(const NormalArgs &a, bool live,
         sy += w * sg * r0.y;
         sz += w * sg * r0.z;
     }
-    wsum = gsum<G>(wsum);
-    sx = gsum<G>(sx);
-    sy = gsum<G>(sy);
-    sz = gsum<G>(sz);
+    wsum = group_sum<G>(wsum);
+    sx = group_sum<G>(sx);
+    sy = group_sum<G>(sy);
+    sz = group_sum<G>(sz);
     const float inv = 1.0f / fmaxf(wsum, 1e-6f);
     vx = n0.x - sx * inv;
     vy = n0.y - sy * inv;
@@ -125,11 +87,6 @@ __global__ void __launch_bounds__(256) normal_loss_forward_kernel(const NormalAr
     if (live && l == 0) loss[n] = vx * vx + vy * vy + vz * vz;
 }
 
-__device__ __forceinline__ void red4(float *addr, float a, float b, float c, float d)
-{
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
 template <int G>
 __global__ void __launch_bounds__(256) normal_loss_backward_kernel(const NormalArgs a, const float *__restrict__ g_loss,
                                                                    float *__restrict__ dnrm /* float4[P] */)
@@ -145,7 +102,7 @@ __global__ void __launch_bounds__(256) normal_loss_backward_kernel(const NormalA
     if (!live) return;
     const float g2 = 2.0f * g_loss[n];
     if (g2 == 0.f) return;
-    if (l == 0) red4(dnrm + own * 4, g2 * vx, g2 * vy, g2 * vz, 0.f);
+    if (l == 0) red_add_v4(dnrm + own * 4, g2 * vx, g2 * vy, g2 * vz, 0.f);
     const float x0 = a.x[3 * n], x1 = a.x[3 * n + 1], x2 = a.x[3 * n + 2];
     for (int k = l; k < a.K; k += G) {
         const int64_t id = a.idx[(size_t)n * a.K + k];
@@ -155,11 +112,11 @@ __global__ void __launch_bounds__(256) normal_loss_backward_kernel(const NormalA
         const float w = a.opac[(size_t)n * a.K + k] *
                         fabsf(((x0 - r1.x) * r0.x + (x1 - r1.y) * r0.y + (x2 - r1.z) * r0.z) * sg) * r0.w * inv;
         const float c = -g2 * w * sg;
-        if (c != 0.f) red4(dnrm + id * 4, c * vx, c * vy, c * vz, 0.f);
+        if (c != 0.f) red_add_v4(dnrm + id * 4, c * vx, c * vy, c * vz, 0.f);
     }
 }
 
-// dL/dq from dL/dn, n = column `col` of R(q) = I + ts * E(q)
+// dL/dq from dL/dn
 __global__ void __launch_bounds__(256) normal_unpack_kernel(int P, const float *__restrict__ scaling,
                                                             const float *__restrict__ quats,
                                                             const float4 *__restrict__ dnrm, float4 *__restrict__ g_quats)
@@ -171,52 +128,9 @@ __global__ void __launch_bounds__(256) normal_unpack_kernel(int P, const float *
         g_quats[g] = make_float4(0, 0, 0, 0);
         return;
     }
-    const float s[3] = {scaling[3 * g], scaling[3 * g + 1], scaling[3 * g + 2]};
-    float smin;
-    const int col = smallest_axis(s, smin);
     const float4 q = ((const float4 *)quats)[g];
-    const float r = q.x, i = q.y, j = q.z, k = q.w;
-    const float ts = 2.0f / (r * r + i * i + j * j + k * k);
-    // E column and its derivatives w.r.t. (r,i,j,k); n = e_col + ts * E[:,col]
-    float E[3], dEr[3], dEi[3], dEj[3], dEk[3];
-    if (col == 0) {
-        E[0] = -(j * j + k * k), E[1] = i * j + k * r, E[2] = i * k - j * r;
-        dEr[0] = 0, dEr[1] = k, dEr[2] = -j;
-        dEi[0] = 0, dEi[1] = j, dEi[2] = k;
-        dEj[0] = -2 * j, dEj[1] = i, dEj[2] = -r;
-        dEk[0] = -2 * k, dEk[1] = r, dEk[2] = i;
-    } else if (col == 1) {
-        E[0] = i * j - k * r, E[1] = -(i * i + k * k), E[2] = j * k + i * r;
-        dEr[0] = -k, dEr[1] = 0, dEr[2] = i;
-        dEi[0] = j, dEi[1] = -2 * i, dEi[2] = r;
-        dEj[0] = i, dEj[1] = 0, dEj[2] = k;
-        dEk[0] = -r, dEk[1] = -2 * k, dEk[2] = j;
-    } else {
-        E[0] = i * k + j * r, E[1] = j * k - i * r, E[2] = -(i * i + j * j);
-        dEr[0] = j, dEr[1] = -i, dEr[2] = 0;
-        dEi[0] = k, dEi[1] = -r, dEi[2] = -2 * i;
-        dEj[0] = r, dEj[1] = k, dEj[2] = -2 * j;
-        dEk[0] = i, dEk[1] = j, dEk[2] = 0;
-    }
-    const float dv[3] = {d.x, d.y, d.z};
-    float dts = 0.f, gr = 0.f, gi = 0.f, gj = 0.f, gk = 0.f;
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-        dts += dv[c] * E[c];
-        gr += dv[c] * dEr[c];
-        gi += dv[c] * dEi[c];
-        gj += dv[c] * dEj[c];
-        gk += dv[c] * dEk[c];
-    }
-    const float cc = -ts * ts * dts;  // d ts / d q_c = -ts^2 q_c
-    g_quats[g] = make_float4(ts * gr + cc * r, ts * gi + cc * i, ts * gj + cc * j, ts * gk + cc * k);
-}
-
-static int group_width_n(int K)
-{
-    int G = 1;
-    while (G < K && G < 32) G <<= 1;
-    return G;
+    const float dn[3] = {d.x, d.y, d.z};
+    g_quats[g] = smallest_axis_backward(smallest_axis(scaling + 3 * g, q), q, dn);
 }
 
 // the packed records, then the backward's per-Gaussian normal gradients
@@ -261,17 +175,9 @@ int sgr_normal_loss_forward(int32_t N, int32_t K, int32_t P, const float *x, con
     float4 *rec = normal_scratch(l, P).rec;
     SGR_LAUNCH(K_FIELD_PACK, st, normal_pack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec));
     NormalArgs a{N, K, x, own_idx, nbr_idx, rec, nbr_opacity};
-    const int G = group_width_n(K), blocks = (N + 256 / G - 1) / (256 / G);
-    sgr::prof_begin(K_FIELD_FWD, st);
-    switch (G) {
-        case 1: normal_loss_forward_kernel<1><<<blocks, 256, 0, st>>>(a, loss); break;
-        case 2: normal_loss_forward_kernel<2><<<blocks, 256, 0, st>>>(a, loss); break;
-        case 4: normal_loss_forward_kernel<4><<<blocks, 256, 0, st>>>(a, loss); break;
-        case 8: normal_loss_forward_kernel<8><<<blocks, 256, 0, st>>>(a, loss); break;
-        case 16: normal_loss_forward_kernel<16><<<blocks, 256, 0, st>>>(a, loss); break;
-        default: normal_loss_forward_kernel<32><<<blocks, 256, 0, st>>>(a, loss); break;
-    }
-    sgr::prof_end(st);
+    SGR_LAUNCH(K_FIELD_FWD, st, with_group_width(K, [&](auto G) {
+                   normal_loss_forward_kernel<G><<<(N + 256 / G - 1) / (256 / G), 256, 0, st>>>(a, loss);
+               }));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }
@@ -289,25 +195,17 @@ int sgr_normal_loss_backward(int32_t N, int32_t K, int32_t P, const float *x, co
     }
     cudaStream_t st = (cudaStream_t)stream;
     Layout l(scratch);
-    const auto [rec, dnrm] = normal_scratch(l, P);
-    SGR_CUDA(cudaMemsetAsync(dnrm, 0, (size_t)P * 16, st));
+    const NormalScratch s = normal_scratch(l, P);
+    SGR_CUDA(cudaMemsetAsync(s.dnrm, 0, (size_t)P * 16, st));
     if (N > 0) {
-        SGR_LAUNCH(K_FIELD_PACK, st, normal_pack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec));
-        NormalArgs a{N, K, x, own_idx, nbr_idx, rec, nbr_opacity};
-        const int G = group_width_n(K), blocks = (N + 256 / G - 1) / (256 / G);
-        sgr::prof_begin(K_FIELD_BWD, st);
-        switch (G) {
-            case 1: normal_loss_backward_kernel<1><<<blocks, 256, 0, st>>>(a, g_loss, dnrm); break;
-            case 2: normal_loss_backward_kernel<2><<<blocks, 256, 0, st>>>(a, g_loss, dnrm); break;
-            case 4: normal_loss_backward_kernel<4><<<blocks, 256, 0, st>>>(a, g_loss, dnrm); break;
-            case 8: normal_loss_backward_kernel<8><<<blocks, 256, 0, st>>>(a, g_loss, dnrm); break;
-            case 16: normal_loss_backward_kernel<16><<<blocks, 256, 0, st>>>(a, g_loss, dnrm); break;
-            default: normal_loss_backward_kernel<32><<<blocks, 256, 0, st>>>(a, g_loss, dnrm); break;
-        }
-        sgr::prof_end(st);
+        SGR_LAUNCH(K_FIELD_PACK, st, normal_pack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, s.rec));
+        NormalArgs a{N, K, x, own_idx, nbr_idx, s.rec, nbr_opacity};
+        SGR_LAUNCH(K_FIELD_BWD, st, with_group_width(K, [&](auto G) {
+                       normal_loss_backward_kernel<G><<<(N + 256 / G - 1) / (256 / G), 256, 0, st>>>(a, g_loss, s.dnrm);
+                   }));
     }
     SGR_LAUNCH(K_FIELD_UNPACK, st,
-               normal_unpack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, scaling, quaternions, (const float4 *)dnrm,
+               normal_unpack_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, scaling, quaternions, (const float4 *)s.dnrm,
                                                                      (float4 *)g_quaternions));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
