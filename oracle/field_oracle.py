@@ -24,6 +24,9 @@ as they stand (tests/golden/make_levelset_golden.py).
 import numpy as np
 import torch
 
+# The clamp bounds as the float32 constants the reference's float32 tensors compare against (torch casts a Python
+# scalar to the tensor's dtype), so a float64 run clamps at exactly the same inputs as the float32 one.
+_f32 = lambda v: float(np.float32(v))
 
 def quaternion_to_matrix(q: torch.Tensor) -> torch.Tensor:
     """pytorch3d.transforms.quaternion_to_matrix (0.7.4): real part first, two_s = 2/|q|^2."""
@@ -50,7 +53,8 @@ def knn_idx(points: torch.Tensor, K: int, queries: torch.Tensor = None) -> torch
 def field_values_torch(x, nbr_idx, points, scaling, quaternions, strengths, density_factor=1.0,
                        density_threshold=1.0, opacity_min_clamp=1e-16, return_sdf_grad=False, sdf_grad_max_value=10.0):
     """get_field_values with closest_gaussians_idx given; tensors may require grad."""
-    s = 1.0 / scaling.clamp(min=1e-8)
+    opacity_min_clamp = _f32(opacity_min_clamp)
+    s = 1.0 / scaling.clamp(min=_f32(1e-8))
     inv_scaled_rot = quaternion_to_matrix(quaternions) * s[:, None]          # :730-735
     c_centers = points[nbr_idx]
     c_isr = inv_scaled_rot[nbr_idx]
@@ -126,8 +130,8 @@ def better_normal_loss_torch(x, gaussian_idx, nbr_idx, points, scaling, quaterni
     s_normals = normals[gaussian_idx]                                                            # :697
     c_normals = c_normals * torch.sign((c_normals * s_normals[:, None]).sum(dim=-1, keepdim=True)).detach()  # :698-700
     w = ((x[:, None] - points[nbr_idx]) * c_normals).sum(dim=-1).abs().detach()                  # :704-706
-    w = nbr_opacity.detach() * w / min_scaling.clamp(min=1e-6) ** 2                              # :707
-    w = w / w.sum(dim=-1).detach().unsqueeze(-1).clamp(min=1e-6)                                 # :710-711
+    w = nbr_opacity.detach() * w / min_scaling.clamp(min=_f32(1e-6)) ** 2                              # :707
+    w = w / w.sum(dim=-1).detach().unsqueeze(-1).clamp(min=_f32(1e-6))                                 # :710-711
     return (s_normals - (w[..., None] * c_normals).sum(dim=-2)).pow(2).sum(dim=-1)               # :714-715
 
 
@@ -147,7 +151,7 @@ def level_surface_points_torch(world_points, camera_center, closest_gaussians_id
     samples = (world_points[:, None, :] + rng * cam_to_samples[:, None, :]).view(-1, 3)
     K = closest_gaussians_idx.shape[1]
     s_idx = closest_gaussians_idx[:, None, :].expand(-1, n_points_in_range, -1).reshape(-1, K)
-    isr = quaternion_to_matrix(quaternions) * (1.0 / scaling.clamp(min=1e-8))[:, None]                      # :1986
+    isr = quaternion_to_matrix(quaternions) * (1.0 / scaling.clamp(min=_f32(1e-8)))[:, None]                      # :1986
     str_ = strengths.view(-1, 1)
 
     def opac(x, idx):

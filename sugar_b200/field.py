@@ -72,6 +72,9 @@ class _Field(torch.autograd.Function):
         ctx.save_for_backward(x, nbr_idx, points, scaling, quaternions, strengths)
         ctx.cfg = (density_factor, density_threshold, opacity_min_clamp, strengths.shape, group, outputs)
         ctx.mark_non_differentiable(nbr_idx)
+        # an output the loss does not use must not reach the kernel as zeros: at rho >= 1 the sdf's d/d rho is
+        # infinite (sqrt'(0)) and 0 * inf would make the sample's gradients NaN where the reference's are finite
+        ctx.set_materialize_grads(False)
         return density, nbr, beta, sdf
 
     @staticmethod
