@@ -16,6 +16,7 @@
 #include <mutex>
 
 #include "sgr_internal.cuh"
+#include "sgr_sh.cuh"
 
 namespace sgr {
 
@@ -470,124 +471,32 @@ struct PreBwdArgs {
     int pf_off;  // floats: where the other views' factor blocks land in shared memory (MULTI)
 };
 
-#define SH_C0 0.28209479177387814f
-#define SH_C1 0.4886025119029199f
-__constant__ float b_SH_C2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
-                                 -1.0925484305920792f, 0.5462742152960396f};
-__constant__ float b_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
-                                 0.3731763325901154f, -0.4570457994644658f, 1.445305721320277f,
-                                 -0.5900435899266435f};
-
-struct f3 {
-    float x, y, z;
-};
-
 // dL/dsh of one view (backward.cu:20-139: dL/dsh_k = basis_k(dir) dL/dRGB) into one shared-memory row [M][3].
 // Write-only: the view-direction term, the only use the reference makes of the coefficients, comes from the
 // forward's Jacobian rows (sh_dir_grad).  `dc` is coefficient 0's row of three, `rest` coefficient 1's (one combined
-// row: rest = dc + 3; raw-parameter mode: two arrays).
+// row: rest = dc + 3; raw-parameter mode: two arrays).  OTHERS: the other views' SH gradients of this Gaussian
+// (registers, `oacc`) join the row here.
 template <bool OTHERS = false>
-__device__ __forceinline__ void sh_grad_row(int deg, int M, float *dc, float *rest, f3 dir_orig, f3 dRGB,
+__device__ __forceinline__ void sh_grad_row(int deg, int M, float *dc, float *rest, f3 d, f3 dRGB,
                                             float out_scale = 1.0f, const float *oacc = nullptr)
 {
     const f3 dS = {dRGB.x * out_scale, dRGB.y * out_scale, dRGB.z * out_scale};  // x 1.0f is exact
-    const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
-    const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
-#define SHB(k, w)                                                                      \
-    {                                                                                  \
-        float *q_ = (k) == 0 ? dc : rest + ((k) - 1) * 3;                              \
-        const float w_ = (w);                                                          \
-        if (OTHERS) { /* the other views' SH gradients of this Gaussian (registers) join the row here */ \
-            q_[0] = fmaf(w_, dS.x, oacc[(k) * 3]);                                     \
-            q_[1] = fmaf(w_, dS.y, oacc[(k) * 3 + 1]);                                 \
-            q_[2] = fmaf(w_, dS.z, oacc[(k) * 3 + 2]);                                 \
-        } else {                                                                       \
-            q_[0] = w_ * dS.x;                                                         \
-            q_[1] = w_ * dS.y;                                                         \
-            q_[2] = w_ * dS.z;                                                         \
-        }                                                                              \
-    }
-    SHB(0, SH_C0);
-    if (deg > 0) {
-        SHB(1, -SH_C1 * y);
-        SHB(2, SH_C1 * z);
-        SHB(3, -SH_C1 * x);
-        if (deg > 1) {
-            const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-            SHB(4, b_SH_C2[0] * xy);
-            SHB(5, b_SH_C2[1] * yz);
-            SHB(6, b_SH_C2[2] * (2.f * zz - xx - yy));
-            SHB(7, b_SH_C2[3] * xz);
-            SHB(8, b_SH_C2[4] * (xx - yy));
-            if (deg > 2) {
-                SHB(9, b_SH_C3[0] * y * (3.f * xx - yy));
-                SHB(10, b_SH_C3[1] * xy * z);
-                SHB(11, b_SH_C3[2] * y * (4.f * zz - xx - yy));
-                SHB(12, b_SH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy));
-                SHB(13, b_SH_C3[4] * x * (4.f * zz - xx - yy));
-                SHB(14, b_SH_C3[5] * z * (xx - yy));
-                SHB(15, b_SH_C3[6] * x * (xx - 3.f * yy));
-            }
+    sh_for_active(deg, [&](auto k) {
+        constexpr int K = decltype(k)::value;
+        float *q = K == 0 ? dc : rest + (K - 1) * 3;
+        const float w = sh_basis<K>(d);
+        if constexpr (OTHERS) {
+            q[0] = fmaf(w, dS.x, oacc[K * 3]);
+            q[1] = fmaf(w, dS.y, oacc[K * 3 + 1]);
+            q[2] = fmaf(w, dS.z, oacc[K * 3 + 2]);
+        } else {
+            q[0] = w * dS.x;
+            q[1] = w * dS.y;
+            q[2] = w * dS.z;
         }
-    }
-#undef SHB
+    });
     // rows above the active degree stay zero (the reference returns zero-filled dL_dsh)
     for (int k = (deg + 1) * (deg + 1) * 3 - 3; k < (M - 1) * 3; k++) rest[k] = 0.f;
-}
-
-// The view-direction term of dL/dmean3D (backward.cu:127-133): dL/ddir = (<dRGBdx, dL/dRGB>, <dRGBdy, ..>,
-// <dRGBdz, ..>) from the Jacobian row `jac` the forward stored, then dnormvdv (auxiliary.h:107-117).
-__device__ __forceinline__ f3 sh_dir_grad(const float *jac, f3 dRGB)
-{
-    return {jac[0] * dRGB.x + jac[1] * dRGB.y + jac[2] * dRGB.z, jac[3] * dRGB.x + jac[4] * dRGB.y + jac[5] * dRGB.z,
-            jac[6] * dRGB.x + jac[7] * dRGB.y + jac[8] * dRGB.z};
-}
-__device__ __forceinline__ void add_dnormvdv(f3 o, f3 ddir, f3 &dmean)
-{
-    const float sum2 = o.x * o.x + o.y * o.y + o.z * o.z;
-    const float invsum32 = 1.0f / sqrtf(sum2 * sum2 * sum2);
-    dmean.x += ((+sum2 - o.x * o.x) * ddir.x - o.y * o.x * ddir.y - o.z * o.x * ddir.z) * invsum32;
-    dmean.y += (-o.x * o.y * ddir.x + (sum2 - o.y * o.y) * ddir.y - o.z * o.y * ddir.z) * invsum32;
-    dmean.z += (-o.x * o.z * ddir.x - o.y * o.z * ddir.y + (sum2 - o.z * o.z) * ddir.z) * invsum32;
-}
-
-// Another view's SH gradient of one Gaussian, accumulated in registers: acc[3k + c] += basis_k(normalize(dir)) * g_c
-// (the dL_dsh part of backward.cu:20-139 is this outer product per view).
-__device__ __forceinline__ void sh_accumulate(int deg, float *acc, f3 dir_orig, f3 g)
-{
-    const float inv = 1.0f / sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
-    const float x = dir_orig.x * inv, y = dir_orig.y * inv, z = dir_orig.z * inv;
-#define SHA(k, w)                                           \
-    {                                                       \
-        const float w_ = (w);                               \
-        acc[(k) * 3] = fmaf(w_, g.x, acc[(k) * 3]);         \
-        acc[(k) * 3 + 1] = fmaf(w_, g.y, acc[(k) * 3 + 1]); \
-        acc[(k) * 3 + 2] = fmaf(w_, g.z, acc[(k) * 3 + 2]); \
-    }
-    SHA(0, SH_C0);
-    if (deg > 0) {
-        SHA(1, -SH_C1 * y);
-        SHA(2, SH_C1 * z);
-        SHA(3, -SH_C1 * x);
-        if (deg > 1) {
-            const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-            SHA(4, b_SH_C2[0] * xy);
-            SHA(5, b_SH_C2[1] * yz);
-            SHA(6, b_SH_C2[2] * (2.f * zz - xx - yy));
-            SHA(7, b_SH_C2[3] * xz);
-            SHA(8, b_SH_C2[4] * (xx - yy));
-            if (deg > 2) {
-                SHA(9, b_SH_C3[0] * y * (3.f * xx - yy));
-                SHA(10, b_SH_C3[1] * xy * z);
-                SHA(11, b_SH_C3[2] * y * (4.f * zz - xx - yy));
-                SHA(12, b_SH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy));
-                SHA(13, b_SH_C3[4] * x * (4.f * zz - xx - yy));
-                SHA(14, b_SH_C3[5] * z * (xx - yy));
-                SHA(15, b_SH_C3[6] * x * (xx - 3.f * yy));
-            }
-        }
-    }
-#undef SHA
 }
 
 constexpr int PB_VB = 7;  // other views whose factors a thread fetches at the top of the kernel (8 ranks: all of them)
@@ -746,7 +655,7 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
                 if (g.x == 0.f && g.y == 0.f && g.z == 0.f) continue;  // not visible in that view (or past the last view)
                 const int uu = u0 + u, v = uu + (uu >= a.my_view ? 1 : 0);
                 const float *cp = a.view_tab[v] + a.campos_off;
-                sh_accumulate(a.v.D, oacc, {mx - __ldg(cp), my - __ldg(cp + 1), mz - __ldg(cp + 2)}, g);
+                sh_accumulate(a.v.D, oacc, sh_dir(mx, my, mz, __ldg(cp), __ldg(cp + 1), __ldg(cp + 2)), g);
             }
         }
     };
@@ -888,13 +797,14 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
             dmean.z += (proj[8] * m_w - proj[11] * mul1) * dmx + (proj[9] * m_w - proj[11] * mul2) * dmy;
             if (a.shs) {
                 const float *cp = a.v.campos;
-                const f3 dir_orig = {mx - cp[0], my - cp[1], mz - cp[2]};
+                // sh_dir's own subtractions, so the two share them (with a separate chain this kernel spills)
+                const f3 dir_orig = {__fsub_rn(mx, cp[0]), __fsub_rn(my, cp[1]), __fsub_rn(mz, cp[2])};
                 add_dnormvdv(dir_orig, ddir, dmean);
                 if (a.dsh) {
                     // accumulated dL/dRGB, already masked where the forward clamped the colour
                     const f3 dRGB = {sm[PB_DCOL + tid * 3], sm[PB_DCOL + tid * 3 + 1], sm[PB_DCOL + tid * 3 + 2]};
-                    sh_grad_row<MULTI>(a.v.D, M, RAW ? sm + PB_SHDC + tid * 3 : row, RAW ? row : row + 3, dir_orig, dRGB,
-                                       MULTI ? a.dsh_scale : 1.0f, oacc);
+                    sh_grad_row<MULTI>(a.v.D, M, RAW ? sm + PB_SHDC + tid * 3 : row, RAW ? row : row + 3,
+                                       sh_dir(mx, my, mz, cp[0], cp[1], cp[2]), dRGB, MULTI ? a.dsh_scale : 1.0f, oacc);
                 }
             }
             o_m3d[0] = dmean.x;
@@ -998,26 +908,11 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
     } else if (a.dsh && M > 0) {
         float *dst = a.dsh + (size_t)base * row_f;
         if (a.shs) {
-            if (a.sh_vec) {
-                const int row_v = row_f >> 2, total = n * row_v;
-                int r = tid / row_v, c = tid - r * row_v;
-                const int dr = PB_T / row_v, dc = PB_T - dr * row_v;
-                for (int k = tid; k < total; k += PB_T) {
-                    ((float4 *)dst)[k] = *(const float4 *)(s_sh + r * a.sh_stride + c * 4);
-                    r += dr;
-                    c += dc;
-                    if (c >= row_v) {
-                        c -= row_v;
-                        r++;
-                    }
-                }
-            } else {
-                const int total = n * row_f;
-                for (int k = tid; k < total; k += PB_T) {
-                    const int r = k / row_f, c = k - r * row_f;
-                    dst[k] = s_sh[r * a.sh_stride + c];
-                }
-            }
+            if (a.sh_vec)
+                sh_rows_walk<PB_T, 4>(n, row_f, a.sh_stride,
+                                      [&](int g, int s) { *(float4 *)(dst + g) = *(const float4 *)(s_sh + s); });
+            else
+                sh_rows_walk<PB_T, 1>(n, row_f, a.sh_stride, [&](int g, int s) { dst[g] = s_sh[s]; });
         } else {
             for (int k = tid; k < n * row_f; k += PB_T) dst[k] = 0.f;
         }
@@ -1107,6 +1002,7 @@ __global__ void __launch_bounds__(SF_T) view_grad_finalize_m16_kernel(int p0, in
         }
     }
     if (!dsh) return;
+    const int used = (deg + 1) * (deg + 1);
     float acc[4][3];
 #pragma unroll
     for (int k = 0; k < 4; k++) acc[k][0] = acc[k][1] = acc[k][2] = 0.f;
@@ -1128,38 +1024,19 @@ __global__ void __launch_bounds__(SF_T) view_grad_finalize_m16_kernel(int p0, in
             const float gr = gv[u][0] * scale, gg = gv[u][1] * scale, gb = gv[u][2] * scale;
             if (gr == 0.f && gg == 0.f && gb == 0.f) continue;  // not visible in this view (or past the last view)
             const float *cp = view_tab ? view_tab[v0 + u] + campos_off : campos + (size_t)(v0 + u) * campos_stride;
-            const float ox = mx - __ldg(cp), oy = my - __ldg(cp + 1), oz = mz - __ldg(cp + 2);
-            const float inv = 1.0f / sqrtf(ox * ox + oy * oy + oz * oz);
-            const float x = ox * inv, y = oy * inv, z = oz * inv;
-            const float xx = x * x, yy = y * y, zz = z * z;
-            float w[4] = {0.f, 0.f, 0.f, 0.f};
-            if (q == 0) {
-                w[0] = SH_C0;
-                if (deg > 0) {
-                    w[1] = -SH_C1 * y;
-                    w[2] = SH_C1 * z;
-                    w[3] = -SH_C1 * x;
-                }
-            } else if (q == 1) {
-                if (deg > 1) {
-                    w[0] = b_SH_C2[0] * x * y;
-                    w[1] = b_SH_C2[1] * y * z;
-                    w[2] = b_SH_C2[2] * (2.f * zz - xx - yy);
-                    w[3] = b_SH_C2[3] * x * z;
-                }
-            } else if (q == 2) {
-                if (deg > 1) w[0] = b_SH_C2[4] * (xx - yy);
-                if (deg > 2) {
-                    w[1] = b_SH_C3[0] * y * (3.f * xx - yy);
-                    w[2] = b_SH_C3[1] * x * y * z;
-                    w[3] = b_SH_C3[2] * y * (4.f * zz - xx - yy);
-                }
-            } else if (deg > 2) {
-                w[0] = b_SH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy);
-                w[1] = b_SH_C3[4] * x * (4.f * zz - xx - yy);
-                w[2] = b_SH_C3[5] * z * (xx - yy);
-                w[3] = b_SH_C3[6] * x * (xx - 3.f * yy);
-            }
+            const f3 d = sh_dir(mx, my, mz, __ldg(cp), __ldg(cp + 1), __ldg(cp + 2));
+            float w[4] = {0.f, 0.f, 0.f, 0.f};  // basis functions 4q .. 4q + 3, zero at and above (deg + 1)^2
+            auto quad = [&](auto q4) {
+                constexpr int K0 = 4 * decltype(q4)::value;
+                sh_for<K0, K0 + 4>([&](auto k) {
+                    constexpr int K = decltype(k)::value;
+                    if (K < used) w[K - K0] = sh_basis<K>(d);
+                });
+            };
+            if (q == 0) quad(std::integral_constant<int, 0>{});
+            else if (q == 1) quad(std::integral_constant<int, 1>{});
+            else if (q == 2) quad(std::integral_constant<int, 2>{});
+            else quad(std::integral_constant<int, 3>{});
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 acc[k][0] = fmaf(w[k], gr, acc[k][0]);
@@ -1209,10 +1086,11 @@ __global__ void __launch_bounds__(SFG_T) view_grad_finalize_kernel(int p0, int p
     }
     if (!dsh) return;
     const int row_f = M * 3;
-    const int stride = (row_f & 1) ? row_f : row_f + 1;  // odd stride: conflict-free scalar access
-    float acc[16][3];
+    int vec;
+    const int stride = sh_row_stride(M, false, &vec);
+    float acc[48];
 #pragma unroll
-    for (int k = 0; k < 16; k++) acc[k][0] = acc[k][1] = acc[k][2] = 0.f;
+    for (int k = 0; k < 48; k++) acc[k] = 0.f;
     if (tid < n) {
         const float mx = means[3 * (size_t)i], my = means[3 * (size_t)i + 1], mz = means[3 * (size_t)i + 2];
         for (int v = 0; v < nviews; v++) {
@@ -1220,58 +1098,17 @@ __global__ void __launch_bounds__(SFG_T) view_grad_finalize_kernel(int p0, int p
             const float gr = g[0] * scale, gg = g[1] * scale, gb = g[2] * scale;
             if (gr == 0.f && gg == 0.f && gb == 0.f) continue;  // not visible in this view
             const float *cp = view_tab ? view_tab[v] + campos_off : campos + (size_t)v * campos_stride;
-            const float ox = mx - cp[0], oy = my - cp[1], oz = mz - cp[2];
-            const float inv = 1.0f / sqrtf(ox * ox + oy * oy + oz * oz);
-            const float x = ox * inv, y = oy * inv, z = oz * inv;
-            float w[16];
-            w[0] = SH_C0;
-            if (deg > 0) {
-                w[1] = -SH_C1 * y;
-                w[2] = SH_C1 * z;
-                w[3] = -SH_C1 * x;
-                if (deg > 1) {
-                    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                    w[4] = b_SH_C2[0] * xy;
-                    w[5] = b_SH_C2[1] * yz;
-                    w[6] = b_SH_C2[2] * (2.f * zz - xx - yy);
-                    w[7] = b_SH_C2[3] * xz;
-                    w[8] = b_SH_C2[4] * (xx - yy);
-                    if (deg > 2) {
-                        w[9] = b_SH_C3[0] * y * (3.f * xx - yy);
-                        w[10] = b_SH_C3[1] * xy * z;
-                        w[11] = b_SH_C3[2] * y * (4.f * zz - xx - yy);
-                        w[12] = b_SH_C3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy);
-                        w[13] = b_SH_C3[4] * x * (4.f * zz - xx - yy);
-                        w[14] = b_SH_C3[5] * z * (xx - yy);
-                        w[15] = b_SH_C3[6] * x * (xx - 3.f * yy);
-                    }
-                }
-            }
-            const int used = (deg + 1) * (deg + 1);
-#pragma unroll
-            for (int k = 0; k < 16; k++)
-                if (k < used) {
-                    acc[k][0] = fmaf(w[k], gr, acc[k][0]);
-                    acc[k][1] = fmaf(w[k], gg, acc[k][1]);
-                    acc[k][2] = fmaf(w[k], gb, acc[k][2]);
-                }
+            sh_accumulate(deg, acc, sh_dir(mx, my, mz, cp[0], cp[1], cp[2]), {gr, gg, gb});
         }
         float *row = s_rows + tid * stride;
 #pragma unroll
-        for (int k = 0; k < 16; k++)
-            if (k < M) {
-                row[k * 3] = acc[k][0];
-                row[k * 3 + 1] = acc[k][1];
-                row[k * 3 + 2] = acc[k][2];
-            }
-        for (int k = 16; k < M; k++) row[k * 3] = row[k * 3 + 1] = row[k * 3 + 2] = 0.f;
+        for (int k = 0; k < 48; k++)
+            if (k < row_f) row[k] = acc[k];
+        for (int k = 48; k < row_f; k++) row[k] = 0.f;
     }
     __syncthreads();
     float *dst = dsh + (size_t)base * row_f;
-    for (int k = tid; k < n * row_f; k += SFG_T) {
-        const int r = k / row_f, c = k - r * row_f;
-        dst[k] = s_rows[r * stride + c];
-    }
+    sh_rows_walk<SFG_T, 1>(n, row_f, stride, [&](int g, int s) { dst[g] = s_rows[s]; });
 }
 
 static int finalize_impl(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree, int32_t num_views,
@@ -1604,8 +1441,8 @@ static int finalize_impl(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t s
                        p0, p1, sh_degree, num_views, means3D, campos, campos_stride, dRGB, (size_t)view_stride, view_tab,
                        campos_off, dL_dsh, reduced_records, scale, dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations));
     } else {
-        const int row_f = M * 3, stride = (row_f & 1) ? row_f : row_f + 1;
-        const size_t dyn = sh ? (size_t)SFG_T * stride * sizeof(float) : 0;
+        int vec;
+        const size_t dyn = sh ? (size_t)SFG_T * sh_row_stride(M, false, &vec) * sizeof(float) : 0;
         SGR_LAUNCH(K_FINALIZE, st,
                    view_grad_finalize_kernel<<<(p1 - p0 + SFG_T - 1) / SFG_T, SFG_T, dyn, st>>>(
                        p0, p1, P, M, sh_degree, num_views, means3D, campos, campos_stride, dRGB, (size_t)view_stride,

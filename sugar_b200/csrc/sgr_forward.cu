@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "sgr_internal.cuh"
+#include "sgr_sh.cuh"
 
 namespace sgr {
 
@@ -46,86 +47,6 @@ struct PreArgs {
     int32_t *radii;
     uint32_t *tile_count;
 };
-
-__constant__ float c_SH_C2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
-                                 -1.0925484305920792f, 0.5462742152960396f};
-__constant__ float c_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
-                                 0.3731763325901154f, -0.4570457994644658f, 1.445305721320277f,
-                                 -0.5900435899266435f};
-#define SH_C0 0.28209479177387814f
-#define SH_C1 0.4886025119029199f
-
-// SH -> RGB for one channel (forward.cu:20-71), operation order as compiled for the reference.
-// `dc` points at coefficient 0 of the channel, `rest` at coefficient 1 (stride 3 floats); for one combined row
-// [M][3] rest = dc + 3, in raw-parameter mode they live in two arrays.
-__device__ __forceinline__ float sh_channel(int deg, const float *dc, const float *rest, float x, float y, float z)
-{
-#define SHK(k) ((k) == 0 ? dc[0] : rest[((k) - 1) * 3])
-    float res = __fmul_rn(SH_C0, SHK(0));
-    if (deg > 0) {
-        res = __fmaf_rn(-__fmul_rn(y, SH_C1), SHK(1), res);
-        res = __fmaf_rn(__fmul_rn(z, SH_C1), SHK(2), res);
-        res = __fmaf_rn(-__fmul_rn(x, SH_C1), SHK(3), res);
-        if (deg > 1) {
-            const float xx = __fmul_rn(x, x), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
-            const float xy = __fmul_rn(x, y), yz = __fmul_rn(y, z), xz = __fmul_rn(x, z);
-            const float zz2 = __fadd_rn(zz, zz);
-            const float xx_yy = __fsub_rn(xx, yy);
-            res = __fmaf_rn(__fmul_rn(xy, c_SH_C2[0]), SHK(4), res);
-            res = __fmaf_rn(__fmul_rn(yz, c_SH_C2[1]), SHK(5), res);
-            res = __fmaf_rn(__fmul_rn(__fsub_rn(__fsub_rn(zz2, xx), yy), c_SH_C2[2]), SHK(6), res);
-            res = __fmaf_rn(__fmul_rn(xz, c_SH_C2[3]), SHK(7), res);
-            res = __fmaf_rn(__fmul_rn(xx_yy, c_SH_C2[4]), SHK(8), res);
-            if (deg > 2) {
-                const float zz4_xx_yy = __fsub_rn(__fmaf_rn(zz, 4.0f, -xx), yy);
-                res = __fmaf_rn(__fmul_rn(__fmul_rn(y, c_SH_C3[0]), __fmaf_rn(xx, 3.0f, -yy)), SHK(9), res);
-                res = __fmaf_rn(__fmul_rn(__fmul_rn(xy, c_SH_C3[1]), z), SHK(10), res);
-                res = __fmaf_rn(__fmul_rn(__fmul_rn(y, c_SH_C3[2]), zz4_xx_yy), SHK(11), res);
-                res = __fmaf_rn(__fmul_rn(__fmul_rn(z, c_SH_C3[3]), __fmaf_rn(yy, -3.0f, __fmaf_rn(xx, -3.0f, zz2))),
-                                SHK(12), res);
-                res = __fmaf_rn(__fmul_rn(__fmul_rn(x, c_SH_C3[4]), zz4_xx_yy), SHK(13), res);
-                res = __fmaf_rn(__fmul_rn(__fmul_rn(z, c_SH_C3[5]), xx_yy), SHK(14), res);
-                res = __fmaf_rn(__fmul_rn(__fmul_rn(x, c_SH_C3[6]), __fmaf_rn(yy, -3.0f, xx)), SHK(15), res);
-            }
-        }
-    }
-#undef SHK
-    return res;
-}
-
-// dRGB/d(dir) for one channel: the three sums dRGBdx, dRGBdy, dRGBdz of backward.cu:36-128 (same terms, same
-// grouping), from the coefficients sh_channel has just read.  `rest` points at coefficient 1 of the channel.
-// The backward's view-direction term of dL/dmean3D is their dot product with dL/dRGB, so it needs these nine
-// numbers per Gaussian instead of the whole SH row.
-__device__ __forceinline__ void sh_channel_jacobian(int deg, const float *rest, float x, float y, float z, float &jx,
-                                                    float &jy, float &jz)
-{
-#define SHK(k) rest[((k) - 1) * 3]
-    jx = -SH_C1 * SHK(3);
-    jy = -SH_C1 * SHK(1);
-    jz = SH_C1 * SHK(2);
-    if (deg > 1) {
-        const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-        jx += c_SH_C2[0] * y * SHK(4) + c_SH_C2[2] * 2.f * -x * SHK(6) + c_SH_C2[3] * z * SHK(7) +
-              c_SH_C2[4] * 2.f * x * SHK(8);
-        jy += c_SH_C2[0] * x * SHK(4) + c_SH_C2[1] * z * SHK(5) + c_SH_C2[2] * 2.f * -y * SHK(6) +
-              c_SH_C2[4] * 2.f * -y * SHK(8);
-        jz += c_SH_C2[1] * y * SHK(5) + c_SH_C2[2] * 2.f * 2.f * z * SHK(6) + c_SH_C2[3] * x * SHK(7);
-        if (deg > 2) {
-            jx += c_SH_C3[0] * SHK(9) * 3.f * 2.f * xy + c_SH_C3[1] * SHK(10) * yz + c_SH_C3[2] * SHK(11) * -2.f * xy +
-                  c_SH_C3[3] * SHK(12) * -3.f * 2.f * xz + c_SH_C3[4] * SHK(13) * (-3.f * xx + 4.f * zz - yy) +
-                  c_SH_C3[5] * SHK(14) * 2.f * xz + c_SH_C3[6] * SHK(15) * 3.f * (xx - yy);
-            jy += c_SH_C3[0] * SHK(9) * 3.f * (xx - yy) + c_SH_C3[1] * SHK(10) * xz +
-                  c_SH_C3[2] * SHK(11) * (-3.f * yy + 4.f * zz - xx) + c_SH_C3[3] * SHK(12) * -3.f * 2.f * yz +
-                  c_SH_C3[4] * SHK(13) * -2.f * xy + c_SH_C3[5] * SHK(14) * -2.f * yz +
-                  c_SH_C3[6] * SHK(15) * -3.f * 2.f * xy;
-            jz += c_SH_C3[1] * SHK(10) * xy + c_SH_C3[2] * SHK(11) * 4.f * 2.f * yz +
-                  c_SH_C3[3] * SHK(12) * 3.f * (2.f * zz - xx - yy) + c_SH_C3[4] * SHK(13) * 4.f * 2.f * xz +
-                  c_SH_C3[5] * SHK(14) * (xx - yy);
-        }
-    }
-#undef SHK
-}
 
 // Cooperative, coalesced copy of n floats into shared memory (fallback when bulk copy is not legal).
 __device__ __forceinline__ void stage_plain(float *dst, const float *__restrict__ src, int n)
@@ -202,26 +123,8 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
     if (!RAW && a.shs) {
         const int row_f = a.v.M * 3;
         const float *src = a.shs + (size_t)base * row_f;
-        if (a.sh_vec) {
-            const int row_v = row_f >> 2, total = n * row_v;
-            int r = tid / row_v, c = tid - r * row_v;  // (row, 16-byte column) advanced without divisions
-            const int dr = PRE_T / row_v, dc = PRE_T - dr * row_v;
-            for (int i = tid; i < total; i += PRE_T) {
-                cp_async16(s_sh + r * a.sh_stride + c * 4, src + (size_t)i * 4);
-                r += dr;
-                c += dc;
-                if (c >= row_v) {
-                    c -= row_v;
-                    r++;
-                }
-            }
-        } else {
-            const int total = n * row_f;
-            for (int i = tid; i < total; i += PRE_T) {
-                const int r = i / row_f, c = i - r * row_f;
-                cp_async4(s_sh + r * a.sh_stride + c, src + i);
-            }
-        }
+        if (a.sh_vec) sh_rows_walk<PRE_T, 4>(n, row_f, a.sh_stride, [&](int g, int s) { cp_async16(s_sh + s, src + g); });
+        else sh_rows_walk<PRE_T, 1>(n, row_f, a.sh_stride, [&](int g, int s) { cp_async4(s_sh + s, src + g); });
         cp_async_commit();
     }
     __syncthreads();  // barrier init visible / plain staging complete
@@ -295,9 +198,7 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
                 r = s_col[tid * 3], g = s_col[tid * 3 + 1], b = s_col[tid * 3 + 2];
             } else {
                 const float *cp = a.v.campos;
-                const float dx = __fsub_rn(mx, cp[0]), dy = __fsub_rn(my, cp[1]), dz = __fsub_rn(mz, cp[2]);
-                const float len = __fsqrt_rn(__fmaf_rn(dz, dz, __fmaf_rn(dx, dx, __fmul_rn(dy, dy))));
-                const float x = __fdiv_rn(dx, len), y = __fdiv_rn(dy, len), z = __fdiv_rn(dz, len);
+                const f3 d = sh_dir(mx, my, mz, cp[0], cp[1], cp[2]);
                 const float *dc, *rest;
                 if (RAW) {
                     dc = s_col + tid * 3;
@@ -306,12 +207,13 @@ __global__ void __launch_bounds__(PRE_T) preprocess_kernel(const PreArgs a)
                     dc = s_sh + tid * a.sh_stride;
                     rest = dc + 3;
                 }
-                r = sh_channel(a.v.D, dc + 0, rest + 0, x, y, z);
-                g = sh_channel(a.v.D, dc + 1, rest + 1, x, y, z);
-                b = sh_channel(a.v.D, dc + 2, rest + 2, x, y, z);
+                auto channel = [&](int c) {
+                    return sh_channel(a.v.D, d, [&](int k) { return k == 0 ? dc[c] : rest[(k - 1) * 3 + c]; });
+                };
+                r = channel(0), g = channel(1), b = channel(2);
                 if (a.v.D > 0) {
 #pragma unroll
-                    for (int c = 0; c < 3; c++) sh_channel_jacobian(a.v.D, rest + c, x, y, z, jac[c], jac[3 + c], jac[6 + c]);
+                    for (int c = 0; c < 3; c++) sh_channel_jacobian(a.v.D, rest + c, d.x, d.y, d.z, jac[c], jac[3 + c], jac[6 + c]);
                 }
                 // clamped <=> result + 0.5 < 0 (forward.cu:63-70)
                 clamp_bits = (r < -0.5f ? 1u : 0u) | (g < -0.5f ? 2u : 0u) | (b < -0.5f ? 4u : 0u);

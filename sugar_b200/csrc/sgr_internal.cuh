@@ -152,21 +152,6 @@ static inline ViewConsts view_consts(const SgrView *view, int M)
 
 static inline bool aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
 
-// Row stride in floats of the per-Gaussian passes' shared-memory SH rows (M coefficients x 3): an odd number of
-// 16-byte units when the rows can move as 16-byte copies (`vec_ok`: the global rows are 16-byte aligned), else an
-// odd number of floats -- conflict-free either way.  *vec = 1 selects the 16-byte copies.
-static inline int sh_row_stride(int M, bool vec_ok, int *vec)
-{
-    const int row_f = M * 3;
-    *vec = (row_f % 4) == 0 && vec_ok;
-    if (*vec) {
-        int s4 = row_f / 4;
-        if ((s4 & 1) == 0) s4 += 1;
-        return s4 * 4;
-    }
-    return (row_f & 1) ? row_f : row_f + 1;
-}
-
 void set_error(const char *fmt, ...);
 int cuda_fail(cudaError_t e, const char *what);
 int device_sm_count();  // SMs of the current device (grid sizes of the grid-stride kernels)

@@ -30,11 +30,11 @@
 #include <math.h>
 
 #include "sgr_internal.cuh"
+#include "sgr_sh.cuh"
 
 namespace sgr {
 
 constexpr int TEX_THREADS = 256;
-constexpr float SH_C0 = 0.28209479177387814f;
 
 __device__ __forceinline__ float fmul(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b); }

@@ -153,14 +153,15 @@ def test_sh_factors_rebuild_the_summed_dsh_with_nine_stored_coefficients():
 def check_sh_factors_rebuild(M, deg):
     """sgr_sh_grad_from_factors on the gathered factors of several views == the sum of the views' dL_dsh; the
     factor of a view is the dL_dcolors the backward returns with SH colours (clamp-masked dL/dRGB).  Also against
-    sum_v basis(normalize(mean - campos_v)) (x) factor_v evaluated in float64."""
+    sum_v basis(normalize(mean - campos_v)) (x) factor_v evaluated in float64.  On one view's factor alone it gives
+    that view's dL_dsh exactly: the backward and the factor kernels evaluate the same basis at the same direction."""
     import torch
     from sugar_b200 import _C, parallel, scenes
     P, W, H = 6000, 160, 96
     base = scenes.make_scene(P, W, H, seed=34, camera="posed")
     views = [base, scenes.with_camera_offset(base, 0.15, (0.3, -0.1, 0.2)),
              scenes.with_camera_offset(base, -0.2, (-0.4, 0.2, 0.5))]
-    want, factors, campos = None, [], []
+    want, factors, campos, dsh = None, [], [], []
     E = torch.Tensor([])
     for v, sc in enumerate(views):
         t = h.to_torch(sc)
@@ -175,6 +176,7 @@ def check_sh_factors_rebuild(M, deg):
                                             t["campos"], geom, R, binning, img, False)
         factors.append(g[1].clone())
         campos.append(t["campos"].clone())
+        dsh.append(g[5].clone())
         want = g[5].double() if want is None else want + g[5].double()
     means = torch.from_numpy(base.means3D).cuda()
     got = parallel.sh_grad_from_factors(means, torch.stack(campos).contiguous(), torch.stack(factors).contiguous(), M, deg)
@@ -186,6 +188,9 @@ def check_sh_factors_rebuild(M, deg):
         d /= np.linalg.norm(d, axis=1, keepdims=True)
         exact = exact + h.sh_basis(d, deg)[:, :M, None] * f.cpu().numpy().astype(np.float64)[:, None, :]
     assert h.rel_err(got.cpu().numpy(), exact) <= 1e-5
+    for f, cp, dsh_v in zip(factors, campos, dsh):
+        one = parallel.sh_grad_from_factors(means, cp[None].contiguous(), f[None].contiguous(), M, deg)
+        assert torch.equal(one, dsh_v)                 # ==, so +0 and -0 match
     used = (deg + 1) ** 2
     if used < M:
         assert float(got[:, used:].abs().max()) == 0.0 and float(want[:, used:].abs().max()) == 0.0
