@@ -560,6 +560,46 @@ SGR_API int sgr_mcubes_emit(int32_t Rx, int32_t Ry, int32_t Rz, const float *vol
                             int64_t n_faces, float *verts, int64_t *faces, void *scratch, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Screened-Poisson reconstruction on a dense grid (sugar_b200/poisson.py states the discrete problem; restated in
+ * oracle/poisson_oracle.py).  A grid is f32[N,N,N] in C order with N = 2^depth; a sample's grid coordinates are
+ * g = (p - o) * inv_h - 0.5 in float32.  Every grid and buffer is caller-allocated; no float atomics, so every output
+ * is identical from run to run.  One stream; the calls that return a host value synchronise it once.
+ * sgr_poisson_bin: each sample goes to the bin of its hat support's lower corner clamp(floor(g), 0, N - 2), bin b
+ *   holding binned[starts[b] .. starts[b+1]) (the last bin ending at n) in sample order, each record (gx, gy, gz,
+ *   sample id bits), by a stable radix sort.  points f32[n,3], starts u32[N^3], binned f32[n,4]; scratch: keys u32[2n],
+ *   records f32[n,4] (binned and records 16-byte aligned), hist u32[256 T] with T = ceil(n / 256), block_sums
+ *   u32[(max(N^3, 256 T) + 4095) / 4096 + 1]; n_occupied (host) <- the number of non-empty bins.
+ * sgr_poisson_splat: every node gathers from its 8 neighbouring bins (increasing bin index, then sample order):
+ *   (starts as sgr_poisson_bin wrote them)
+ *   mode 0 out0 = -area * sum_s normals[s] . grad phi(g_s), out1 = alpha * area * sum_s phi(g_s) (attr = normals f32[n,3]);
+ *   mode 1 out0 = sum_s phi(g_s); mode 2 out0 = sum_s phi(g_s) attr[s, channel] (attr f32[n,3]).  Outputs f32[N^3].
+ * sgr_poisson_coarsen: coarse[I] = the sum of the 8 children of I in fine f32[N^3]; coarse f32[(N/2)^3], N >= 8.
+ * sgr_poisson_residual_norm: norm (host) <- |b - A u|_2 for A = coeff * (7-point Neumann stencil) + diag(q);
+ *   u == NULL gives |b|_2.  partial f64[1024].
+ * sgr_poisson_vcycle: one V(2,2) cycle over levels l = 0 .. depth - 2 (side 2^depth >> l, stencil coefficient 2^l):
+ *   u, b, q are HOST arrays of depth - 1 device grids; u[0], b[0], q[0] the system, q[l > 0] its sgr_poisson_coarsen
+ *   pyramid; u[l > 0] and b[l > 0] are scratch.  norm (host) <- the fine residual norm after the cycle.
+ * sgr_poisson_interpolate: values[s] = trilinear interpolation of grid f32[N^3] at g = points[s * stride + a] * scale
+ *   + offset (clamped to the grid); with sum != NULL, sum (host) <- the sum of the values (partial f64[1024]).
+ *   values may be NULL when sum is given.
+ *   Limits: n > 0, N a power of two in [4, 1024], 3 <= depth <= 10.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API int sgr_poisson_bin(int32_t n, const float *points, int32_t N, float ox, float oy, float oz, float inv_h,
+                            uint32_t *starts, float *binned, uint32_t *keys, float *records, uint32_t *hist,
+                            uint32_t *block_sums, int64_t *n_occupied, void *stream);
+SGR_API int sgr_poisson_splat(int32_t N, int32_t n, const uint32_t *starts, const float *binned, int32_t mode,
+                              const float *attr, int32_t channel, float area, float alpha, float *out0, float *out1,
+                              void *stream);
+SGR_API int sgr_poisson_coarsen(int32_t N, const float *fine, float *coarse, void *stream);
+SGR_API int sgr_poisson_residual_norm(int32_t N, float coeff, const float *u, const float *b, const float *q,
+                                      double *partial, double *norm, void *stream);
+SGR_API int sgr_poisson_vcycle(int32_t depth, float *const *u, float *const *b, const float *const *q, double *partial,
+                               double *norm, void *stream);
+SGR_API int sgr_poisson_interpolate(int32_t N, const float *grid, int64_t m, const float *points, int32_t stride,
+                                    float scale, float offset, float *values, double *partial, double *sum,
+                                    void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Quadric edge-collapse decimation (open3d's simplify_quadric_decimation with maximum_error = inf and
  * boundary_weight = 1, as coarse_mesh.py:433-463 and :716-744 call it), restated in oracle/decimate_oracle.py:
  * rounds of independent collapses until the face count is at most `target` or no edge can be collapsed.  The

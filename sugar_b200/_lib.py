@@ -143,6 +143,14 @@ PROTOTYPES = {
     "sgr_mcubes_scratch_bytes": (C.c_size_t, [C.c_int32] * 3),
     "sgr_mcubes_count": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double] + [C.c_void_p] * 4),
     "sgr_mcubes_emit": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double, C.c_int64, C.c_int64] + [C.c_void_p] * 4),
+    "sgr_poisson_bin": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32] + [C.c_float] * 4 + [C.c_void_p] * 8),
+    "sgr_poisson_splat": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                    C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sgr_poisson_coarsen": (C.c_int, [C.c_int32] + [C.c_void_p] * 3),
+    "sgr_poisson_residual_norm": (C.c_int, [C.c_int32, C.c_float] + [C.c_void_p] * 6),
+    "sgr_poisson_vcycle": (C.c_int, [C.c_int32] + [C.c_void_p] * 6),
+    "sgr_poisson_interpolate": (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_float] +
+                                [C.c_void_p] * 4),
     "sgr_decimate_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "sgr_decimate": (C.c_int, [C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 11),
     "sgr_densify_stats": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 6),
