@@ -417,6 +417,29 @@ SGR_API int sgr_meshbind_backward(int32_t F, int32_t n_per, int32_t V, const flo
                                   const float *g_points, const float *g_scaling, const float *g_quaternions,
                                   float *g_verts, float *g_scales_raw, float *g_complex_raw, void *stream);
 
+/* The editable bound model (make_editable / get_edited_quaternions_and_scales, sugar_model.py:562-667, and the
+ * `scaling` / `quaternions` properties with editable set), forward only: the forward above at the current `verts`,
+ * with each Gaussian's in-plane rotation turned by the bary-weighted change in angle of its face's vertex axes and
+ * each plane scale multiplied by the bary-weighted stretch of those axes, both measured against `reference_verts`
+ * f32[V,3] (the vertices make_editable snapshotted).  out_rows NULL: Gaussian g goes to row g of points / scaling /
+ * quaternions; else to row out_rows[g] (i64[P]), and a negative entry skips it. */
+SGR_API int sgr_meshbind_edited_forward(int32_t F, int32_t n_per, int32_t V, const float *verts,
+                                        const float *reference_verts, const int64_t *faces, const float *bary,
+                                        const float *scales_raw, const float *complex_raw, float thickness,
+                                        const int64_t *out_rows, float *points, float *scaling, float *quats,
+                                        void *stream);
+
+/* ------------------------------------------------------------------------------------------
+ * SH colours at a rotated view direction (SuGaRCompositor's sh_rotations, sugar_compositor.py:139-151):
+ * colors[i] = max(eval_sh(normalize(means[i] - campos) @ R_g) + 0.5, 0) per channel, in the rasterizer's own basis
+ * and rounding (at R = I the forward's in-kernel colour, to the bit).  Rows group_start[g] .. group_start[g+1] - 1
+ * (i64[G+1], group_start[0] = 0, group_start[G] = P) take group_rot[g] (f32[G,9], row-major 3x3).
+ *   means f32[P,3], shs f32[P,M,3] with (sh_degree + 1)^2 <= M, campos f32[3], colors f32[P,3].  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API int sgr_sh_colors_rotated(int32_t P, int32_t M, int32_t sh_degree, const float *means, const float *shs,
+                                  const float *campos, int32_t G, const int64_t *group_start, const float *group_rot,
+                                  float *colors, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Exact K-nearest-neighbour search (uniform grid).  Replaces pytorch3d.ops.knn_points as SuGaR
  * calls it: reset_neighbors (sugar_model.py:1013-1030, queries == points, K = 16) and

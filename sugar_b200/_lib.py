@@ -120,6 +120,8 @@ PROTOTYPES = {
     "sgr_density_estimation_backward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 15),
     "sgr_meshbind_forward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 5 + [C.c_float] + [C.c_void_p] * 4),
     "sgr_meshbind_backward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 12),
+    "sgr_meshbind_edited_forward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 6 + [C.c_float] + [C.c_void_p] * 5),
+    "sgr_sh_colors_rotated": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 4),
     "sgr_knn_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_knn": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                           C.c_void_p]),

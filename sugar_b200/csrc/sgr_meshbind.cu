@@ -9,6 +9,8 @@
 // step.  One thread per FACE: the frame is built once and shared by the face's n Gaussians; in the backward
 // the face's Gaussians are folded into the frame's adjoint first, so a face issues 9 atomics to its three
 // vertices instead of 9 per Gaussian.
+// The edited model (make_editable, get_edited_quaternions_and_scales :562-667) is a forward-only kernel of its own on
+// the same frame: render-time arithmetic for a deformed or animated mesh.
 //
 // Third-party arithmetic restated from pytorch3d 0.7.4 (not under /root/reference):
 //   Meshes.faces_normals_packed : n = (v1 - v0) x (v2 - v0), n / max(|n|, 1e-6)
@@ -164,6 +166,101 @@ SGR_HD void meshbind_face_forward(int f, int n_per, const float *__restrict__ ve
     }
 }
 
+// y = x / max(|x|, eps), divided as F.normalize divides (the edited binding's vertex axes)
+SGR_HD V3 normalize_div(V3 x, float eps, float &len)
+{
+    len = sqrtf(dot(x, x));
+    const float d = fmaxf(len, eps);
+    return {x.x / d, x.y / d, x.z / d};
+}
+
+// The face's vertex axes normalize(mean - v_k) and their lengths (sugar_model.py:636-642).  The angle axes of :598-603,
+// normalize(v_k - mean) with the third one negated, are (-A_0, -A_1, A_2) exactly: negation commutes with every rounding.
+SGR_HD void vertex_axes(V3 v0, V3 v1, V3 v2, V3 A[3], float len[3])
+{
+    const V3 s = (v0 + v1) + v2, m = {s.x / 3.0f, s.y / 3.0f, s.z / 3.0f};
+    A[0] = normalize_div(m - v0, 1e-12f, len[0]);
+    A[1] = normalize_div(m - v1, 1e-12f, len[1]);
+    A[2] = normalize_div(m - v2, 1e-12f, len[2]);
+}
+
+// arccos(clamp(<angle axis k, base>, -1, 1)) for the three axes (:606-607)
+SGR_HD void axis_angles(const V3 A[3], V3 base, float ang[3])
+{
+    const float sg[3] = {-1.f, -1.f, 1.f};
+#pragma unroll
+    for (int k = 0; k < 3; k++) ang[k] = acosf(fminf(fmaxf(sg[k] * dot(A[k], base), -1.f), 1.f));
+}
+
+// The edited model's Gaussians of face f (get_edited_quaternions_and_scales, sugar_model.py:572-667, with the
+// `quaternions` / `scaling` properties' final normalize and plane-scale product): the face frame of bind_to_mesh at the
+// current vertices, each Gaussian's learned in-plane rotation turned by the bary-weighted change of the vertex-axis
+// angles, and each plane scale stretched by the bary-weighted change of the axis lengths, both against the reference
+// vertices.  Gaussian g is written to row out_rows[g] (skipped when negative), or to row g - row0 when out_rows is NULL.
+SGR_HD void meshbind_face_edited_forward(int f, int n_per, const float *__restrict__ verts,
+                                         const float *__restrict__ reference_verts, const int64_t *__restrict__ faces,
+                                         const float *__restrict__ bary, const float *__restrict__ scales_raw,
+                                         const float *__restrict__ complex_raw, float thickness,
+                                         const int64_t *__restrict__ out_rows, int64_t row0, float *__restrict__ points,
+                                         float *__restrict__ scaling, float *__restrict__ quats)
+{
+    const Frame fr = face_frame(verts, faces, f);
+    const V3 r0 = ld3(reference_verts + 3 * faces[3 * (size_t)f]), r1 = ld3(reference_verts + 3 * faces[3 * (size_t)f + 1]),
+             r2 = ld3(reference_verts + 3 * faces[3 * (size_t)f + 2]);
+    V3 A[3], RA[3];
+    float len[3], rlen[3], ang[3], rang[3], blen;
+    vertex_axes(fr.v0, fr.v1, fr.v2, A, len);
+    vertex_axes(r0, r1, r2, RA, rlen);
+    axis_angles(A, fr.R1b, ang);                                   // faces_base is bind_to_mesh's base_R_1
+    axis_angles(RA, normalize_eps(r0 - r1, 1e-12f, blen), rang);   // the same normalize: equal vertices, equal angles
+    float dang[3];
+    V3 O[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        dang[k] = ang[k] - rang[k];
+        O[k] = cross(A[k], fr.fn);                                 // :639, against the pytorch3d face normal
+    }
+    for (int n = 0; n < n_per; n++) {
+        const size_t g = (size_t)f * n_per + n;
+        const int64_t row = out_rows ? out_rows[g] : (int64_t)g - row0;
+        if (row < 0) continue;
+        const float b0 = bary[3 * n], b1 = bary[3 * n + 1], b2 = bary[3 * n + 2];
+        const V3 p = (b0 * fr.v0 + b1 * fr.v1) + b2 * fr.v2;
+        points[3 * row] = p.x;
+        points[3 * row + 1] = p.y;
+        points[3 * row + 2] = p.z;
+        // the learned complex number turned by the point's angle (:608-621)
+        const float pa = (dang[0] * b0 + dang[1] * b1) + dang[2] * b2;
+        float sa, ca;
+        sincosf(pa, &sa, &ca);
+        const float cr = complex_raw[2 * g], ci = complex_raw[2 * g + 1];
+        const float cl = 1.0f / fmaxf(sqrtf(cr * cr + ci * ci), 1e-12f);
+        const float x = cr * cl, y = ci * cl;
+        const float zr = x * ca - y * sa, zi = x * sa + y * ca;
+        const V3 R1 = zr * fr.R1b + zi * fr.R2b, R2 = (-zi) * fr.R1b + zr * fr.R2b;
+        float q[4], s;
+        int k;
+        mat2quat(fr.R0, R1, R2, q, k, s);
+        const float ql = 1.0f / fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
+        quats[4 * row] = q[0] * ql;
+        quats[4 * row + 1] = q[1] * ql;
+        quats[4 * row + 2] = q[2] * ql;
+        quats[4 * row + 3] = q[3] * ql;
+        // stretch of each in-plane axis along the vertex axes (:644-660)
+        float st1[3], st2[3];
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            const float a1 = dot(R1, A[j]) * len[j] / rlen[j], o1 = dot(R1, O[j]);
+            const float a2 = dot(R2, A[j]) * len[j] / rlen[j], o2 = dot(R2, O[j]);
+            st1[j] = sqrtf(a1 * a1 + o1 * o1);
+            st2[j] = sqrtf(a2 * a2 + o2 * o2);
+        }
+        scaling[3 * row] = thickness;
+        scaling[3 * row + 1] = expf(scales_raw[2 * g]) * ((st1[0] * b0 + st1[1] * b1) + st1[2] * b2);
+        scaling[3 * row + 2] = expf(scales_raw[2 * g + 1]) * ((st2[0] * b0 + st2[1] * b1) + st2[2] * b2);
+    }
+}
+
 SGR_HD void vadd(float *p, float v)
 {
 #ifdef __CUDA_ARCH__
@@ -260,6 +357,40 @@ __global__ void __launch_bounds__(128) meshbind_forward_kernel(int F, int n_per,
     if (f < F) meshbind_face_forward(f, n_per, verts, faces, bary, scales_raw, complex_raw, thickness, points, scaling, quats);
 }
 
+// Without out_rows a CTA's Gaussians are one contiguous run of rows: they are staged in shared memory (10 floats each)
+// and leave in coalesced stores.  Stored straight from each thread, n_per > 1 rows per thread put every store
+// instruction on 32 separate sectors (4x slower at n_per = 6, measured).  out_rows scatters anyway and stores directly.
+constexpr int EDIT_T = 128;
+constexpr int EDIT_STAGE_MAX_N = 9;   // 128 faces x 9 Gaussians x 40 B = 45 KB of shared memory
+
+__global__ void __launch_bounds__(EDIT_T) meshbind_edited_forward_kernel(
+    int F, int n_per, const float *__restrict__ verts, const float *__restrict__ reference_verts,
+    const int64_t *__restrict__ faces, const float *__restrict__ bary, const float *__restrict__ scales_raw,
+    const float *__restrict__ complex_raw, float thickness, const int64_t *__restrict__ out_rows, int staged,
+    float *__restrict__ points, float *__restrict__ scaling, float *__restrict__ quats)
+{
+    const int f = blockIdx.x * EDIT_T + threadIdx.x;
+    if (!staged) {
+        if (f < F)
+            meshbind_face_edited_forward(f, n_per, verts, reference_verts, faces, bary, scales_raw, complex_raw,
+                                         thickness, out_rows, 0, points, scaling, quats);
+        return;
+    }
+    extern __shared__ float s_rows[];
+    float *sp = s_rows, *ss = sp + 3 * EDIT_T * n_per, *sq = ss + 3 * EDIT_T * n_per;
+    const int64_t g0 = (int64_t)blockIdx.x * EDIT_T * n_per;
+    const int cnt = min(EDIT_T, F - (int)(blockIdx.x * EDIT_T)) * n_per;
+    if (f < F)
+        meshbind_face_edited_forward(f, n_per, verts, reference_verts, faces, bary, scales_raw, complex_raw, thickness,
+                                     nullptr, g0, sp, ss, sq);
+    __syncthreads();
+    for (int i = threadIdx.x; i < 3 * cnt; i += EDIT_T) {
+        points[3 * g0 + i] = sp[i];
+        scaling[3 * g0 + i] = ss[i];
+    }
+    for (int i = threadIdx.x; i < 4 * cnt; i += EDIT_T) quats[4 * g0 + i] = sq[i];
+}
+
 __global__ void __launch_bounds__(128) meshbind_backward_kernel(int F, int n_per, const float *__restrict__ verts,
                                                                 const int64_t *__restrict__ faces,
                                                                 const float *__restrict__ bary,
@@ -299,6 +430,15 @@ extern "C" void meshbind_host_backward(int F, int n_per, const float *verts, con
         meshbind_face_backward(f, n_per, verts, faces, bary, scales_raw, complex_raw, g_points, g_scaling, g_quats, g_verts,
                                g_scales_raw, g_complex_raw);
 }
+extern "C" void meshbind_host_edited_forward(int F, int n_per, const float *verts, const float *reference_verts,
+                                             const int64_t *faces, const float *bary, const float *scales_raw,
+                                             const float *complex_raw, float thickness, const int64_t *out_rows,
+                                             float *points, float *scaling, float *quats)
+{
+    for (int f = 0; f < F; f++)
+        meshbind_face_edited_forward(f, n_per, verts, reference_verts, faces, bary, scales_raw, complex_raw, thickness,
+                                     out_rows, 0, points, scaling, quats);
+}
 #else
 extern "C" int sgr_meshbind_forward(int32_t F, int32_t n_per, int32_t V, const float *verts, const int64_t *faces,
                                     const float *bary, const float *scales_raw, const float *complex_raw, float thickness,
@@ -314,6 +454,30 @@ extern "C" int sgr_meshbind_forward(int32_t F, int32_t n_per, int32_t V, const f
     SGR_LAUNCH(K_MISC, st,
                meshbind_forward_kernel<<<(F + 127) / 128, 128, 0, st>>>(F, n_per, verts, faces, bary, scales_raw, complex_raw,
                                                                        thickness, points, scaling, quaternions));
+    SGR_CUDA(cudaGetLastError());
+    return SGR_OK;
+}
+
+extern "C" int sgr_meshbind_edited_forward(int32_t F, int32_t n_per, int32_t V, const float *verts,
+                                           const float *reference_verts, const int64_t *faces, const float *bary,
+                                           const float *scales_raw, const float *complex_raw, float thickness,
+                                           const int64_t *out_rows, float *points, float *scaling, float *quaternions,
+                                           void *stream)
+{
+    if (F < 0 || n_per <= 0 || V < 0 ||
+        (F > 0 && (!verts || !reference_verts || !faces || !bary || !scales_raw || !complex_raw || !points || !scaling ||
+                   !quaternions))) {
+        set_error("bad arguments to sgr_meshbind_edited_forward");
+        return SGR_EINVAL;
+    }
+    if (F == 0) return SGR_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int staged = !out_rows && n_per <= EDIT_STAGE_MAX_N;
+    const size_t smem = staged ? sizeof(float) * 10 * EDIT_T * n_per : 0;
+    SGR_LAUNCH(K_MISC, st,
+               meshbind_edited_forward_kernel<<<(F + EDIT_T - 1) / EDIT_T, EDIT_T, smem, st>>>(
+                   F, n_per, verts, reference_verts, faces, bary, scales_raw, complex_raw, thickness, out_rows, staged,
+                   points, scaling, quaternions));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }

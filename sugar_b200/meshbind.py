@@ -13,6 +13,9 @@ vertices, `_scales` and `_quaternions`.
 
     b = bind_to_mesh(verts, faces, bary, scales_raw, complex_raw, thickness)
     b.points [F*n,3], b.scaling [F*n,3], b.quaternions [F*n,4]
+
+`bind_to_edited_mesh` is the editable model (make_editable / get_edited_quaternions_and_scales, :562-667): the mesh
+moved away from the vertices it was made editable at, forward only, one kernel (sgr_meshbind_edited_forward).
 """
 import math
 from types import SimpleNamespace
@@ -87,4 +90,53 @@ def bind_to_mesh(verts, faces, bary, scales_raw, complex_raw, thickness):
     surface_mesh_thickness).  Returns namespace(points, scaling, quaternions).  Shapes, dtypes and devices are checked
     (ValueError); face ids are not range-checked, which would cost a host synchronisation per step."""
     points, scaling, quats = _MeshBind.apply(verts, faces, bary, scales_raw, complex_raw, float(thickness))
+    return SimpleNamespace(points=points, scaling=scaling, quaternions=quats)
+
+
+def edited_args(verts, reference_verts, faces, bary, scales_raw, complex_raw, thickness):
+    """The checked arguments of one sgr_meshbind_edited_forward launch -> SimpleNamespace (F, n, V, P, tensors as
+    the kernel reads them).  ValueError on a wrong shape, dtype or device, or, under grad mode, on an input that
+    requires grad: the edited binding is forward only."""
+    verts = tensor(verts, "verts", torch.float32, ("V", 3))
+    dev = verts.device
+    V = verts.shape[0]
+    reference_verts = tensor(reference_verts, "reference_verts", torch.float32, (V, 3), dev)
+    faces = tensor(faces, "faces", torch.int64, ("F", 3), dev)
+    if torch.is_tensor(bary) and bary.dim() == 3 and bary.shape[2] == 1:      # the reference's [n,3,1]
+        bary = bary[..., 0]
+    bary = tensor(bary, "bary", torch.float32, ("n", 3), dev)
+    F, n = faces.shape[0], bary.shape[0]
+    scales_raw = tensor(scales_raw, "scales_raw", torch.float32, (F * n, 2), dev)
+    complex_raw = tensor(complex_raw, "complex_raw", torch.float32, (F * n, 2), dev)
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (verts, reference_verts, bary, scales_raw, complex_raw)):
+        raise ValueError("the edited binding is forward only: detach its inputs or run it under torch.no_grad()")
+    return SimpleNamespace(F=F, n=n, V=V, P=F * n, verts=verts, reference_verts=reference_verts, faces=faces, bary=bary,
+                           scales_raw=scales_raw, complex_raw=complex_raw, thickness=float(thickness))
+
+
+def edited_launch(a, points, scaling, quats, out_rows=None):
+    """One sgr_meshbind_edited_forward launch of checked arguments `a` (edited_args) into float32 CUDA buffers, at row
+    g, or at row out_rows[g] (int64 [P], negative: skipped) when given."""
+    require_cuda("meshbind", a.verts)
+    with torch.cuda.device(a.verts.device):
+        check(lib.sgr_meshbind_edited_forward(
+            a.F, a.n, a.V, a.verts.data_ptr(), a.reference_verts.data_ptr(), a.faces.data_ptr(), a.bary.data_ptr(),
+            a.scales_raw.data_ptr(), a.complex_raw.data_ptr(), a.thickness,
+            None if out_rows is None else out_rows.data_ptr(), points.data_ptr(), scaling.data_ptr(),
+            quats.data_ptr(), stream(a.verts.device)))
+
+
+def bind_to_edited_mesh(verts, reference_verts, faces, bary, scales_raw, complex_raw, thickness):
+    """The Gaussians of an EDITABLE bound model: SuGaR.points / .scaling / .quaternions after make_editable() was
+    called with the mesh at `reference_verts` [V,3] and the mesh then moved to `verts` [V,3] (sugar_model.py:562-667).
+    Each Gaussian's in-plane rotation turns with the change in angle of its face's vertex axes, and its two plane
+    scales stretch with their change in length.  Other arguments as bind_to_mesh.  Forward only (ValueError when an
+    input requires grad under grad mode).  Returns namespace(points, scaling, quaternions), each [F*n, .]."""
+    a = edited_args(verts, reference_verts, faces, bary, scales_raw, complex_raw, thickness)
+    require_cuda("meshbind", a.verts)
+    dev = a.verts.device
+    points = torch.empty((a.P, 3), device=dev)
+    scaling = torch.empty((a.P, 3), device=dev)
+    quats = torch.empty((a.P, 4), device=dev)
+    edited_launch(a, points, scaling, quats)
     return SimpleNamespace(points=points, scaling=scaling, quaternions=quats)
