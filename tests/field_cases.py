@@ -13,8 +13,9 @@ float64, allowing a small floor plus what the reference's own float32 chain is o
 o32 is the oracle in float32, o32r the same with each sample's K neighbour columns reversed (a second summation
 order), ours' a second GPU run (the order of the atomics).
     values     |ours - v64| <= floor_v (|v64| + scale) + 3 p          per sample or entry
-    gradients  |ours - g64| <= 1e-4 rowmax|g64| + 4 p + floor_T max|g64|   per row (h.row_errors), the max taken over
-               the row's group (the surface cloud, or one edge group) so an edge's large rows do not hide the rest
+    gradients  |ours - g64| <= 1e-4 rowmax|g64| + 4 p + 2 G + floor_T max|g64|   per row (h.row_errors), the max
+               taken over the row's group (the surface cloud, or one edge group) so an edge's large rows do not hide
+               the rest; G = grad_term_error, the per-term rounding that two summation orders cannot show
 Normal-loss samples with a neighbour where 0 < |<n_k, n_own>| <= 1e-6 (the sign is a coin toss in float32) or a
 Gaussian whose two smallest scales are 1 ulp apart are excluded; exact zeros and exact ties are not.
 """
@@ -40,9 +41,10 @@ VALUE_FLOOR = dict(density=1e-6,                       # 7.6e-8
                    sdf_grad=4e-6,                      # 1.6e-6
                    densest=5e-6,                       # 2.6e-6
                    normal=1e-6)                        # see value_scale
-GRAD_FLOOR = dict(field={"scaling": 2e-3},             # 1.6e-3 (the thinnest cases: dL/ds ~ 1/s^3 cancels)
-                  densest={"scaling": 3e-4},           # 1.6e-4
-                  normal={})                           # default 1e-6 everywhere else (measured <= 9e-7)
+# Gradient floors: with 2 G in the allowance, the smallest floor the float32 oracle in four orders and the kernels'
+# float32 stand-in need over G is at most 4.4e-9 (k16_df1's dL/dstrengths; 0 to 1e-41 elsewhere,
+# test_field_grad_rows_cpu), so every gradient takes the 1e-6 default.
+GRAD_FLOOR = dict(field={}, densest={}, normal={})
 # Gradients that are zero in exact arithmetic, so that every entry is the rounding of cancelling terms: the normal
 # loss's dL/dq in groups where each sample's weighted neighbour normals sum to its own (v = 0) or no weight is left
 # (|n_own|^2 = 1 for every q).  Their values are checked.
@@ -375,19 +377,23 @@ def value_bound(k, v64, v32, v32r, scale, ours=None, ours2=None, model=None):
     return (b if model is None else b + 2.0 * model), floor
 
 
-def grad_bound(kind, leaf, g64, g32, g32r, rows, ours=None, ours2=None):
-    """The allowance of each entry of g [R, C] for the rows of one group, and its floor part."""
+def grad_bound(kind, leaf, g64, g32, g32r, rows, ours=None, ours2=None, model=None):
+    """The allowance of each entry of g [R, C] for the rows of one group, its floor part and its 2 G part (G the
+    per-term rounding bound grad_term_error, passed as `model`)."""
     g64 = g64.reshape(len(g64), -1)
     sh = lambda a: None if a is None else np.asarray(a).reshape(g64.shape)
     gmax = np.abs(g64[rows]).max() if len(rows) else 0.0
     floor = np.broadcast_to(GRAD_FLOOR.get(kind, {}).get(leaf, 1e-6) * gmax, g64.shape)
     b = (1e-4 * np.abs(g64).max(1, keepdims=True) + 4.0 * _p(sh(g32), sh(g32r), g64, sh(ours2), sh(ours)) + floor)
-    return b, floor
+    gm = np.zeros(g64.shape) if model is None else 2.0 * sh(model)
+    return b + gm, floor, gm
 
 
-def check(kind, case, got, ref, got2=None, excluded=None, value_keys=None, model=None):
-    """Hold `got` = (values, grads) to the rule against ref = probes(...).  Returns a report
-    {(group, tensor): dict(ratio, worst, n_over, rows, floor_dominated)} and the number of excluded samples."""
+def check(kind, case, got, ref, got2=None, excluded=None, value_keys=None, model=None, gmodel=None):
+    """Hold `got` = (values, grads) to the rule against ref = probes(...), gradients with gmodel = grad_term_error(...)
+    when given.  Returns a report {(group, tensor): dict(ratio, worst, n_over, rows, floor_dominated)}; a gradient's
+    entry also has g_dominated (the share of rows whose allowance 2 G dominates) and `by`, what dominates the worst
+    row's allowance ('floor', 'G' or 'p', the 1e-4 and float32-order part)."""
     (v64, g64), (v32, g32), (v32r, g32r) = ref
     vals, grads = got
     vals2, grads2 = got2 if got2 is not None else (None, None)
@@ -407,12 +413,18 @@ def check(kind, case, got, ref, got2=None, excluded=None, value_keys=None, model
             if (kind, gname, k) in NOISE_ONLY:
                 continue
             rows = srows[keep[srows]] if k == "x" else grows
-            b, fl = grad_bound(kind, k, g64[k], g32[k], g32r[k], rows, grads[k], None if grads2 is None else grads2[k])
+            b, fl, gm = grad_bound(kind, k, g64[k], g32[k], g32r[k], rows, grads[k],
+                                   None if grads2 is None else grads2[k], None if gmodel is None else gmodel[k])
             want = g64[k].reshape(len(g64[k]), -1)
             r = h.row_errors(np.asarray(grads[k]).reshape(want.shape)[rows], want[rows], b[rows])
+            by = "-"
+            if len(rows):
+                i, c = rows[r["worst_row"]], r["worst_col"]
+                by = max((fl[i, c], "floor"), (gm[i, c], "G"), (b[i, c] - fl[i, c] - gm[i, c], "p"))[1]
             rep[(gname, "d" + k)] = dict(ratio=r["ratio"], worst=int(rows[r["worst_row"]]) if len(rows) else -1,
-                                         n_over=r["n_over"], rows=len(rows),
-                                         floor_dominated=float((fl[rows] * 2 >= b[rows]).mean()) if len(rows) else 0.0)
+                                         n_over=r["n_over"], rows=len(rows), by=by,
+                                         floor_dominated=float((fl[rows] * 2 >= b[rows]).mean()) if len(rows) else 0.0,
+                                         g_dominated=float((gm[rows] * 2 >= b[rows]).mean()) if len(rows) else 0.0)
     return rep
 
 
@@ -422,7 +434,8 @@ def field_oracle_beta(case):
 
 
 def failures(rep):
-    return {k: (round(v["ratio"], 3), v["worst"], v["n_over"]) for k, v in rep.items() if v["n_over"]}
+    """{(group, tensor): (worst ratio, worst row, rows over, what dominates the worst row's allowance)}"""
+    return {k: (round(v["ratio"], 3), v["worst"], v["n_over"], v.get("by", "-")) for k, v in rep.items() if v["n_over"]}
 
 
 def worst(rep):
@@ -484,3 +497,379 @@ def term_error(case):
     f = lambda v: v.numpy()
     return {"closest_gaussian_opacities": f(E_o), "density": f(E_rho), "sdf": f(E_sdf), "beta": f(K * U * beta),
             "densest": f(E_rho + E_t)}
+
+
+# ----------------------------------------------------------------------------------- per-term error model: gradients
+# The backward kernels (field_pair_backward, densest_backward_kernel's lane-0 terms, normal_loss_backward_kernel and
+# smallest_axis_backward) restated once, op for op, over an arithmetic `F`:
+#   _Err   float64 values, each carrying a first-order bound on the absolute error of computing it in float32: every
+#          result is rounded once (U |v|; expf 2 ulp) and carries its operands' errors through its partials, a group
+#          sum of n terms adds (n - 1) U sum |c|, a per-Gaussian sum K U sum |c|.  grad_term_error is C_GRAD times that.
+#   _F32   float32 torch, in the kernels' lane order (lane l takes slots l, l + G, ...; then the xor butterfly): a CPU
+#          stand-in for the kernels (kernel_stand_in).
+# Two neighbour orders of the float32 oracle only change the order of its sums.  On flat Gaussians the gradients'
+# per-term rounding dominates (u = R^T (x - mu) cancels to ~s while |x - mu| is the in-plane scale, and dL/ds ~ 1/s^3
+# amplifies it), and a kernel that rounds those terms differently misses a p-only allowance by orders of magnitude.
+class _E:
+    """A float64 value and a first-order bound on the absolute error of its float32 evaluation."""
+    __slots__ = ("v", "e")
+
+    def __init__(self, v, e=None):
+        self.v = v
+        self.e = torch.zeros_like(v) if e is None else e
+
+    def __getitem__(self, i):
+        return _E(self.v[i], self.e[i])
+
+    def __add__(a, b):
+        b = _lift(b)
+        return _rnd(a.v + b.v, a.e + b.e)
+
+    def __sub__(a, b):
+        b = _lift(b)
+        return _rnd(a.v - b.v, a.e + b.e)
+
+    def __mul__(a, b):
+        b = _lift(b)
+        return _rnd(a.v * b.v, a.e * b.v.abs() + b.e * a.v.abs())
+
+    def __truediv__(a, b):
+        b = _lift(b)
+        v = a.v / b.v
+        return _rnd(v, (a.e + v.abs() * b.e) / b.v.abs())
+
+    __radd__ = lambda a, b: _lift(b) + a
+    __rsub__ = lambda a, b: _lift(b) - a
+    __rmul__ = lambda a, b: _lift(b) * a
+    __rtruediv__ = lambda a, b: _lift(b) / a
+    __neg__ = lambda a: _E(-a.v, a.e)
+
+
+def _lift(a):
+    return a if isinstance(a, _E) else _E(torch.as_tensor(a, dtype=torch.float64))
+
+
+def _rnd(v, e):
+    return _E(v, e + U * v.abs())
+
+
+def _group_width(K):
+    G = 1
+    while G < K and G < 32:
+        G *= 2
+    return G
+
+
+class _Err:
+    @staticmethod
+    def exact(a):
+        return _E(torch.from_numpy(np.asarray(a, np.float64)))
+
+    val = staticmethod(lambda a: a.v)
+
+    @staticmethod
+    def exp(a):
+        v = torch.exp(a.v)
+        return _E(v, v * (a.e + 4 * U))
+
+    @staticmethod
+    def log(a):
+        v = torch.log(a.v)
+        return _E(v, a.e / a.v + 2 * U * v.abs())
+
+    @staticmethod
+    def sqrt(a):
+        v = torch.sqrt(a.v)
+        return _E(v, a.e / (2 * v) + U * v)
+
+    @staticmethod
+    def abs(a):
+        return _E(a.v.abs(), a.e)
+
+    @staticmethod
+    def where(c, a, b):
+        a, b = _lift(a), _lift(b)
+        return _E(torch.where(c, a.v, b.v), torch.where(c, a.e, b.e))
+
+    @staticmethod
+    def group(a):
+        n = a.v.shape[1]
+        return _E(a.v.sum(1), a.e.sum(1) + (n - 1) * U * a.v.abs().sum(1))
+
+    @staticmethod
+    def scatter(P, idx, a, K):
+        z = lambda t: torch.zeros(P, dtype=torch.float64).index_add_(0, idx, t.reshape(-1))
+        return _E(z(a.v), z(a.e) + K * U * z(a.v.abs()))
+
+
+class _F32:
+    @staticmethod
+    def exact(a):
+        return torch.from_numpy(np.ascontiguousarray(a, np.float32))
+
+    val = staticmethod(lambda a: a)
+    exp, log, sqrt, abs = torch.exp, torch.log, torch.sqrt, torch.abs
+
+    @staticmethod
+    def where(c, a, b):
+        f = lambda t: t if torch.is_tensor(t) else torch.tensor(t, dtype=torch.float32)
+        return torch.where(c, f(a), f(b))
+
+    @staticmethod
+    def lanes(a):
+        """The G lanes' partial sums of a [N, K] (lane l: slots l, l + G, ... in order)."""
+        K = a.shape[1]
+        G = _group_width(K)
+        out = []
+        for l in range(G):
+            s = torch.zeros(a.shape[0], dtype=torch.float32)
+            for k in range(l, K, G):
+                s = s + a[:, k]
+            out.append(s)
+        return out
+
+    @staticmethod
+    def group(a):
+        s = _F32.lanes(a)
+        o = len(s) // 2
+        while o:
+            s = [s[l] + s[l ^ o] for l in range(len(s))]
+            o //= 2
+        return s[0]
+
+    @staticmethod
+    def scatter(P, idx, a, K):
+        return torch.zeros(P, dtype=torch.float32).index_add_(0, idx, a.reshape(-1))
+
+
+def _quat_rot(q):
+    """quat_to_rot: R (rows of columns) and two_s of q = (r, i, j, k)."""
+    r, i, j, k = q
+    ts = 2.0 / (r * r + i * i + j * j + k * k)
+    m = [[1 - ts * (j * j + k * k), ts * (i * j - k * r), ts * (i * k + j * r)],
+         [ts * (i * j + k * r), 1 - ts * (i * i + k * k), ts * (j * k - i * r)],
+         [ts * (i * k - j * r), ts * (j * k + i * r), 1 - ts * (i * i + j * j)]]
+    return m, ts
+
+
+def _rot_backward(A, q, ts):
+    qr, qi, qj, qk = q
+    dts = (A[0][0] * -(qj * qj + qk * qk) + A[0][1] * (qi * qj - qk * qr) + A[0][2] * (qi * qk + qj * qr) +
+           A[1][0] * (qi * qj + qk * qr) + A[1][1] * -(qi * qi + qk * qk) + A[1][2] * (qj * qk - qi * qr) +
+           A[2][0] * (qi * qk - qj * qr) + A[2][1] * (qj * qk + qi * qr) + A[2][2] * -(qi * qi + qj * qj))
+    c = -ts * ts * dts
+    dqr = ts * (-qk * A[0][1] + qj * A[0][2] + qk * A[1][0] - qi * A[1][2] - qj * A[2][0] + qi * A[2][1]) + c * qr
+    dqi = ts * (qj * (A[0][1] + A[1][0]) + qk * (A[0][2] + A[2][0]) + qr * (A[2][1] - A[1][2]) -
+                2.0 * qi * (A[1][1] + A[2][2])) + c * qi
+    dqj = ts * (qi * (A[0][1] + A[1][0]) + qr * (A[0][2] - A[2][0]) + qk * (A[1][2] + A[2][1]) -
+                2.0 * qj * (A[0][0] + A[2][2])) + c * qj
+    dqk = ts * (qr * (A[1][0] - A[0][1]) + qi * (A[0][2] + A[2][0]) + qj * (A[1][2] + A[2][1]) -
+                2.0 * qk * (A[0][0] + A[1][1])) + c * qk
+    return [dqr, dqi, dqj, dqk]
+
+
+def _axis_backward(F, col, q, ts, dn):
+    """smallest_axis_backward: dL/dR is dn in column `col`."""
+    A = [[F.where(col == j, dn[i], 0.0) for j in range(3)] for i in range(3)]
+    return _rot_backward(A, q, ts)
+
+
+def _column(F, m, col):
+    return [F.where(col == 0, m[i][0], F.where(col == 1, m[i][1], m[i][2])) for i in range(3)]
+
+
+def _pair_backward(F, x, mu, strength, q, invs, s_ok, col, df, Gk, gbK):
+    """field_pair_backward over all (sample, slot) pairs: dL/dx (= -dL/dmu), dL/dsigma, dL/dq, dL/ds."""
+    m, ts = _quat_rot(q)
+    sh = [x[i] - mu[i] for i in range(3)]
+    u = [m[0][j] * sh[0] + m[1][j] * sh[1] + m[2][j] * sh[2] for j in range(3)]
+    w = [u[j] * invs[j] for j in range(3)]
+    d2raw = w[0] * w[0] + w[1] * w[1] + w[2] * w[2]
+    big = F.val(d2raw) > 1e8
+    e = df * F.exp(-0.5 * F.where(big, 1e8, d2raw))
+    o = strength * e
+    dsig = Gk * e
+    dd2 = F.where(big, 0.0, Gk * o * -0.5)
+    du, ds = [], []
+    for j in range(3):
+        dw = dd2 * 2.0 * w[j]
+        du.append(dw * invs[j])
+        dsj = F.where(s_ok[j], -(dw * u[j]) * invs[j] * invs[j], 0.0)
+        ds.append(F.where(col == j, dsj + gbK, dsj))
+    dsh = [m[i][0] * du[0] + m[i][1] * du[1] + m[i][2] * du[2] for i in range(3)]
+    A = [[sh[i] * du[j] for j in range(3)] for i in range(3)]
+    return dsh, dsig, _rot_backward(A, q, ts), ds
+
+
+def _first_min(s):
+    return torch.from_numpy(np.argmin(np.asarray(s), 1))
+
+
+def _kernel_backward(case, kind, w, F, opac=None):
+    """The kernels' gradients of sum_n w_n . out_n under F: {leaf: [rows, C]} (and, for the float32 stand-in, the
+    per-pair and per-lane pieces the planted defects of the CPU tests take out)."""
+    N, K = case["nbr_idx"].shape
+    P = len(case["points"])
+    nb, gi = torch.from_numpy(case["nbr_idx"]), torch.from_numpy(case["gaussian_idx"])
+    sraw = case["scaling"]
+    xs, pts, qs = F.exact(case["x"]), F.exact(case["points"]), F.exact(case["quaternions"])
+    x = [xs[:, i:i + 1] for i in range(3)]
+    mu = [pts[:, i][nb] for i in range(3)]
+    q = [qs[:, c][nb] for c in range(4)]
+    col_g = _first_min(sraw)
+    extra = {}
+    if kind == "normal":
+        # normal_pack_kernel: n, 1 / max(s_col, 1e-6)^2
+        mg, _ = _quat_rot([qs[:, c] for c in range(4)])
+        ng = _column(F, mg, col_g)
+        cmin = F.exact(np.maximum(sraw[np.arange(P), col_g.numpy()], F32(1e-6)))
+        cg = 1.0 / (cmin * cmin)
+        n_k = [ng[i][nb] for i in range(3)]
+        n0 = [ng[i][gi][:, None] for i in range(3)]
+        dot = n_k[0] * n0[0] + n_k[1] * n0[1] + n_k[2] * n0[2]
+        sg = torch.sign(F.val(dot))
+        op = F.exact(opac)
+        wk = op * F.abs(((x[0] - mu[0]) * n_k[0] + (x[1] - mu[1]) * n_k[1] + (x[2] - mu[2]) * n_k[2]) * sg) * cg[nb]
+        wsum = F.group(wk)
+        sv = [F.group(wk * sg * n_k[i]) for i in range(3)]
+        inv = 1.0 / F.where(F.val(wsum) < 1e-6, 1e-6, wsum)
+        v = [n0[i][:, 0] - sv[i] * inv for i in range(3)]
+        g2 = 2.0 * F.exact(w)
+        c = -g2[:, None] * (wk * inv[:, None]) * sg
+        idx = torch.cat([gi, nb.reshape(-1)])
+        dn = [F.scatter(P, idx, _cat(F, [g2 * v[i], c * v[i][:, None]]), K) for i in range(3)]
+        qg = [qs[:, c] for c in range(4)]
+        dq = _axis_backward(F, col_g, qg, _quat_rot(qg)[1], dn)
+        return {"quaternions": _stack(F, dq)}, {"normal": v[0] * v[0] + v[1] * v[1] + v[2] * v[2]}
+    # pass 1: rho and beta of the sample in the forward's lane order
+    st = F.exact(case["strengths"])[nb]
+    invs_g = 1.0 / F.exact(np.maximum(sraw, F32(1e-8)))
+    invs = [invs_g[:, j][nb] for j in range(3)]
+    m, _ = _quat_rot(q)
+    sh = [x[i] - mu[i] for i in range(3)]
+    wv = [(m[0][j] * sh[0] + m[1][j] * sh[1] + m[2][j] * sh[2]) * invs[j] for j in range(3)]
+    d2 = wv[0] * wv[0] + wv[1] * wv[1] + wv[2] * wv[2]
+    dens = F.group(case["density_factor"] * st * F.exp(-0.5 * F.where(F.val(d2) > 1e8, 1e8, d2)))
+    b = F.group(F.exact(sraw.min(1))[nb]) / float(K)
+    zero = F.exact(np.zeros(N))
+    if kind == "field":
+        gd = F.exact(w["density"]) if "density" in w else zero
+        gb = F.exact(w["beta"]) if "beta" in w else zero
+        if "sdf" in w:                        # sdf_from_density, sdf_offset = 0 at density_threshold 1
+            gs = F.exact(w["sdf"])
+            ge1 = F.val(dens) >= 1.0
+            d = F.where(ge1, dens / (dens + 1e-12), dens)
+            dd = F.where(ge1, 1.0 / (dens + 1e-12), 1.0)
+            low = F.val(d) < float(F32(1e-16))
+            cl = F.where(low, float(F32(1e-16)), d)
+            dd = F.where(low, 0.0, dd)
+            root = F.sqrt(-2.0 * F.log(cl))
+            gb = gb + gs * root
+            gd = F.where(F.val(dd) != 0, gd + gs * (-b / (cl * root)) * dd, gd)
+        Gk = gd[:, None]
+        if "closest_gaussian_opacities" in w:
+            Gk = Gk + F.exact(w["closest_gaussian_opacities"])
+    else:                                     # densest: |rho - t| at lane 0
+        og = [qs[:, c][gi] for c in range(4)]
+        mo, tso = _quat_rot(og)
+        n = _column(F, mo, col_g[gi])
+        dvec = [xs[:, i] - pts[:, i][gi] for i in range(3)]
+        e = dvec[0] * n[0] + dvec[1] * n[1] + dvec[2] * n[2]
+        t = F.exp(-0.5 * (e * e) / (b * b))
+        s = torch.sign(F.val(dens - t)) * F.exact(w)
+        ib2 = 1.0 / (b * b)
+        gd, gb, ge = s, -s * t * (e * e) * ib2 / b, s * t * e * ib2
+        Gk = gd[:, None]
+    col = col_g[nb]
+    s_ok = [torch.from_numpy(sraw[:, j] >= F32(1e-8))[nb] for j in range(3)]
+    dsh, dsig, dq, ds = _pair_backward(F, x, mu, st, q, invs, s_ok, col, case["density_factor"], Gk,
+                                       (gb / float(K))[:, None])
+    dx = [F.group(dsh[i]) for i in range(3)]
+    per_pair = {"points": [-v for v in dsh], "strengths": [dsig], "quaternions": dq, "scaling": ds}
+    own = {}
+    if kind == "densest":
+        dx = [dx[i] + ge * n[i] for i in range(3)]
+        own = {"points": [-ge * n[i] for i in range(3)],
+               "quaternions": _axis_backward(F, col_g[gi], og, tso, [ge * dvec[i] for i in range(3)])}
+    if F is _F32:
+        extra = {"pair": per_pair, "lanes": [_F32.lanes(v) for v in dsh], "gbK": gb / float(K)}
+    out = {"x": _stack(F, dx)}
+    for k, cs in per_pair.items():
+        rows = []
+        for c, v in enumerate(cs):
+            if k in own:
+                rows.append(F.scatter(P, torch.cat([nb.reshape(-1), gi]), _cat(F, [v, own[k][c]]), K))
+            else:
+                rows.append(F.scatter(P, nb.reshape(-1), v, K))
+        out[k] = _stack(F, rows)
+    return out, extra
+
+
+def _cat(F, parts):
+    flat = lambda a: a.reshape(-1)
+    if F is _Err:
+        return _E(torch.cat([flat(p.v) for p in parts]), torch.cat([flat(p.e) for p in parts]))
+    return torch.cat([flat(p) for p in parts])
+
+
+def _stack(F, cols):
+    if F is _Err:
+        return _E(torch.stack([c.v for c in cols], 1), torch.stack([c.e for c in cols], 1))
+    return torch.stack(cols, 1)
+
+
+# The bound's own factor.  The float32 oracle evaluates the same gradients in another algebraic order
+# (L^-1 = R diag(1/s) first, dL/dR summed over a Gaussian's pairs before one quaternion backward, dL/ds through
+# d(1/s)), so its per-op roundings are not the stand-in's.  At C_GRAD = 1 the worst error over floor + G in test_field_grad_rows_cpu is 0.38
+# for the stand-in and 0.38 for the oracle in four orders (k5's dL/dx; <= 0.22 for the normal's dL/dq), so no
+# extra factor is needed.
+C_GRAD = 1.0
+
+
+def grad_term_error(case, kind, w, opac=None):
+    """First-order bound G on the per-term float32 rounding of every gradient entry ('field', 'densest', 'normal'):
+    {leaf: float64 array shaped like the gradient}.  w: field_weights(case) for 'field', the per-sample weights for
+    'densest' and 'normal'; opac: the float32 neighbour opacities the normal loss is given."""
+    rows, _ = _kernel_backward(case, kind, w, _Err, opac)
+    return {k: C_GRAD * v.e.numpy().reshape(_shape(case, k)) for k, v in rows.items()}
+
+
+def kernel_stand_in(case, kind, w, opac=None):
+    """The kernels' float32 gradients on the CPU (grads, pieces): {leaf: float64 array}, and the per-pair and per-lane
+    float32 pieces of the field and densest backwards."""
+    rows, extra = _kernel_backward(case, kind, w, _F32, opac)
+    return {k: v.double().numpy().reshape(_shape(case, k)) for k, v in rows.items()}, extra
+
+
+def _shape(case, k):
+    return {"x": case["x"].shape, "points": case["points"].shape, "scaling": case["scaling"].shape,
+            "quaternions": case["quaternions"].shape, "strengths": case["strengths"].shape}[k]
+
+
+def sdf_grad_error(case):
+    """First-order bound on the float32 rounding of sdf_grad = beta / (rho sqrt(-2 ln rho)) (-d rho / dx), [N, 3]:
+    the coefficient times the field backward's bound on d rho / dx (grad_term_error with a loss on the density alone),
+    plus |d rho / dx| times the coefficient's own error (E_rho through (rho r)' = r - 1/r, r = sqrt(-2 ln rho), and
+    beta's K U); without the E_rho part where rho is clamped below, and 0 at rho >= 1 (no trainer reaches it)."""
+    N, K = case["nbr_idx"].shape
+    ones = {"density": np.ones(N)}
+    rows, _ = _kernel_backward(case, "field", ones, _Err)
+    gx, Gx = rows["x"].v.numpy(), C_GRAD * rows["x"].e.numpy()
+    t = lambda k: torch.from_numpy(np.ascontiguousarray(case[k])).double()
+    v = fo.field_values_torch(t("x"), torch.from_numpy(case["nbr_idx"]), t("points"), t("scaling"), t("quaternions"),
+                              t("strengths"), case["density_factor"])
+    rho, beta = v["density"].numpy(), v["beta"].numpy()
+    omc = float(F32(1e-16))
+    live = (rho > omc) & (rho < 1.0)
+    cl = np.where(live, rho, np.where(rho >= 1.0, 0.5, omc))
+    r = np.sqrt(-2.0 * np.log(cl))
+    coef = np.where(rho < 1.0, beta / np.maximum(cl * r, omc), 0.0)
+    dcoef = coef * (np.where(live, np.abs(r - 1.0 / r) / (cl * r) * term_error(case)["density"], 0.0) + (K + 8) * U)
+    return coef[:, None] * Gx + dcoef[:, None] * np.abs(gx)
+
+
+def normal_value_error(case, opac):
+    """First-order bound on the float32 rounding of the better-normal loss |v|^2 per sample, [N] (the same op-by-op
+    propagation as grad_term_error through the normals, weights, their sums and v = n_own - sum_k w_k m_k)."""
+    _, extra = _kernel_backward(case, "normal", np.zeros(len(case["x"])), _Err, opac)
+    return C_GRAD * extra["normal"].e.numpy()
