@@ -552,6 +552,25 @@ SGR_API int sgr_texture_bake_view(int32_t V, int32_t F, int32_t n_uv, int32_t T,
                                   const float *viewmatrix, const float *projmatrix, int32_t W, int32_t H,
                                   const float *image, const float *zbuf, const int64_t *pix_to_face, float *tex_sum,
                                   int32_t *tex_count, int32_t *owner, int32_t *pix_texel, void *stream);
+/* sgr_texture_render: the textured mesh's image as metrics.py renders it (MeshRasterizer, faces_per_pixel 1, blur 0;
+ * SoftPhongShader with AmbientLights and default Materials, so the shaded colour is the texel; softmax_rgb_blend with
+ * sigma = gamma = 1e-4).  Every pixel with pix_to_face in [0, F) samples `texture` at the face's UV (the bake's
+ * barycentrics and float32 UV) as TexturesUV does: grid_sample on the map flipped in y at 2 uv - 1, align_corners,
+ * border padding, bilinear (torch's weights and summation order) or nearest; then blends with the K = 1 formula,
+ * z_inv = (zfar - zbuf) / (zfar - znear), w = exp((z_inv - max(z_inv, eps)) / gamma), delta = max(exp((eps -
+ * max(z_inv, eps)) / gamma), eps), eps = 1e-10, out = (w c + delta bg) / (w + delta).  The edge term prob is taken as
+ * 1 (pytorch3d's is sigmoid(-dists / sigma) < 1 near a face's edges).  Other pixels (and faces with a vertex or UV id out
+ * of range) are bg.  Deterministic, no atomics.
+ *   texture f32[Ht,Wt,3], verts_uv f32[n_uv,2] (8-byte aligned), faces_uv i64[F,3], zbuf f32[H,W], pix_to_face i64[H,W],
+ *   sampling_mode SGR_SAMPLE_*, finite znear < zfar, image f32[3,H,W] fully written.  Wt*Ht, W*H <= 2^31 - 1. */
+#define SGR_SAMPLE_BILINEAR 0
+#define SGR_SAMPLE_NEAREST 1
+SGR_API int sgr_texture_render(int32_t V, int32_t F, int32_t n_uv, int32_t Wt, int32_t Ht, const float *verts,
+                               const int64_t *faces, const float *verts_uv, const int64_t *faces_uv,
+                               const float *texture, const float *viewmatrix, const float *projmatrix, int32_t W,
+                               int32_t H, const float *zbuf, const int64_t *pix_to_face, int32_t sampling_mode,
+                               float bg_r, float bg_g, float bg_b, double znear, double zfar, float *image,
+                               void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Marching-cubes mesh of the coarse model (the use_marching_cubes branch of coarse_mesh.py:623-714).

@@ -13,10 +13,18 @@ around `iters` calls, `repeats` rounds alternating the arms in one process:
     extraction        the whole extract_texture_image_and_uv_from_gaussians over all views (one call per round)
     ref_init_torch    the reference's initial-texel lines restated in PyTorch (oracle/texture_oracle.initial_texture)
                       on the GPU: the only reference-side arm, pytorch3d being unavailable
+    mesh_render       texture.render_textured_mesh of one view (bilinear): rasterize_mesh, its argument checks and
+                      the shading kernel, the mean over the views
+    shade             the shading kernel alone over a view's z-buffer (texture._shade), bilinear
+    shade_nearest     the same with sampling_mode='nearest'
+    shade_torch       the same pass in PyTorch from the perspective-correct barycentrics pytorch3d's rasterizer hands
+                      its shader (computed outside the timing): gathers for the UV interpolation, F.grid_sample on the
+                      flipped map, the K = 1 blend
 Byte model: texture_init_kernel 12 B per texel written + per face 24 B ids + 36 B vertices + n x 52 B Gaussians;
 per view texture_claim_kernel + texture_add_kernel 36 B per pixel (12 B image, 4 B zbuf, 8 B face id, 8 B texel scratch
 written and read, 4 B owner) + 108 B per baked pixel (face ids, vertices, UV ids and UVs, before cache reuse) + 32 B per
-winning texel (sum and count read and written).  HBM shares are against the H100 SXM data sheet's 3.35 TB/s.  Every
+winning texel (sum and count read and written); texture_render_kernel 24 B per pixel (zbuf, face id, the RGB written)
++ 156 B per covered pixel (face and UV ids, vertices, UVs, four texels; before cache reuse).  HBM shares are against the H100 SXM data sheet's 3.35 TB/s.  Every
 line carries the card's name, power limit and max SM clock, read in the same run.
 """
 import argparse
@@ -80,6 +88,43 @@ def profile_kernels(torch, fn):
     return kern
 
 
+def torch_barycentrics(torch, verts, faces, cam, p2f):
+    """float32 [H,W,3] perspective-correct barycentrics of each pixel's face (0 where none), in float64 on the GPU
+    through the z-buffer's projection: what pytorch3d's rasterizer returns beside pix_to_face."""
+    v = torch.cat([verts.double(), torch.ones(verts.shape[0], 1, device=verts.device, dtype=torch.float64)], 1)
+    z = (v @ cam.viewmatrix.double())[:, 2]
+    h = v @ cam.projmatrix.double()
+    ndc = h[:, :2] / (h[:, 3:4] + 1e-7)
+    x, y = ((ndc[:, 0] + 1.0) * W - 1.0) * 0.5, ((ndc[:, 1] + 1.0) * H - 1.0) * 0.5
+    pix = torch.nonzero(p2f.reshape(-1) >= 0)[:, 0]
+    f = faces[p2f.reshape(-1)[pix]]
+    X, Y, Z = x[f], y[f], z[f]
+    sx, sy = (pix % W).double(), (pix // W).double()
+    area = (X[:, 2] - X[:, 0]) * (Y[:, 1] - Y[:, 0]) - (Y[:, 2] - Y[:, 0]) * (X[:, 1] - X[:, 0])
+    b = torch.stack([((sx - X[:, (e + 1) % 3]) * (Y[:, (e + 2) % 3] - Y[:, (e + 1) % 3]) -
+                      (sy - Y[:, (e + 1) % 3]) * (X[:, (e + 2) % 3] - X[:, (e + 1) % 3])) / area for e in range(3)], 1)
+    w = b * torch.stack([Z[:, 1] * Z[:, 2], Z[:, 0] * Z[:, 2], Z[:, 0] * Z[:, 1]], 1)
+    out = torch.zeros(H * W, 3, device=verts.device)
+    out[pix] = (w / w.sum(1, keepdim=True).clamp(min=1e-8)).float()
+    return out.view(H, W, 3)
+
+
+def shade_torch_pass(torch, faces_uv, verts_uv, tex, zbuf, p2f, bary, znear=1e-4, zfar=100.0):
+    """interpolate_face_attributes, TexturesUV.sample_textures (bilinear) and softmax_rgb_blend (K = 1, prob = 1,
+    black background) in PyTorch.  -> [3,H,W]"""
+    mask = p2f >= 0
+    uv = (bary[..., None] * verts_uv[faces_uv[p2f.clamp(min=0)]]).sum(-2) * mask[..., None]       # [H,W,2]
+    maps = torch.flip(tex.permute(2, 0, 1)[None], [2])
+    c = torch.nn.functional.grid_sample(maps, (uv * 2.0 - 1.0)[None], mode="bilinear", align_corners=True,
+                                        padding_mode="border")[0]                                  # [3,H,W]
+    eps = 1e-10
+    z_inv = (zfar - zbuf) / (zfar - znear) * mask
+    z_max = z_inv.clamp(min=eps)
+    w = mask * torch.exp((z_inv - z_max) / 1e-4)
+    delta = torch.exp((eps - z_max) / 1e-4).clamp(min=eps)
+    return (w * c) / (w + delta)
+
+
 def case_line(args, name, info):
     import torch
     from oracle import texture_oracle as to
@@ -115,7 +160,13 @@ def case_line(args, name, info):
         zbufs = [splatmesh.rasterize_mesh(verts, faces, c) for c in cams]
     state = texture.new_bake_state(init)
     it = iter(range(10 ** 9))
-    pick = lambda: next(it) % len(cams)
+    last = [0]
+
+    def pick():
+        last[0] = next(it) % len(cams)
+        return last[0]
+
+    it_k = lambda: last[0]            # the view pick() just chose (the shade arms' z-buffer for their camera)
 
     def bake_one():
         k = pick()
@@ -132,6 +183,18 @@ def case_line(args, name, info):
             "extraction": lambda: texture.extract_texture_image_and_uv_from_gaussians(
                 verts, faces, pts, scaling, quats, strengths, sh_dc, cams, square_size=S),
             "ref_init_torch": lambda: to.initial_texture(verts, faces, pts, scaling, quats, sh_dc, S, margins=False)}
+    bary = [torch_barycentrics(torch, verts, faces, c, p2f) for c, (_, p2f) in zip(cams, zbufs)]
+
+    def shade_torch(k):
+        zbuf, p2f = zbufs[k]
+        return shade_torch_pass(torch, faces_uv, verts_uv, init, zbuf, p2f, bary[k])
+
+    arms.update({
+        "mesh_render": lambda: texture.render_textured_mesh(verts, faces, verts_uv, faces_uv, init, cams[pick()]),
+        "shade": lambda: texture._shade(verts, faces, verts_uv, faces_uv, init, cams[pick()], *zbufs[it_k()]),
+        "shade_nearest": lambda: texture._shade(verts, faces, verts_uv, faces_uv, init, cams[pick()], *zbufs[it_k()],
+                                                sampling_mode="nearest"),
+        "shade_torch": lambda: shade_torch(pick())})
     iters = {k: (1 if k == "extraction" else args.iters) for k in arms}
     for fn in arms.values():
         fn()
@@ -146,20 +209,27 @@ def case_line(args, name, info):
                                                              cams, square_size=S)[2]
     t2 = texture.extract_texture_image_and_uv_from_gaussians(verts, faces, pts, scaling, quats, strengths, sh_dc,
                                                              cams, square_size=S)[2]
+    # the shading kernel against the torch pass at view 0 (bilinear; the UVs differ by their float32 rounding)
+    shade_max_diff = float((texture._shade(verts, faces, verts_uv, faces_uv, init, cams[0], *zbufs[0]) -
+                            shade_torch(0)).abs().max())
     # per-view stats for the byte model
     baked = sum(int(((p2f >= 0) & (z > 0)).sum()) for z, p2f in zbufs) / len(zbufs)
     st = texture.new_bake_state(init)
     texture._bake(st, verts, faces, verts_uv, faces_uv, cams[0], images[0], *zbufs[0])
     winners = int((st.count > 0).sum())
     kern_init = profile_kernels(torch, arms["initial_texture"])
+    kern_shade = profile_kernels(torch, lambda: texture._shade(verts, faces, verts_uv, faces_uv, init, cams[0],
+                                                               *zbufs[0]))
     kern_bake = profile_kernels(torch, lambda: texture._bake(st, verts, faces, verts_uv, faces_uv, cams[0],
                                                              images[0], *zbufs[0]))
-    kern = {**kern_init, **kern_bake}
+    kern = {**kern_init, **kern_bake, **kern_shade}
     npix = W * H
     model = {"texture_init_kernel": 12 * T * T + F * (60 + 52 * n),
-             "bake (claim + add)": 36 * npix + 108 * int((zbufs[0][1] >= 0).sum()) + 32 * winners}
+             "bake (claim + add)": 36 * npix + 108 * int((zbufs[0][1] >= 0).sum()) + 32 * winners,
+             "texture_render_kernel": 24 * npix + 156 * int((zbufs[0][1] >= 0).sum())}
     bake_ms = kern.get("texture_claim_kernel", 0.0) + kern.get("texture_add_kernel", 0.0)
-    times = {"texture_init_kernel": kern.get("texture_init_kernel"), "bake (claim + add)": bake_ms or None}
+    times = {"texture_init_kernel": kern.get("texture_init_kernel"), "bake (claim + add)": bake_ms or None,
+             "texture_render_kernel": kern.get("texture_render_kernel")}
     gbs = {k: round(model[k] / (times[k] * 1e-3) / 1e9, 1) for k in model if times.get(k)}
     print(json.dumps({
         "what": "UV texture extraction", "case": name, "faces": F, "gaussians_per_face": n, "texture_size": T,
@@ -167,7 +237,7 @@ def case_line(args, name, info):
         "median_ms": {k: median(v) for k, v in ms.items()},
         "mean_baked_pixels_per_view": round(baked), "winning_texels_view0": winners,
         "init_texels_differing_from_torch_restatement": init_diff,
-        "deterministic": bool(torch.equal(t1, t2)), "kernels_ms": kern, "model_bytes": model, "achieved_gbs": gbs,
+        "deterministic": bool(torch.equal(t1, t2)), "shade_vs_torch_max_abs_diff": shade_max_diff, "kernels_ms": kern, "model_bytes": model, "achieved_gbs": gbs,
         "hbm_frac_of_3350_gbs": {k: round(x / PEAK_GBS, 3) for k, x in gbs.items()}, "card": info}), flush=True)
     del images, zbufs, state, st
     torch.cuda.empty_cache()

@@ -139,6 +139,8 @@ PROTOTYPES = {
     "sgr_texture_init": (C.c_int, [C.c_int32] * 5 + [C.c_void_p] * 8),
     "sgr_texture_bake_view": (C.c_int, [C.c_int32] * 4 + [C.c_void_p] * 6 + [C.c_int32, C.c_int32] +
                               [C.c_void_p] * 8),
+    "sgr_texture_render": (C.c_int, [C.c_int32] * 5 + [C.c_void_p] * 7 + [C.c_int32] * 2 + [C.c_void_p] * 2 +
+                           [C.c_int32] + [C.c_float] * 3 + [C.c_double] * 2 + [C.c_void_p] * 2),
     "sgr_density_grid_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_density_grid": (C.c_int, [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32, C.c_float] + [C.c_int32] * 3 +
                          [C.c_void_p] * 3 + [C.c_float] + [C.c_void_p] * 3),

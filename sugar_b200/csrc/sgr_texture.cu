@@ -27,6 +27,12 @@
 // A texel has one writer per view and views are added in call order, so the float32 sums are the reference's
 // ((0 + c_1) + c_2) + ... whenever each view's pixel on a texel is the same; of several pixels of one view on one
 // texel the highest row-major index is kept (the reference's non-accumulating index_put keeps an unspecified one).
+//
+// Render of the textured mesh (metrics.py --use_uv_texture), one kernel over the H*W pixels:
+//   texture_render_kernel pixels with pix_to_face >= 0: the UV exactly as texture_claim_kernel finds it (one shared
+//                         helper), TexturesUV's sample (nearest: the bake's lookup; bilinear: grid_sampler_2d's CUDA
+//                         arithmetic), then softmax_rgb_blend at K = 1 with prob = 1 against the background; other
+//                         pixels are the background.  Planar [3,H,W] output, one write per value.
 #include <math.h>
 
 #include "sgr_internal.cuh"
@@ -130,6 +136,57 @@ __device__ __forceinline__ int nearest_index(float uv, int T)
     return (int)rintf(fminf(fmaxf(ix, 0.0f), (float)(T - 1)));                   // clip_coordinates, nearbyint
 }
 
+// The UV of face f at pixel p's sample point, as pytorch3d's interpolate_face_attributes computes it from the z-buffer:
+// the face's perspective-correct barycentrics b' in double through the z-buffer's projection (view z, projmatrix /
+// (w + 1e-7), ndc2pix), then the UV in float32 (fma chain from 0 over the three corners).  m holds the view and
+// projection matrices (32 floats).  -> false, with u, v untouched, when a vertex or UV id of the face is out of range.
+__device__ __forceinline__ bool face_uv_at_pixel(int p, int W, int H, int V, int n_uv, long long f,
+                                                 const float *__restrict__ verts,
+                                                 const long long *__restrict__ faces,
+                                                 const float2 *__restrict__ verts_uv,
+                                                 const long long *__restrict__ faces_uv, const float *m, float &u,
+                                                 float &v)
+{
+    double x[3], y[3], z[3];
+    float2 uv[3];
+    bool ok = true;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const long long id = __ldg(faces + 3 * f + c), tid = __ldg(faces_uv + 3 * f + c);
+        ok = ok && id >= 0 && id < V && tid >= 0 && tid < n_uv;
+        const long long vi = ok ? id : 0;
+        const double px = verts[3 * vi], py = verts[3 * vi + 1], pz = verts[3 * vi + 2];
+        z[c] = px * m[2] + py * m[6] + pz * m[10] + m[14];
+        const double hx = px * m[16] + py * m[20] + pz * m[24] + m[28];
+        const double hy = px * m[17] + py * m[21] + pz * m[25] + m[29];
+        const double hw = px * m[19] + py * m[23] + pz * m[27] + m[31];
+        const double inv_w = __drcp_rn(hw + 1e-7);
+        x[c] = ((hx * inv_w + 1.0) * W - 1.0) * 0.5;  // ndc2pix
+        y[c] = ((hy * inv_w + 1.0) * H - 1.0) * 0.5;
+        uv[c] = __ldg(verts_uv + (ok ? tid : 0));
+    }
+    if (!ok) return false;
+    const double sx = p % W, sy = p / W;  // the pixel's sample point in ndc2pix units
+    const double area = (x[2] - x[0]) * (y[1] - y[0]) - (y[2] - y[0]) * (x[1] - x[0]);
+    double b[3];
+#pragma unroll
+    for (int e = 0; e < 3; e++) {
+        const int a = (e + 1) % 3, c = (e + 2) % 3;
+        b[e] = ((sx - x[a]) * (y[c] - y[a]) - (sy - y[a]) * (x[c] - x[a])) / area;
+    }
+    const double w0 = b[0] * z[1] * z[2], w1 = b[1] * z[0] * z[2], w2 = b[2] * z[0] * z[1];
+    const double inv = 1.0 / fmax(w0 + w1 + w2, 1e-8);
+    const float bp[3] = {(float)(w0 * inv), (float)(w1 * inv), (float)(w2 * inv)};
+    u = 0.0f;
+    v = 0.0f;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        u = fmaf(bp[c], uv[c].x, u);
+        v = fmaf(bp[c], uv[c].y, v);
+    }
+    return true;
+}
+
 __global__ void __launch_bounds__(TEX_THREADS) texture_claim_kernel(int n_pix, int W, int H, int V, int F, int n_uv, int T,
                                                                     const float *__restrict__ verts,
                                                                     const long long *__restrict__ faces,
@@ -149,46 +206,9 @@ __global__ void __launch_bounds__(TEX_THREADS) texture_claim_kernel(int n_pix, i
     if (p >= n_pix) return;
     int texel = -1;
     const long long f = pix_to_face[p];
-    if (f >= 0 && f < F && zbuf[p] > 0.0f) {
-        double x[3], y[3], z[3];
-        float2 uv[3];
-        bool ok = true;
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            const long long id = __ldg(faces + 3 * f + c), tid = __ldg(faces_uv + 3 * f + c);
-            ok = ok && id >= 0 && id < V && tid >= 0 && tid < n_uv;
-            const long long vi = ok ? id : 0;
-            const double px = verts[3 * vi], py = verts[3 * vi + 1], pz = verts[3 * vi + 2];
-            z[c] = px * m[2] + py * m[6] + pz * m[10] + m[14];
-            const double hx = px * m[16] + py * m[20] + pz * m[24] + m[28];
-            const double hy = px * m[17] + py * m[21] + pz * m[25] + m[29];
-            const double hw = px * m[19] + py * m[23] + pz * m[27] + m[31];
-            const double inv_w = __drcp_rn(hw + 1e-7);
-            x[c] = ((hx * inv_w + 1.0) * W - 1.0) * 0.5;  // ndc2pix
-            y[c] = ((hy * inv_w + 1.0) * H - 1.0) * 0.5;
-            uv[c] = __ldg(verts_uv + (ok ? tid : 0));
-        }
-        if (ok) {
-            const double sx = p % W, sy = p / W;  // the pixel's sample point in ndc2pix units
-            const double area = (x[2] - x[0]) * (y[1] - y[0]) - (y[2] - y[0]) * (x[1] - x[0]);
-            double b[3];
-#pragma unroll
-            for (int e = 0; e < 3; e++) {
-                const int a = (e + 1) % 3, c = (e + 2) % 3;
-                b[e] = ((sx - x[a]) * (y[c] - y[a]) - (sy - y[a]) * (x[c] - x[a])) / area;
-            }
-            const double w0 = b[0] * z[1] * z[2], w1 = b[1] * z[0] * z[2], w2 = b[2] * z[0] * z[1];
-            const double inv = 1.0 / fmax(w0 + w1 + w2, 1e-8);
-            const float bp[3] = {(float)(w0 * inv), (float)(w1 * inv), (float)(w2 * inv)};
-            float u = 0.0f, v = 0.0f;
-#pragma unroll
-            for (int c = 0; c < 3; c++) {
-                u = fmaf(bp[c], uv[c].x, u);
-                v = fmaf(bp[c], uv[c].y, v);
-            }
-            texel = (T - 1 - nearest_index(v, T)) * T + nearest_index(u, T);
-        }
-    }
+    float u, v;
+    if (f >= 0 && f < F && zbuf[p] > 0.0f && face_uv_at_pixel(p, W, H, V, n_uv, f, verts, faces, verts_uv, faces_uv, m, u, v))
+        texel = (T - 1 - nearest_index(v, T)) * T + nearest_index(u, T);
     pix_texel[p] = texel;
     if (texel >= 0) atomicMax(owner + texel, p);
 }
@@ -210,6 +230,87 @@ __global__ void __launch_bounds__(TEX_THREADS) texture_add_kernel(int n_pix, con
     }
     count[t] += 1;
     owner[t] = -1;
+}
+
+// grid_sample's bilinear value (align_corners, border padding) of channel ch of the [Ht,Wt,3] map flipped in y at
+// (u, v), as grid_sampler_2d's CUDA kernel computes it: unnormalise and clip each coordinate, the four corner weights
+// from the floor corner, then out = 0 and one fma per in-bounds corner in the order nw, ne, sw, se.  Row r of the flipped
+// map is row Ht-1-r of `tex`.
+__device__ __forceinline__ void bilinear_texel(float u, float v, int Wt, int Ht, const float *__restrict__ tex,
+                                               float out[3])
+{
+    const float gx = fsub(fmul(u, 2.0f), 1.0f), gy = fsub(fmul(v, 2.0f), 1.0f);      // pixel_uvs * 2.0 - 1.0
+    const float ix = fminf((float)(Wt - 1), fmaxf(fmul(fmul(fadd(gx, 1.0f), 0.5f), (float)(Wt - 1)), 0.0f));
+    const float iy = fminf((float)(Ht - 1), fmaxf(fmul(fmul(fadd(gy, 1.0f), 0.5f), (float)(Ht - 1)), 0.0f));
+    const int x0 = (int)floorf(ix), y0 = (int)floorf(iy), x1 = x0 + 1, y1 = y0 + 1;
+    const float wx1 = fsub((float)x1, ix), wx0 = fsub(ix, (float)x0);
+    const float wy1 = fsub((float)y1, iy), wy0 = fsub(iy, (float)y0);
+    const int xs[4] = {x0, x1, x0, x1}, ys[4] = {y0, y0, y1, y1};
+    const float ws[4] = {fmul(wx1, wy1), fmul(wx0, wy1), fmul(wx1, wy0), fmul(wx0, wy0)};   // nw, ne, sw, se
+    out[0] = out[1] = out[2] = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        if (xs[k] >= Wt || ys[k] >= Ht) continue;   // x0, y0 >= 0 after clipping
+        const float *t = tex + 3 * ((size_t)(Ht - 1 - ys[k]) * Wt + xs[k]);
+#pragma unroll
+        for (int c = 0; c < 3; c++) out[c] = fmaf(__ldg(t + c), ws[k], out[c]);
+    }
+}
+
+// softmax_rgb_blend's K = 1 arithmetic with prob = 1: z_inv = (zfar - z) / (zfar - znear) and the division by gamma both
+// multiply by a float32 reciprocal, as torch's CUDA division by a scalar does.
+struct BlendConsts {
+    float zfar, inv_range, inv_gamma, bg[3];
+};
+
+constexpr float BLEND_EPS = 1e-10f;
+constexpr double BLEND_GAMMA = 1e-4;
+
+__global__ void __launch_bounds__(TEX_THREADS) texture_render_kernel(int n_pix, int W, int H, int V, int F, int n_uv,
+                                                                     int Wt, int Ht, int nearest,
+                                                                     const float *__restrict__ verts,
+                                                                     const long long *__restrict__ faces,
+                                                                     const float2 *__restrict__ verts_uv,
+                                                                     const long long *__restrict__ faces_uv,
+                                                                     const float *__restrict__ tex,
+                                                                     const float *__restrict__ view,
+                                                                     const float *__restrict__ proj,
+                                                                     const float *__restrict__ zbuf,
+                                                                     const long long *__restrict__ pix_to_face,
+                                                                     BlendConsts k, float *__restrict__ out)
+{
+    __shared__ float m[32];  // view, proj
+    if (threadIdx.x < 16) m[threadIdx.x] = view[threadIdx.x];
+    else if (threadIdx.x < 32) m[threadIdx.x] = proj[threadIdx.x - 16];
+    __syncthreads();
+    const int p = blockIdx.x * TEX_THREADS + threadIdx.x;
+    if (p >= n_pix) return;
+    float rgb[3] = {k.bg[0], k.bg[1], k.bg[2]};
+    const long long f = pix_to_face[p];
+    float u, v;
+    if (f >= 0 && f < F && face_uv_at_pixel(p, W, H, V, n_uv, f, verts, faces, verts_uv, faces_uv, m, u, v)) {
+        float c[3];
+        if (nearest) {
+            const float *t = tex + 3 * ((size_t)(Ht - 1 - nearest_index(v, Ht)) * Wt + nearest_index(u, Wt));
+#pragma unroll
+            for (int d = 0; d < 3; d++) c[d] = __ldg(t + d);
+        } else {
+            bilinear_texel(u, v, Wt, Ht, tex, c);
+        }
+        // phong_shading with AmbientLights and default Materials: (1 + 0) * texel + 0
+#pragma unroll
+        for (int d = 0; d < 3; d++) c[d] = fadd(c[d], 0.0f);
+        const float zi = fmul(fsub(k.zfar, zbuf[p]), k.inv_range);
+        const float zmax = zi < BLEND_EPS ? BLEND_EPS : zi;                         // clamp(min=eps) keeps NaN
+        const float w = expf(fmul(fsub(zi, zmax), k.inv_gamma));                    // prob * exp(...), prob = 1
+        float delta = expf(fmul(fsub(BLEND_EPS, zmax), k.inv_gamma));
+        delta = delta < BLEND_EPS ? BLEND_EPS : delta;
+        const float denom = fadd(w, delta);
+#pragma unroll
+        for (int d = 0; d < 3; d++) rgb[d] = __fdiv_rn(fadd(fmul(w, c[d]), fmul(delta, k.bg[d])), denom);
+    }
+#pragma unroll
+    for (int d = 0; d < 3; d++) out[(size_t)d * n_pix + p] = rgb[d];
 }
 
 static int tex_blocks(long long n) { return (int)((n + TEX_THREADS - 1) / TEX_THREADS); }
@@ -289,6 +390,55 @@ int sgr_texture_bake_view(int32_t V, int32_t F, int32_t n_uv, int32_t T, const f
     SGR_LAUNCH(K_MISC, st,
                texture_add_kernel<<<tex_blocks(n_pix), TEX_THREADS, 0, st>>>((int)n_pix, pix_texel, image, owner,
                                                                                tex_sum, tex_count));
+    SGR_CUDA(cudaGetLastError());
+    return SGR_OK;
+}
+
+int sgr_texture_render(int32_t V, int32_t F, int32_t n_uv, int32_t Wt, int32_t Ht, const float *verts,
+                       const int64_t *faces, const float *verts_uv, const int64_t *faces_uv, const float *texture,
+                       const float *viewmatrix, const float *projmatrix, int32_t W, int32_t H, const float *zbuf,
+                       const int64_t *pix_to_face, int32_t sampling_mode, float bg_r, float bg_g, float bg_b,
+                       double znear, double zfar, float *image, void *stream)
+{
+    if (V < 0 || F < 0 || n_uv < 0 || Wt < 1 || Ht < 1 || (long long)Wt * Ht > INT32_MAX || W < 0 || H < 0 ||
+        (long long)W * H > INT32_MAX) {
+        set_error("sgr_texture_render: bad sizes V=%d F=%d n_uv=%d texture %dx%d W=%d H=%d (Wt*Ht, W*H <= 2^31 - 1)",
+                  V, F, n_uv, Wt, Ht, W, H);
+        return SGR_EINVAL;
+    }
+    if (sampling_mode != SGR_SAMPLE_BILINEAR && sampling_mode != SGR_SAMPLE_NEAREST) {
+        set_error("sgr_texture_render: sampling_mode %d (0 bilinear, 1 nearest)", sampling_mode);
+        return SGR_EINVAL;
+    }
+    if (!(znear < zfar) || !isfinite(znear) || !isfinite(zfar)) {
+        set_error("sgr_texture_render: need finite znear < zfar, got %g, %g", znear, zfar);
+        return SGR_EINVAL;
+    }
+    const long long n_pix = (long long)W * H;
+    if (n_pix == 0) return SGR_OK;
+    if (!image || !zbuf || !pix_to_face || !texture || !viewmatrix || !projmatrix ||
+        (F > 0 && (!verts || !faces || !verts_uv || !faces_uv))) {
+        set_error("sgr_texture_render: null pointer");
+        return SGR_EINVAL;
+    }
+    if ((size_t)verts_uv & 7) {
+        set_error("sgr_texture_render: verts_uv must be 8-byte aligned");
+        return SGR_EINVAL;
+    }
+    // F == 0 still launches: every pixel is empty and takes the background
+    BlendConsts k;
+    k.zfar = (float)zfar;
+    k.inv_range = 1.0f / (float)(zfar - znear);
+    k.inv_gamma = 1.0f / (float)BLEND_GAMMA;
+    k.bg[0] = bg_r;
+    k.bg[1] = bg_g;
+    k.bg[2] = bg_b;
+    cudaStream_t st = (cudaStream_t)stream;
+    SGR_LAUNCH(K_MISC, st,
+               texture_render_kernel<<<tex_blocks(n_pix), TEX_THREADS, 0, st>>>(
+                   (int)n_pix, W, H, V, F, n_uv, Wt, Ht, sampling_mode == SGR_SAMPLE_NEAREST, verts,
+                   (const long long *)faces, (const float2 *)verts_uv, (const long long *)faces_uv, texture,
+                   viewmatrix, projmatrix, zbuf, (const long long *)pix_to_face, k, image));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }

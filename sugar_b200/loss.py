@@ -9,6 +9,8 @@ coarse_density.py:101-103, 456-461, refine.py:103-105, 499-504):
 image is the target and is not differentiated (it must not require grad).  The window is the reference's 11x11
 Gaussian (sigma 1.5) and is applied separably; everything else -- zero padding, per-channel planes, C1 / C2 -- is the
 reference's.  There is no CPU fallback.
+
+`psnr` is the evaluation's PSNR (gaussian_splatting/utils/image_utils.py), plain torch beside `ssim` for scoring renders.
 """
 import ctypes as C
 import math
@@ -114,3 +116,10 @@ def l1_dssim_loss(pred, gt, dssim_factor=0.2):
     forward and one backward launch pair."""
     l1, s = l1_ssim_per_image(pred, gt)
     return (1.0 - dssim_factor) * l1.mean() + dssim_factor * (1.0 - s.mean())
+
+
+def psnr(img1, img2):
+    """gaussian_splatting/utils/image_utils.py:17-19: per image of the [B,...] inputs, 20 log10(1 / sqrt(mse)) -> [B,1].
+    Plain torch (an evaluation metric, not on a training path)."""
+    mse = ((img1 - img2) ** 2).view(img1.shape[0], -1).mean(1, keepdim=True)
+    return 20 * torch.log10(1.0 / torch.sqrt(mse))

@@ -31,8 +31,11 @@ Two places where this differs from the reference on purpose:
 The initial texels follow the reference's float32 arithmetic as its CPU evaluation orders it; where two Gaussians'
 densities at a texel are within rounding of each other (argmax near-ties) the chosen Gaussian can differ.
 
-Not built: n_sh > 1 (inconsistent with texture_with_gaussian_renders in the reference), postprocess_mesh's border-face
-removal (off by default) and the .obj / .mtl / .png writers.  Everything runs on the GPU only, under no_grad.
+The textured mesh's image, as metrics.py --use_uv_texture renders it, is `render_textured_mesh`; objfile.py writes and
+reads the .obj / .mtl / .png files.
+
+Not built: n_sh > 1 (inconsistent with texture_with_gaussian_renders in the reference) and postprocess_mesh's border-face
+removal (off by default).  Everything runs on the GPU only, under no_grad.
 """
 import math
 from types import SimpleNamespace
@@ -43,6 +46,7 @@ from ._lib import check, check_ids, lib, require_cuda, same_device, stream, tens
 from .splatmesh import cam_matrix
 
 INT32_MAX = 2 ** 31 - 1
+SAMPLING_MODES = {"bilinear": 0, "nearest": 1}   # SGR_SAMPLE_BILINEAR, SGR_SAMPLE_NEAREST
 SH_C0 = 0.28209479177387814
 
 
@@ -230,3 +234,68 @@ def extract_texture_image_and_uv_from_gaussians(verts, faces, points, scaling, q
             # faces were checked by initial_texture, the layout's ids and rasterize_mesh's output are in range
             _bake(state, verts, faces, verts_uv, faces_uv, cam, image, zbuf, pix_to_face)
         return verts_uv, faces_uv, finish(state)
+
+
+def render_textured_mesh(verts, faces, verts_uv, faces_uv, texture, cam, sampling_mode="bilinear",
+                         background=(0.0, 0.0, 0.0), znear=1e-4, zfar=100.0):
+    """The textured mesh's image as the reference's metrics.py --use_uv_texture renders it: MeshRasterizer (one face
+    per pixel, blur 0) and SoftPhongShader with AmbientLights, so the colour is TexturesUV's sample, blended by
+    softmax_rgb_blend (sigma = gamma = 1e-4) over `background`.  znear = 1e-4 is the attribute the reference's cameras
+    set, zfar = 100 the shader's default.
+
+    verts float32 [V,3], faces int64 [F,3], verts_uv float32 [n_uv,2], faces_uv int64 [F,3], texture float32 [Ht,Wt,3]
+    (row 0 at v = 1, as TexturesUV flips it), `cam` as steps.camera_from_scene builds it; sampling_mode 'bilinear'
+    (load_objs_as_meshes' default) or 'nearest'.  -> float32 [3,H,W].  splatmesh.rasterize_mesh, then one kernel.
+
+    One deliberate difference: the blend's edge weight prob = sigmoid(-dists / sigma) is taken as 1, because the
+    z-buffer does not compute pytorch3d's dists.  In front of the far band the reference's prob c / prob changes a colour
+    by at most about one ulp; inside the band (z within about 0.25 % of zfar - znear below zfar) the colour differs where
+    prob < 1; past zfar the reference still mixes pixels near a face's edge towards the background by prob.  Pixels
+    without a face are the background."""
+    if sampling_mode not in SAMPLING_MODES:
+        raise ValueError(f"sampling_mode must be one of {sorted(SAMPLING_MODES)}, got {sampling_mode!r}")
+    bg = [float(x) for x in background]
+    if len(bg) != 3:
+        raise ValueError(f"background must have 3 values, got {len(bg)}")
+    znear, zfar = float(znear), float(zfar)
+    if not (math.isfinite(znear) and math.isfinite(zfar) and znear < zfar):
+        raise ValueError(f"need finite znear < zfar, got {znear}, {zfar}")
+    dev = verts.device
+    verts = tensor(verts, "verts", torch.float32, ("N", 3))
+    faces = _faces(faces)
+    F = faces.shape[0]
+    verts_uv = tensor(verts_uv, "verts_uv", torch.float32, ("N", 2), align=8)   # one float2 load per UV vertex
+    faces_uv = tensor(faces_uv, "faces_uv", torch.int64, (F, 3))
+    texture = tensor(texture, "texture", torch.float32, ("Ht", "Wt", 3))
+    Ht, Wt = texture.shape[0], texture.shape[1]
+    if not (0 < Ht and 0 < Wt and Ht * Wt <= INT32_MAX):
+        raise ValueError(f"texture {Wt}x{Ht}: need 0 < Wt, Ht and Wt*Ht <= 2^31 - 1")
+    H, W = int(cam.height), int(cam.width)
+    same_device(dev, faces=faces, verts_uv=verts_uv, faces_uv=faces_uv, texture=texture)
+    cam_matrix(cam, "viewmatrix", dev)
+    cam_matrix(cam, "projmatrix", dev)
+    V, n_uv = verts.shape[0], verts_uv.shape[0]
+    if V > INT32_MAX or n_uv > INT32_MAX:
+        raise ValueError(f"{V} vertices / {n_uv} UV vertices: at most 2^31 - 1 each")
+    check_ids((faces_uv, 0, n_uv, "faces_uv ids"))
+    require_cuda("texture", verts, faces, verts_uv, faces_uv, texture)
+    from .splatmesh import rasterize_mesh
+    zbuf, pix_to_face = rasterize_mesh(verts, faces, cam)     # checks the face vertex ids and the image size
+    return _shade(verts, faces, verts_uv, faces_uv, texture, cam, zbuf, pix_to_face, sampling_mode, bg, znear, zfar)
+
+
+def _shade(verts, faces, verts_uv, faces_uv, texture, cam, zbuf, pix_to_face, sampling_mode="bilinear",
+           background=(0.0, 0.0, 0.0), znear=1e-4, zfar=100.0):
+    """The shading kernel alone over a z-buffer of rasterize_mesh, on arguments render_textured_mesh has checked."""
+    dev = verts.device
+    H, W = int(cam.height), int(cam.width)
+    Ht, Wt = texture.shape[0], texture.shape[1]
+    view, proj = cam.viewmatrix.contiguous(), cam.projmatrix.contiguous()
+    with torch.no_grad(), torch.cuda.device(dev):
+        image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        check(lib.sgr_texture_render(verts.shape[0], faces.shape[0], verts_uv.shape[0], Wt, Ht, verts.data_ptr(),
+                                     faces.data_ptr(), verts_uv.data_ptr(), faces_uv.data_ptr(), texture.data_ptr(),
+                                     view.data_ptr(), proj.data_ptr(), W, H, zbuf.data_ptr(), pix_to_face.data_ptr(),
+                                     SAMPLING_MODES[sampling_mode], *[float(x) for x in background], float(znear),
+                                     float(zfar), image.data_ptr(), stream(dev)))
+    return image
