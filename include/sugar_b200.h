@@ -500,6 +500,23 @@ SGR_API int sgr_mesh_nc_backward(int32_t Q, int32_t V, const float *verts, const
                                  void *scratch, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Border-face erosion of the refined mesh (postprocess_mesh, sugar_extractors/refined_mesh.py:140-147): `iterations`
+ * rounds, each one launch on `stream`, no host synchronisation.  Entry 3 f + m is edge m of face f, (0,1), (1,2),
+ * (2,0); the entries are grouped in runs of equal (unordered) edges, built once per call by the caller
+ * (sugar_b200/postprocess.py):
+ *   entry_run i32[3F]    the run of each entry
+ *   run_ptr   i32[R+1]   CSR offsets of the runs into run_faces (entries past R are not read)
+ *   run_faces i32[3F]    the face of each entry, run by run
+ *   mask      u8[F]      in: the live faces (0 / 1); out: those alive after the rounds
+ *   mask_tmp  u8[F]      scratch, distinct from mask
+ * A live face stays in a round iff each of its three runs holds at least 2 entries whose face was live at the start
+ * of the round (a face's own two entries on one edge count twice).  Deterministic, no atomics.
+ * Limits: 0 <= F <= (2^31 - 1) / 3, iterations >= 0.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API int sgr_border_peel(int32_t F, int32_t iterations, const int32_t *entry_run, const int32_t *run_ptr,
+                            const int32_t *run_faces, uint8_t *mask, uint8_t *mask_tmp, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Splatted mesh and nearest-face triangle z-buffer: the default depth source of the level-set extraction
  * (compute_level_surface_points_from_camera_fast with use_gaussian_depth=False, sugar_model.py:1880-1968).
  * sgr_splat_mesh: SuGaR.splat_mesh(camera) for primitive 'diamond', mode 'perspective' (sugar_model.py:481-514,

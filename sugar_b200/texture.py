@@ -34,8 +34,8 @@ densities at a texel are within rounding of each other (argmax near-ties) the ch
 The textured mesh's image, as metrics.py --use_uv_texture renders it, is `render_textured_mesh`; objfile.py writes and
 reads the .obj / .mtl / .png files.
 
-Not built: n_sh > 1 (inconsistent with texture_with_gaussian_renders in the reference) and postprocess_mesh's border-face
-removal (off by default).  Everything runs on the GPU only, under no_grad.
+Not built: n_sh > 1 (inconsistent with texture_with_gaussian_renders in the reference).  postprocess_mesh's border-face
+removal is postprocess.py.  Everything runs on the GPU only, under no_grad.
 """
 import math
 from types import SimpleNamespace
