@@ -725,6 +725,34 @@ SGR_API int sgr_densify_emit(int32_t P, int32_t n_keep, int32_t n_clone, int32_t
                              const float *scales, const float *quaternions, const float *normals, float inv_split,
                              int32_t *src_row, void *stream);
 
+/* ---- Adam step (csrc/sgr_adam.cu): the trainers' optimizer update, every parameter group in one launch -------------
+ * sugar_b200/optim.py is the caller.  Each segment is one float32 parameter tensor of n elements with its gradient and
+ * Adam moments, all updated in place; the scalars are torch's foreach Adam's for this step, computed on the host in
+ * float64 and rounded to float32:
+ *   one_minus_beta1 = 1 - beta1, beta2, one_minus_beta2 = 1 - beta2, bias_correction2_sqrt = (1 - beta2^t)^0.5,
+ *   eps, step_size = -(lr / (1 - beta1^t)).
+ * Per element, each op rounded on its own as torch's foreach kernels round it: m = lerp(m, g, 1 - beta1) (ATen's
+ * lerp), v = v * beta2 + (1 - beta2) * (g * g), d = sqrt(v) / bias_correction2_sqrt + eps, p = p + step_size * (m / d).
+ * 0 <= n <= 2^31 - 1, no null pointer in a segment with n > 0, n_segs <= SGR_ADAM_MAX_SEGMENTS; segs is a HOST
+ * array.  Any float offset is legal (float4 accesses when a segment's four pointers are 16-byte aligned).  No host
+ * synchronisation.
+ * ------------------------------------------------------------------------------------------ */
+#define SGR_ADAM_MAX_SEGMENTS 8
+typedef struct SgrAdamSegment {
+    float *param;
+    const float *grad;
+    float *exp_avg;
+    float *exp_avg_sq;
+    int64_t n;
+    float one_minus_beta1;
+    float beta2;
+    float one_minus_beta2;
+    float bias_correction2_sqrt;
+    float eps;
+    float step_size;   /* negative */
+} SgrAdamSegment;
+SGR_API int sgr_adam_step(int32_t n_segs, const SgrAdamSegment *segs, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */
@@ -736,7 +764,8 @@ SGR_API int sgr_profile_read(float *total_ms, int *counts);
 SGR_API int sgr_profile_timeline(int max_records, int *kinds, float *t_begin_ms, float *t_end_ms);
 
 /* sizeof of an ABI struct as the library was compiled (0 SgrView, 1 SgrGaussians, 2 SgrBackwardPlan, 3 SgrFieldParams,
- * 4 SgrSsimParams, 5 SgrDensifyGates, 6 SgrDensifyColumn; else 0): lets a foreign-language binding check its own struct layout. */
+ * 4 SgrSsimParams, 5 SgrDensifyGates, 6 SgrDensifyColumn, 7 SgrAdamSegment; else 0): lets a foreign-language binding
+ * check its own struct layout. */
 SGR_API size_t sgr_struct_bytes(int32_t which);
 SGR_API const char *sgr_last_error(void);
 SGR_API const char *sgr_version(void);

@@ -56,6 +56,12 @@ class SgrDensifyColumn(C.Structure):
     _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("width", C.c_int32), ("kind", C.c_int32)]
 
 
+class SgrAdamSegment(C.Structure):
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
+                ("n", C.c_int64), ("one_minus_beta1", C.c_float), ("beta2", C.c_float), ("one_minus_beta2", C.c_float),
+                ("bias_correction2_sqrt", C.c_float), ("eps", C.c_float), ("step_size", C.c_float)]
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 STAGE_HOOK = C.CFUNCTYPE(None, C.c_void_p, C.c_int32)
 
@@ -163,6 +169,7 @@ PROTOTYPES = {
                              [C.c_void_p] * 2),
     "sgr_densify_emit": (C.c_int, [C.c_int32] * 5 + [C.c_void_p, C.c_int32, C.POINTER(SgrDensifyColumn)] +
                          [C.c_void_p] * 4 + [C.c_float, C.c_void_p, C.c_void_p]),
+    "sgr_adam_step": (C.c_int, [C.c_int32, C.POINTER(SgrAdamSegment), C.c_void_p]),
     "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_launch_count": (C.c_ulonglong, []),
     "sgr_num_kernel_kinds": (C.c_int, []),
@@ -190,7 +197,7 @@ def _load():
 
 lib = _load()
 for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams, SgrSsimParams, SgrDensifyGates,
-                          SgrDensifyColumn)):
+                          SgrDensifyColumn, SgrAdamSegment)):
     if lib.sgr_struct_bytes(_i) != C.sizeof(_t):   # a stale library or a binding edited without the header
         raise SgrError(f"{LIB_PATH}: struct {_t.__name__} is {lib.sgr_struct_bytes(_i)} bytes in the library, "
                        f"{C.sizeof(_t)} in this binding -- rebuild with `python sugar_b200/build.py`")

@@ -336,6 +336,7 @@ size_t sgr_struct_bytes(int32_t which)
         case 4: return sizeof(SgrSsimParams);
         case 5: return sizeof(SgrDensifyGates);
         case 6: return sizeof(SgrDensifyColumn);
+        case 7: return sizeof(SgrAdamSegment);
         default: return 0;
     }
 }

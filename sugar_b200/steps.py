@@ -219,18 +219,19 @@ def coarse_density_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, den
     return loss.detach(), stats
 
 
-def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0, normal_consistency_factor=0.0):
+def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0, normal_consistency_factor=0.0, sh_deg=3):
     """One refinement iteration's render for mesh-bound Gaussians (sugar_trainers/refine.py; model properties
     sugar_model.py:384-398 points, :415-441 scaling, :443-479 quaternions).  `raw`: verts [V,3], sh_dc, sh_rest,
     densities [P,1], scales [P,2] (in-plane), quaternions [P,2] (the learned 2-D rotation as a complex number);
     `mesh`: faces [F,3] int64, bary [n,3,1], thickness, optionally `topology` (meshloss.mesh_topology of the faces,
     built once); P = F * n.  normal_consistency_factor > 0 adds the surface mesh's normal consistency
-    (refine.py:775-783, 0.1 in the trainers) through ops.mesh_normal_consistency."""
+    (refine.py:775-783, 0.1 in the trainers) through ops.mesh_normal_consistency.  `sh_deg`: the SH degree rendered
+    (the refinement's warm-up raises it from 0 to 3, train.refine_sh_degree)."""
     a = ops.bind_to_mesh(raw["verts"], mesh.faces, mesh.bary, raw["scales"], raw["quaternions"], mesh.thickness)
     b = SimpleNamespace(points=a.points, scaling=a.scaling, quaternions=a.quaternions,
                         strengths=torch.sigmoid(raw["densities"]).view(-1, 1),
                         sh=torch.cat([raw["sh_dc"], raw["sh_rest"]], dim=1))
-    image, radii, _ = render(ops, b, cam, torch.zeros(3, device=b.points.device), sh_deg=3)
+    image, radii, _ = render(ops, b, cam, torch.zeros(3, device=b.points.device), sh_deg=sh_deg)
     loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
     if normal_consistency_factor > 0.0:
         loss = loss + normal_consistency_factor * ops.mesh_normal_consistency(raw["verts"], mesh.faces,

@@ -1,0 +1,191 @@
+"""The trainers' iteration schedules over this package's steps and optimizer.
+
+    opt = train_coarse(raw, views, knn_idx, mode="sdf", spatial_extent=extent)     # coarse_sdf.py / coarse_density.py
+    opt = train_refined(raw, mesh, views, spatial_lr_scale=refine_spatial_lr_scale(n_vertices, extent))   # refine.py
+
+`train_coarse` is the `initialize_from_trained_3dgs=True` path of the coarse trainers (coarse_sdf.py:466-800,
+coarse_density.py:475-815), where densification is off (coarse_sdf.py:71-73) and the SH degree stays at 3.  Each
+iteration `it`:
+
+    1. a CPU randperm of the views at the start of each epoch
+    2. the points group's learning rate from the exponential schedule
+    3. when it - 1 is in prune_at: prune the Gaussians with strength < prune_threshold (Densifier.prune_points), and
+       reset the K-NN table if it > regularize_from                                        coarse_sdf.py:486-499
+    4. K-NN reset when it > regularize_from and (it == regularize_from + 1 or it % reset_neighbors_every == 0)
+                                                                                           :554-561
+    5. it > sdf_from (and > regularize_from): steps.coarse_sdf_step / coarse_density_step, which run the backward;
+       otherwise the RGB render, the photometric loss, plus entropy_factor * the mean binary entropy of the visible
+       Gaussians' strengths when entropy_window[0] < it < entropy_window[1] (:538-551), and the backward
+    6. optimizer.step(), zero_grad(set_to_none=True)
+
+The reference starts its trained-3DGS runs at iteration 7000 (coarse_sdf.py:476-477); `first_iteration=7000` does the
+same, the default 1 runs the whole schedule.  `train_refined` is refine.py:518-850: steps.refine_step with the SH
+degree min(3, (it - 1) // sh_warmup_every) (the warm-up, :849-851), then the optimizer.
+
+`views` is a sequence of (cam, gt_rgb [3,H,W]) with `cam` from steps.camera_from_scene.  Both functions update `raw`
+in place and return the optimizer (a SugarOptimizer; its state_dict() and raw are a checkpoint; pass one in as
+`optimizer=` to reach it during the loop or to resume).  `on_iteration(it, loss, events)` is called after each
+optimizer step with the loss as a device tensor and `events`, the dict that coarse_phase / refine_phase return.
+Nothing is read back to the host beyond what the reference reads: the prune's scan and the sampled-Gaussian counts
+the steps read.  `generator` (a CPU torch.Generator, or None for the default one) draws the view order; the SDF
+samples come from the default CUDA generator, as in the reference.
+"""
+import torch
+
+from . import knn, steps
+from .densify import Densifier
+from .optim import SugarOptimizer, group_table
+
+
+def coarse_phase(it, regularize_from=7000, entropy_window=(7000, 9000), prune_at=(9000,), reset_neighbors_every=500,
+                 sdf_from=9000):
+    """-> the coarse trainers' decisions at iteration `it` (>= 1), as a dict: "sh_degree" (always 3), and "prune",
+    "reset_neighbors", "entropy", "sdf" present (True) when they happen.  A pure function of the schedule."""
+    ev = {"sh_degree": 3}
+    prune = (it - 1) in prune_at
+    if prune:
+        ev["prune"] = True
+    if (prune and it >= regularize_from + 1) or \
+            (it > regularize_from and (it == regularize_from + 1 or it % reset_neighbors_every == 0)):
+        ev["reset_neighbors"] = True
+    if entropy_window[0] < it < entropy_window[1]:
+        ev["entropy"] = True
+    if it > regularize_from and it > sdf_from:
+        ev["sdf"] = True
+    return ev
+
+
+def refine_sh_degree(it, sh_warmup_every=1000):
+    """The refinement's SH degree at iteration `it` (>= 1): 0 at first, one more every sh_warmup_every, at most 3."""
+    return min(3, (it - 1) // sh_warmup_every)
+
+
+def refine_phase(it, sh_warmup_every=1000):
+    """-> the refinement's events at iteration `it`: {"sh_degree": refine_sh_degree(it)}."""
+    return {"sh_degree": refine_sh_degree(it, sh_warmup_every)}
+
+
+def refine_spatial_lr_scale(n_vertices_in_fg, spatial_extent=None, fg_bbox=None):
+    """refine.py:452-459: 10 * bbox_radius / sqrt(n_vertices_in_fg), bbox_radius half the diagonal of `fg_bbox`
+    ((min xyz, max xyz)) when given, else the cameras' spatial extent (mcubes.camera_spatial_extent).  The square root
+    and the bounding-box norm are float32, as the reference's tensors compute them."""
+    if fg_bbox is not None:
+        lo, hi = fg_bbox
+        bbox_radius = ((torch.tensor(hi) - torch.tensor(lo)).norm(dim=-1) / 2.0).item()
+    elif spatial_extent is not None:
+        bbox_radius = spatial_extent
+    else:
+        raise ValueError("refine_spatial_lr_scale needs spatial_extent or fg_bbox")
+    return 10.0 * bbox_radius / torch.tensor(n_vertices_in_fg).pow(1 / 2).item()
+
+
+def entropy_loss(strengths, visible):
+    """Mean of -o log(o + 1e-10) - (1 - o) log(1 - o + 1e-10) over the visible Gaussians' strengths o, without a host
+    read: a masked sum over the visible count (nan when none is visible, as the reference's empty mean)."""
+    o = strengths.view(-1)
+    h = -o * torch.log(o + 1e-10) - (1 - o) * torch.log(1 - o + 1e-10)
+    return torch.where(visible, h, torch.zeros_like(h)).sum() / visible.sum()
+
+
+def _optimizer(optimizer, raw, spatial_lr_scale, bound):
+    """A new SugarOptimizer over `raw`, or the caller's after checking that its groups hold raw's tensors."""
+    if optimizer is None:
+        return SugarOptimizer(raw, spatial_lr_scale=spatial_lr_scale, bound=bound)
+    keys = {name: key for name, key, _ in group_table(1.0, bound)}
+    if not isinstance(optimizer, SugarOptimizer) or len(optimizer.param_groups) != len(keys) or \
+            any(g["params"][0] is not raw[keys[g["name"]]] for g in optimizer.param_groups):
+        raise ValueError(f"optimizer must be a SugarOptimizer over raw's tensors (bound={bound})")
+    return optimizer
+
+
+def _epochs(n_views, generator):
+    while True:
+        yield from torch.randperm(n_views, generator=generator).tolist()
+
+
+def train_coarse(raw, views, knn_idx, mode="sdf", spatial_extent=None, num_iterations=15_000, regularize_from=7000,
+                 entropy_window=(7000, 9000), entropy_factor=0.1, prune_at=(9000,), prune_threshold=0.5,
+                 reset_neighbors_every=500, sdf_from=9000, dssim_factor=0.2, n_samples=1_000_000, generator=None,
+                 on_iteration=None, first_iteration=1, optimizer=None):
+    """The coarse trainer's loop (see the module docstring).  `raw`: steps.activate's dict of leaf tensors (updated in
+    place, replaced by the prune); `knn_idx` [P,K] the K-NN table of raw["points"]; `spatial_extent` the cameras'
+    (mcubes.camera_spatial_extent): the points' learning-rate scale, the Densifier's scene extent and the SDF
+    normalisation.  `optimizer`: a SugarOptimizer over `raw` to continue (one the caller keeps, e.g. to save its
+    state_dict from on_iteration, or one loaded from a checkpoint with first_iteration after it); by default a new one.
+    -> the SugarOptimizer."""
+    if mode not in ("sdf", "density"):
+        raise ValueError(f"mode must be 'sdf' or 'density', got {mode!r}")
+    if spatial_extent is None or not spatial_extent > 0:
+        raise ValueError(f"spatial_extent must be > 0 (mcubes.camera_spatial_extent), got {spatial_extent}")
+    if len(views) == 0:
+        raise ValueError("views is empty")
+    if first_iteration < 1:
+        raise ValueError(f"first_iteration must be >= 1, got {first_iteration}")
+    if entropy_window[1] > max(sdf_from, regularize_from) + 1:
+        raise ValueError(f"entropy_window {tuple(entropy_window)} overlaps the SDF phase (it > {sdf_from}): the "
+                         "regularised steps do not add the entropy term")
+    K = knn_idx.shape[1]
+    ops = steps.ours_ops()
+    optimizer = _optimizer(optimizer, raw, spatial_extent, bound=False)
+    densifier = Densifier(raw, optimizer, scene_extent=spatial_extent)
+    order = _epochs(len(views), generator)
+    dev = raw["points"].device
+    bg = torch.zeros(3, device=dev)
+    for it in range(first_iteration, num_iterations + 1):
+        cam, gt = views[next(order)]
+        optimizer.update_learning_rate(it)
+        ev = coarse_phase(it, regularize_from, entropy_window, prune_at, reset_neighbors_every, sdf_from)
+        if "prune" in ev:
+            densifier.prune_points(torch.sigmoid(raw["densities"].detach()).view(-1) < prune_threshold)
+        if "reset_neighbors" in ev:
+            knn_idx = knn.reset_neighbors(raw["points"].detach(), K)[1]
+        if "sdf" in ev:
+            if mode == "sdf":
+                loss, _ = steps.coarse_sdf_step(raw, cam, gt, knn_idx, ops, n_samples=n_samples,
+                                                spatial_extent=spatial_extent, dssim_factor=dssim_factor,
+                                                fused_depth=True)
+            else:
+                loss, _ = steps.coarse_density_step(raw, cam, gt, knn_idx, ops, n_samples=n_samples,
+                                                    dssim_factor=dssim_factor)
+        else:
+            a = steps.activate(raw)
+            image, radii, _ = steps.render(ops, a, cam, bg, sh_deg=3)
+            loss = steps.photometric_loss(ops, image, gt, dssim_factor)
+            if "entropy" in ev:
+                loss = loss + entropy_factor * entropy_loss(a.strengths, radii > 0)
+            loss.backward()
+            loss = loss.detach()
+        optimizer.step()
+        optimizer.zero_grad(set_to_none=True)
+        if on_iteration is not None:
+            on_iteration(it, loss, ev)
+    return optimizer
+
+
+def train_refined(raw, mesh, views, spatial_lr_scale, num_iterations=15_000, dssim_factor=0.2,
+                  normal_consistency_factor=0.1, sh_warmup_every=1000, generator=None, on_iteration=None,
+                  first_iteration=1, optimizer=None):
+    """The refinement's loop (see the module docstring).  `raw`: steps.refine_step's dict (verts, sh_dc, sh_rest,
+    densities, scales [P,2], quaternions [P,2]; leaf tensors, updated in place); `mesh` as refine_step takes it (give it
+    a `topology` to build the edge table once); `spatial_lr_scale` from refine_spatial_lr_scale; `first_iteration` and
+    `optimizer` (a bound SugarOptimizer over `raw`) as train_coarse takes them.  -> the SugarOptimizer (bound)."""
+    if len(views) == 0:
+        raise ValueError("views is empty")
+    if not spatial_lr_scale > 0:
+        raise ValueError(f"spatial_lr_scale must be > 0, got {spatial_lr_scale}")
+    if first_iteration < 1:
+        raise ValueError(f"first_iteration must be >= 1, got {first_iteration}")
+    ops = steps.ours_ops()
+    optimizer = _optimizer(optimizer, raw, spatial_lr_scale, bound=True)
+    order = _epochs(len(views), generator)
+    for it in range(first_iteration, num_iterations + 1):
+        cam, gt = views[next(order)]
+        optimizer.update_learning_rate(it)
+        ev = refine_phase(it, sh_warmup_every)
+        loss, _ = steps.refine_step(raw, mesh, cam, gt, ops, dssim_factor=dssim_factor,
+                                    normal_consistency_factor=normal_consistency_factor, sh_deg=ev["sh_degree"])
+        optimizer.step()
+        optimizer.zero_grad(set_to_none=True)
+        if on_iteration is not None:
+            on_iteration(it, loss, ev)
+    return optimizer
