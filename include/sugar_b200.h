@@ -106,8 +106,8 @@ SGR_API int sgr_rasterize_forward(const SgrView *view, const SgrGaussians *g,
  * dL_dcolors is the gradient of colors_precomp when colours were precomputed; with SH colours it is the
  * clamp-masked dL/dRGB per Gaussian (the reference's value is unmasked there, but no caller can observe
  * it: colors_precomp is absent).  dL_dsh may be NULL: when M == 0, or with SH present to select "factor
- * mode" -- dL_dsh is not produced, and sgr_view_grad_finalize / sgr_sh_grad_from_factors rebuild (the sum over
- * views of) dL_dsh from dL_dcolors.  All other outputs are unchanged.  Output pointers that are 16-byte aligned
+ * mode" -- dL_dsh is not produced, and sgr_view_grad_finalize rebuilds (the sum over views of) dL_dsh
+ * from dL_dcolors.  All other outputs are unchanged.  Output pointers that are 16-byte aligned
  * leave through TMA bulk stores. */
 SGR_API int sgr_rasterize_backward(const SgrView *view, const SgrGaussians *g, const int32_t *radii,
                            const void *geom_buffer, const void *binning_buffer, const void *image_buffer,
@@ -167,16 +167,82 @@ SGR_API int sgr_rasterize_backward_feature(const SgrView *view, const SgrGaussia
 #define SGR_STAGE_BLEND_DONE 1
 #define SGR_STAGE_CHUNK_DONE 16
 typedef void (*SgrStageHook)(void *ctx, int32_t stage);
+typedef struct SgrPeerPlan SgrPeerPlan;
 typedef struct SgrBackwardPlan {
     SgrStageHook hook; /* may be NULL */
     void *hook_ctx;
     int32_t num_chunks;
     float *reduce_records; /* may be NULL */
     float *dL_dsh_rest;    /* raw-parameter mode (SgrGaussians.activations): f32[P,M-1,3], fully written */
-    /* Peer mode (sgr_peer_* below).  When peer_flag_tab is non-NULL the backward signals the peer ranks itself, on
-     * `stream`, with sequence number peer_seq: slot peer_slot_blend once the blend pass is enqueued (dL_dcolors, which
-     * the caller placed in its peer-visible factor block, is final), slot peer_slot_chunk0 + c after chunk c of the
-     * per-Gaussian pass (reduce_records, placed in the peer-visible record array, holds the chunk's rows). */
+    int32_t chunk_taper;   /* 0: equal chunks; else every chunk half the size of the one before it */
+    const SgrPeerPlan *peer; /* NULL: no peer exchange, see SgrPeerPlan below */
+} SgrBackwardPlan;
+SGR_API int sgr_rasterize_backward_staged(const SgrView *view, const SgrGaussians *g, const int32_t *radii,
+                                          const void *geom_buffer, const void *binning_buffer, const void *image_buffer,
+                                          int64_t num_rendered, const float *dL_dout_color, float *dL_dmeans2D,
+                                          float *dL_dcolors, float *dL_dopacity, float *dL_dmeans3D, float *dL_dcov3D,
+                                          float *dL_dsh, float *dL_dscales, float *dL_drotations, void *grad_scratch,
+                                          void *stream, const SgrBackwardPlan *plan);
+SGR_API int sgr_backward_chunk_range(int32_t P, int32_t num_chunks, int32_t chunk, int32_t taper, int32_t *p0,
+                                     int32_t *p1); /* taper: SgrBackwardPlan.chunk_taper */
+
+/* Epilogue of the view-parallel step for the Gaussians [p0, p1), after the exchange (either half optional):
+ *  - dL_dsh[P,M,3] rows = sum over views v of basis_k(normalize(mean - campos[v])) * dRGB[v][P,3]  (the SH part of
+ *    backward.cu:20-139 is an outer product per view): the gathered factors of view v start at dRGB + v * view_stride
+ *    floats (f32[P,3]; view_stride >= 3P) and its camera position at campos + v * campos_stride floats -- the
+ *    exchange appends every view's camera position to its factor block so that one all-gather carries both;
+ *  - reduced_records f32[P,11] (all-reduced) are split into dL_dmeans3D / dL_dopacity / dL_dscales / dL_drotations.
+ * Every output row of the range is fully written; `scale` (e.g. 1/num_views) multiplies everything. */
+SGR_API int sgr_view_grad_finalize(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree, int32_t num_views,
+                                   const float *means3D, const float *campos, const float *dRGB, int64_t view_stride,
+                                   int32_t campos_stride, float *dL_dsh, const float *reduced_records, float scale,
+                                   float *dL_dmeans3D, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
+                                   void *stream);
+
+/* ---- View-parallel exchange over peer memory (NVLink / NVSwitch): csrc/sgr_peer.cu.  No counterpart in the reference.
+ * sgr_peer_alloc     one zero-filled device allocation on the current device whose CUDA IPC handle (sgr_peer_export,
+ *                    64 bytes, to be sent to the other ranks by any means) maps it at offset 0;
+ * sgr_peer_import    maps a peer's allocation into this process (lazy peer access); sgr_peer_close unmaps it.
+ * Flag words: the first sgr_peer_flag_bytes() of an allocation used with signal / wait are u32
+ * [SGR_PEER_MAX_SLOTS][SGR_PEER_MAX_RANKS]; word [slot][j] is written by rank j only.
+ * sgr_peer_signal    (on `stream`) writes `seq` into word [slot][my_rank] of EVERY rank's flags (flag_tab: device array
+ *                    of nranks pointers to the ranks' flag words), after a system-scope fence;
+ * sgr_peer_wait      (on `stream`) spins until words [slot0 .. slot0+nslots)[0 .. nranks) of the LOCAL flags have all
+ *                    reached seq (wrap-safe); traps after timeout_s seconds (<= 0: 20 s) instead of hanging;
+ * sgr_peer_reduce_records_synced  second half of the records' all-reduce for the chunk of Gaussians [p0, p1) (p0 a
+ *                    multiple of 64): this rank sums the slice of the chunk it OWNS -- the 64-record blocks b with
+ *                    b * nranks / blocks == my_rank, the ones the per-Gaussian pass stored here
+ *                    (SgrPeerPlan.peer_record_stages) -- over the nranks staging arrays rec_tab points to (device
+ *                    array of pointers to f32[11P + 4]; normally all LOCAL), in rank order, and stores the sums into
+ *                    every rank's sum array (sum_tab, likewise; remote entries are posted NVLink writes).  The flag
+ *                    handshake is folded into the kernel: it first waits until every rank's word of wait_slot in the
+ *                    LOCAL flags has reached seq (flags NULL: no wait), and its last CTA to finish writes seq into
+ *                    word [signal_slot][my_rank] of every rank's flags (flag_tab NULL: no signal; `counter`: a
+ *                    zero-initialised u32 in local device memory that the kernel re-arms, one per concurrently running
+ *                    launch). */
+#define SGR_PEER_MAX_RANKS 64
+#define SGR_PEER_MAX_SLOTS 64
+SGR_API int sgr_peer_alloc(size_t bytes, void **ptr);
+SGR_API int sgr_peer_free(void *ptr);
+SGR_API int sgr_peer_export(const void *ptr, void *handle64);
+SGR_API int sgr_peer_import(const void *handle64, void **ptr);
+SGR_API int sgr_peer_close(void *ptr);
+SGR_API size_t sgr_peer_flag_bytes(void);
+SGR_API int sgr_peer_signal(void *const *flag_tab, int32_t nranks, int32_t slot, int32_t my_rank, uint32_t seq,
+                            void *stream);
+SGR_API int sgr_peer_wait(const void *flags, int32_t nranks, int32_t slot0, int32_t nslots, uint32_t seq,
+                          double timeout_s, void *stream);
+SGR_API int sgr_peer_reduce_records_synced(const void *const *rec_tab, void *const *sum_tab, int32_t nranks,
+                                           int32_t my_rank, int32_t p0, int32_t p1, const void *flags, int32_t wait_slot,
+                                           void *const *flag_tab, int32_t signal_slot, uint32_t seq, void *counter,
+                                           double timeout_s, void *stream);
+
+/* The peer exchange of a backward (SgrBackwardPlan.peer): the backward signals the peer ranks itself, on `stream`,
+ * with sequence number peer_seq: slot peer_slot_blend once the blend pass is enqueued (dL_dcolors, which the caller
+ * placed in its peer-visible factor block, is final), slot peer_slot_chunk0 + c after chunk c of the per-Gaussian
+ * pass (reduce_records, placed in the peer-visible record array, holds the chunk's rows).  The backward checks every
+ * field before it enqueues anything. */
+struct SgrPeerPlan {
     void *const *peer_flag_tab; /* DEVICE array of peer_nranks pointers: every rank's flag words, see sgr_peer_signal */
     int32_t peer_nranks, peer_rank, peer_slot_blend, peer_slot_chunk0;
     uint32_t peer_seq;
@@ -190,12 +256,11 @@ typedef struct SgrBackwardPlan {
     const void *peer_flags;
     float peer_dsh_scale;
     double peer_timeout_s;
-    int32_t chunk_taper; /* 0: equal chunks; else every chunk half the size of the one before it */
     /* With peer_view_blocks: DEVICE array of peer_nranks pointers, entry j = rank j's staging array (f32[11P + 4]) for
      * records COMING FROM this rank (entry peer_rank = reduce_records itself).  CTA b of a chunk's launch then stores its
      * 64 records into the array of the rank that owns them (owner = b * nranks / CTAs of the chunk; what
-     * sgr_peer_reduce_records assumes) with a TMA bulk store over NVLink -- the reduce-scatter half of the records'
-     * all-reduce is fused into the pass.  NULL: all records go to reduce_records. */
+     * sgr_peer_reduce_records_synced assumes) with a TMA bulk store over NVLink -- the reduce-scatter half of the
+     * records' all-reduce is fused into the pass.  NULL: all records go to reduce_records. */
     float *const *peer_record_stages;
     /* Optional second stream for the backward's own signals: each signal kernel then runs there, behind an event
      * recorded on `stream`, and the per-Gaussian chunks follow one another on `stream` without the signals' launches
@@ -215,80 +280,7 @@ typedef struct SgrBackwardPlan {
     const float *peer_sums;
     int32_t peer_slot_reduced0;
     uint64_t peer_emulate_ranks;
-} SgrBackwardPlan;
-SGR_API int sgr_rasterize_backward_staged(const SgrView *view, const SgrGaussians *g, const int32_t *radii,
-                                          const void *geom_buffer, const void *binning_buffer, const void *image_buffer,
-                                          int64_t num_rendered, const float *dL_dout_color, float *dL_dmeans2D,
-                                          float *dL_dcolors, float *dL_dopacity, float *dL_dmeans3D, float *dL_dcov3D,
-                                          float *dL_dsh, float *dL_dscales, float *dL_drotations, void *grad_scratch,
-                                          void *stream, const SgrBackwardPlan *plan);
-SGR_API int sgr_backward_chunk_range(int32_t P, int32_t num_chunks, int32_t chunk, int32_t *p0, int32_t *p1);
-SGR_API int sgr_backward_chunk_range_tapered(int32_t P, int32_t num_chunks, int32_t chunk, int32_t taper, int32_t *p0,
-                                             int32_t *p1); /* SgrBackwardPlan.chunk_taper */
-
-/* Epilogue of the view-parallel step for the Gaussians [p0, p1), after the exchange (either half optional):
- *  - dL_dsh[P,M,3] rows = sum over views v of basis_k(normalize(mean - campos[v])) * dRGB[v][P,3]  (the SH part of
- *    backward.cu:20-139 is an outer product per view): the gathered factors of view v start at dRGB + v * view_stride
- *    floats (f32[P,3]; view_stride >= 3P) and its camera position at campos + v * campos_stride floats -- the
- *    exchange appends every view's camera position to its factor block so that one all-gather carries both;
- *  - reduced_records f32[P,11] (all-reduced) are split into dL_dmeans3D / dL_dopacity / dL_dscales / dL_drotations.
- * Every output row of the range is fully written; `scale` (e.g. 1/num_views) multiplies everything. */
-SGR_API int sgr_view_grad_finalize(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree, int32_t num_views,
-                                   const float *means3D, const float *campos, const float *dRGB, int64_t view_stride,
-                                   int32_t campos_stride, float *dL_dsh, const float *reduced_records, float scale,
-                                   float *dL_dmeans3D, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
-                                   void *stream);
-/* The same epilogue reading every view's factor block through a DEVICE-resident table of num_views pointers
- * (view_blocks[v] -> f32[3P] factors followed by that view's camera position, 3 floats).  The entries may point into
- * other GPUs' memory mapped with sgr_peer_import: the all-gather of the factors is then fused into this kernel's loads
- * over NVLink and no gathered copy exists. */
-SGR_API int sgr_view_grad_finalize_peers(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree,
-                                         int32_t num_views, const float *means3D, const float *const *view_blocks,
-                                         float *dL_dsh, const float *reduced_records, float scale, float *dL_dmeans3D,
-                                         float *dL_dopacity, float *dL_dscales, float *dL_drotations, void *stream);
-
-/* ---- View-parallel exchange over peer memory (NVLink / NVSwitch): csrc/sgr_peer.cu.  No counterpart in the reference.
- * sgr_peer_alloc     one zero-filled device allocation on the current device whose CUDA IPC handle (sgr_peer_export,
- *                    64 bytes, to be sent to the other ranks by any means) maps it at offset 0;
- * sgr_peer_import    maps a peer's allocation into this process (lazy peer access); sgr_peer_close unmaps it.
- * Flag words: the first sgr_peer_flag_bytes() of an allocation used with signal / wait are u32
- * [SGR_PEER_MAX_SLOTS][SGR_PEER_MAX_RANKS]; word [slot][j] is written by rank j only.
- * sgr_peer_signal    (on `stream`) writes `seq` into word [slot][my_rank] of EVERY rank's flags (flag_tab: device array
- *                    of nranks pointers to the ranks' flag words), after a system-scope fence;
- * sgr_peer_wait      (on `stream`) spins until words [slot0 .. slot0+nslots)[0 .. nranks) of the LOCAL flags have all
- *                    reached seq (wrap-safe); traps after timeout_s seconds (<= 0: 20 s) instead of hanging;
- * sgr_peer_reduce_records  second half of the records' all-reduce for the chunk of Gaussians [p0, p1) (p0 a multiple of
- *                    64): this rank sums the slice of the chunk it OWNS -- the 64-record blocks b with
- *                    b * nranks / blocks == my_rank, the ones the per-Gaussian pass stored here
- *                    (SgrBackwardPlan.peer_record_stages) -- over the nranks staging arrays rec_tab points to (device
- *                    array of pointers to f32[11P + 4]; normally all LOCAL), in rank order, and stores the sums into
- *                    every rank's sum array (sum_tab, likewise; remote entries are posted NVLink writes). */
-#define SGR_PEER_MAX_RANKS 64
-#define SGR_PEER_MAX_SLOTS 64
-SGR_API int sgr_peer_alloc(size_t bytes, void **ptr);
-SGR_API int sgr_peer_free(void *ptr);
-SGR_API int sgr_peer_export(const void *ptr, void *handle64);
-SGR_API int sgr_peer_import(const void *handle64, void **ptr);
-SGR_API int sgr_peer_close(void *ptr);
-SGR_API size_t sgr_peer_flag_bytes(void);
-SGR_API int sgr_peer_signal(void *const *flag_tab, int32_t nranks, int32_t slot, int32_t my_rank, uint32_t seq,
-                            void *stream);
-SGR_API int sgr_peer_wait(const void *flags, int32_t nranks, int32_t slot0, int32_t nslots, uint32_t seq,
-                          double timeout_s, void *stream);
-SGR_API int sgr_peer_reduce_records(const void *const *rec_tab, void *const *sum_tab, int32_t nranks, int32_t my_rank,
-                                    int32_t p0, int32_t p1, void *stream);
-/* The same with the flag handshake folded into the kernel: it first waits until every rank's word of wait_slot in the
- * LOCAL flags has reached seq (flags NULL: no wait), and its last CTA to finish writes seq into word
- * [signal_slot][my_rank] of every rank's flags (flag_tab NULL: no signal; `counter`: a zero-initialised u32 in local
- * device memory that the kernel re-arms, one per concurrently running launch). */
-SGR_API int sgr_peer_reduce_records_synced(const void *const *rec_tab, void *const *sum_tab, int32_t nranks,
-                                           int32_t my_rank, int32_t p0, int32_t p1, const void *flags, int32_t wait_slot,
-                                           void *const *flag_tab, int32_t signal_slot, uint32_t seq, void *counter,
-                                           double timeout_s, void *stream);
-
-/* The SH half alone, over all Gaussians (kept for callers that only exchange factors). */
-SGR_API int sgr_sh_grad_from_factors(int32_t P, int32_t M, int32_t sh_degree, int32_t num_views, const float *means3D,
-                                     const float *campos, const float *dRGB, float *dL_dsh, void *stream);
+};
 
 /* markVisible (rasterizer_impl.cu:141-153): present[i] = view-space z > 0.2. */
 SGR_API int sgr_mark_visible(int32_t P, const float *means3D, const float *viewmatrix,
@@ -764,7 +756,7 @@ SGR_API int sgr_profile_read(float *total_ms, int *counts);
 SGR_API int sgr_profile_timeline(int max_records, int *kinds, float *t_begin_ms, float *t_end_ms);
 
 /* sizeof of an ABI struct as the library was compiled (0 SgrView, 1 SgrGaussians, 2 SgrBackwardPlan, 3 SgrFieldParams,
- * 4 SgrSsimParams, 5 SgrDensifyGates, 6 SgrDensifyColumn, 7 SgrAdamSegment; else 0): lets a foreign-language binding
+ * 4 SgrSsimParams, 5 SgrDensifyGates, 6 SgrDensifyColumn, 7 SgrAdamSegment, 8 SgrPeerPlan; else 0): lets a foreign-language binding
  * check its own struct layout. */
 SGR_API size_t sgr_struct_bytes(int32_t which);
 SGR_API const char *sgr_last_error(void);

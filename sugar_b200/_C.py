@@ -314,8 +314,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             elif ex is not None:
                 ex.run_backward(launch, b, P, M, int(degree), means3D, campos, has_cov_precomp=has_cov)
             elif raw:   # the plan carries the second SH gradient array
-                launch(_lib.SgrBackwardPlan(_lib.STAGE_HOOK(0), None, 1, None,
-                                            b["sh_rest"].data_ptr() if M > 1 else None))
+                launch(_lib.SgrBackwardPlan(num_chunks=1, dL_dsh_rest=b["sh_rest"].data_ptr() if M > 1 else None))
             else:
                 launch(None)
     out = (b["means2D"], b["colors"], b["opacity"], b["means3D"], b["cov3D"], b["sh"], b["scales"], b["rotations"])

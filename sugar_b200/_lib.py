@@ -66,16 +66,19 @@ ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 STAGE_HOOK = C.CFUNCTYPE(None, C.c_void_p, C.c_int32)
 
 
-class SgrBackwardPlan(C.Structure):
-    _fields_ = [("hook", STAGE_HOOK), ("hook_ctx", C.c_void_p), ("num_chunks", C.c_int32),
-                ("reduce_records", C.c_void_p), ("dL_dsh_rest", C.c_void_p),
-                ("peer_flag_tab", C.c_void_p), ("peer_nranks", C.c_int32), ("peer_rank", C.c_int32),
+class SgrPeerPlan(C.Structure):
+    _fields_ = [("peer_flag_tab", C.c_void_p), ("peer_nranks", C.c_int32), ("peer_rank", C.c_int32),
                 ("peer_slot_blend", C.c_int32), ("peer_slot_chunk0", C.c_int32), ("peer_seq", C.c_uint32),
                 ("peer_view_blocks", C.c_void_p), ("peer_flags", C.c_void_p), ("peer_dsh_scale", C.c_float),
-                ("peer_timeout_s", C.c_double), ("chunk_taper", C.c_int32),
-                ("peer_record_stages", C.c_void_p), ("peer_signal_stream", C.c_void_p),
+                ("peer_timeout_s", C.c_double), ("peer_record_stages", C.c_void_p), ("peer_signal_stream", C.c_void_p),
                 ("peer_side_stream", C.c_void_p), ("peer_rec_tab", C.c_void_p), ("peer_sum_tab", C.c_void_p),
                 ("peer_sums", C.c_void_p), ("peer_slot_reduced0", C.c_int32), ("peer_emulate_ranks", C.c_uint64)]
+
+
+class SgrBackwardPlan(C.Structure):
+    _fields_ = [("hook", STAGE_HOOK), ("hook_ctx", C.c_void_p), ("num_chunks", C.c_int32),
+                ("reduce_records", C.c_void_p), ("dL_dsh_rest", C.c_void_p), ("chunk_taper", C.c_int32),
+                ("peer", C.POINTER(SgrPeerPlan))]
 
 
 # name -> (restype, argtypes); kept in one table so tests can check it against the header
@@ -92,11 +95,9 @@ PROTOTYPES = {
                                       [C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
     "sgr_rasterize_backward_feature": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians)] + [C.c_void_p] * 4 +
                                        [C.c_int64] + [C.c_void_p] * 15),
-    "sgr_backward_chunk_range":(C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
-    "sgr_backward_chunk_range_tapered": (C.c_int, [C.c_int32] * 4 + [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "sgr_backward_chunk_range": (C.c_int, [C.c_int32] * 4 + [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "sgr_view_grad_finalize": (C.c_int, [C.c_int32] * 6 + [C.c_void_p] * 3 + [C.c_int64, C.c_int32] + [C.c_void_p] * 2 +
                                [C.c_float] + [C.c_void_p] * 5),
-    "sgr_view_grad_finalize_peers": (C.c_int, [C.c_int32] * 6 + [C.c_void_p] * 4 + [C.c_float] + [C.c_void_p] * 5),
     "sgr_peer_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p)]),
     "sgr_peer_free": (C.c_int, [C.c_void_p]),
     "sgr_peer_export": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -105,12 +106,10 @@ PROTOTYPES = {
     "sgr_peer_flag_bytes": (C.c_size_t, []),
     "sgr_peer_signal": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32, C.c_void_p]),
     "sgr_peer_wait": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32, C.c_double, C.c_void_p]),
-    "sgr_peer_reduce_records": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "sgr_peer_reduce_records_synced": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                  C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_uint32, C.c_void_p,
                                                  C.c_double, C.c_void_p]),
     "sgr_mark_visible": (C.c_int, [C.c_int32] + [C.c_void_p] * 5),
-    "sgr_sh_grad_from_factors": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 5),
     "sgr_geometry_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_binning_bytes": (C.c_size_t, [C.c_int64]),
     "sgr_image_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
@@ -197,7 +196,7 @@ def _load():
 
 lib = _load()
 for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams, SgrSsimParams, SgrDensifyGates,
-                          SgrDensifyColumn, SgrAdamSegment)):
+                          SgrDensifyColumn, SgrAdamSegment, SgrPeerPlan)):
     if lib.sgr_struct_bytes(_i) != C.sizeof(_t):   # a stale library or a binding edited without the header
         raise SgrError(f"{LIB_PATH}: struct {_t.__name__} is {lib.sgr_struct_bytes(_i)} bytes in the library, "
                        f"{C.sizeof(_t)} in this binding -- rebuild with `python sugar_b200/build.py`")

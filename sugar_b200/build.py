@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("SGR_LIB_OUT", os.path.join(HERE, "lib", "libsugar_b200.so"))
-SOURCES = ["sgr_api.cu", "sgr_forward.cu", "sgr_backward.cu", "sgr_field.cu", "sgr_normal.cu", "sgr_knn.cu", "sgr_meshbind.cu",
+SOURCES = ["sgr_api.cu", "sgr_forward.cu", "sgr_backward.cu", "sgr_exchange.cu", "sgr_field.cu", "sgr_normal.cu", "sgr_knn.cu", "sgr_meshbind.cu",
            "sgr_peer.cu", "sgr_loss.cu", "sgr_meshloss.cu", "sgr_splatmesh.cu",
            "sgr_texture.cu", "sgr_mcubes.cu", "sgr_decimate.cu", "sgr_densify.cu", "sgr_poisson.cu", "sgr_compose.cu",
            "sgr_postprocess.cu", "sgr_adam.cu"]

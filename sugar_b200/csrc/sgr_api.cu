@@ -199,6 +199,38 @@ static int rasterize_backward(const char *who, const SgrView *view, const SgrGau
         set_error("null pointer passed to %s", who);
         return SGR_EINVAL;
     }
+    // the plan as well, before anything is enqueued: a peer-mode backward that gave up after its BLEND signal had gone
+    // out would leave the other ranks waiting for it until their wait kernels trap
+    if (g->activations != 0 && g->shs && dL_dsh && g->M > 1 && !(plan && plan->dL_dsh_rest)) {
+        set_error("raw-parameter mode needs SgrBackwardPlan.dL_dsh_rest");
+        return SGR_EINVAL;
+    }
+    const SgrPeerPlan *pp = plan ? plan->peer : nullptr;
+    const int nchunks = backward_chunks(g->P, plan ? plan->num_chunks : 1);
+    const auto slots_ok = [&](int slot0, int nslots) { return slot0 >= 0 && slot0 + nslots <= SGR_PEER_MAX_SLOTS; };
+    if (pp && (!pp->peer_flag_tab || pp->peer_nranks < 1 || pp->peer_nranks > SGR_PEER_MAX_RANKS || pp->peer_rank < 0 ||
+               pp->peer_rank >= pp->peer_nranks || !slots_ok(pp->peer_slot_blend, 1) ||
+               !slots_ok(pp->peer_slot_chunk0, nchunks) || (pp->peer_signal_stream && nchunks > 19))) {
+        set_error("SgrPeerPlan: needs peer_flag_tab, 1 <= peer_nranks <= %d, peer_rank < peer_nranks, flag slots in the "
+                  "table and, with peer_signal_stream, at most 19 chunks", SGR_PEER_MAX_RANKS);
+        return SGR_EINVAL;
+    }
+    const bool views = pp && pp->peer_view_blocks && dL_dsh && g->shs;
+    if (views && (g->activations != 0 || !pp->peer_flags)) {
+        set_error("peer_view_blocks: needs peer_flags and activated (not raw) parameters");
+        return SGR_EINVAL;
+    }
+    if (views && pp->peer_record_stages && !records) {
+        set_error("peer_record_stages needs reduce_records (the local staging array)");
+        return SGR_EINVAL;
+    }
+    if (pp && pp->peer_side_stream &&
+        (!pp->peer_rec_tab || !pp->peer_sum_tab || !pp->peer_sums || !pp->peer_flags || !records || !dL_dmeans3D ||
+         !dL_dopacity || !dL_dscales || !dL_drotations || nchunks > 16 || !slots_ok(pp->peer_slot_reduced0, nchunks))) {
+        set_error("peer_side_stream needs peer_rec_tab / peer_sum_tab / peer_sums / peer_flags, reduce_records, the four "
+                  "record-bound gradient arrays, at most 16 chunks and peer_slot_reduced0 + chunks inside the flag table");
+        return SGR_EINVAL;
+    }
     return launch_backward(view, g, radii, geom_buffer, binning_buffer, image_buffer, num_rendered, dL_dout_color,
                            dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales,
                            dL_drotations, grad_scratch, (cudaStream_t)stream, plan, feat);
@@ -337,6 +369,7 @@ size_t sgr_struct_bytes(int32_t which)
         case 5: return sizeof(SgrDensifyGates);
         case 6: return sizeof(SgrDensifyColumn);
         case 7: return sizeof(SgrAdamSegment);
+        case 8: return sizeof(SgrPeerPlan);
         default: return 0;
     }
 }

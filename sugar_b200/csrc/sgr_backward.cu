@@ -13,8 +13,6 @@
 // splats at a time in a transposed pass and issues two 16-byte vector reductions
 // (red.global.add.v4.f32 -> SASS REDG.E.ADD.F32x4) plus one scalar per (8x4 block, Gaussian): 3 L2
 // operations instead of 9 per (pixel, Gaussian).
-#include <mutex>
-
 #include "sgr_internal.cuh"
 #include "sgr_sh.cuh"
 
@@ -500,7 +498,6 @@ __device__ __forceinline__ void sh_grad_row(int deg, int M, float *dc, float *re
 }
 
 constexpr int PB_VB = 7;  // other views whose factors a thread fetches at the top of the kernel (8 ranks: all of them)
-constexpr int PB_T = 64;
 static_assert(PB_T == 64, "the peer record exchange (sgr_peer.cu) works in blocks of 64 records");
 // dynamic shared memory carve-up (floats): inputs, outputs, then the SH block
 constexpr int PB_GACC = 0;                     // PB_T*8
@@ -921,219 +918,6 @@ __global__ void __launch_bounds__(PB_T) preprocess_backward_kernel(const PreBwdA
     if (out_bulk && tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-// ------------------------------------------------------------------------------------------------
-// View-parallel epilogue (one thread per Gaussian of a chunk), after the exchange:
-//  * dL_dsh from the views' factors: dL_dsh[i] = sum_v basis(normalize(mean_i - campos_v)) (x) dRGB_v[i]
-//    (the SH part of backward.cu:20-139 is an outer product per view).  The 3*M accumulators stay in
-//    registers over the views and the rows leave through shared memory as coalesced stores.
-//  * the all-reduced 44-byte records (means3D 3 | opacity 1 | scales 3 | rotations 4) are split into
-//    the four gradient arrays autograd expects.
-// Either half is optional.
-// ------------------------------------------------------------------------------------------------
-// Where view v's factor block [P,3] starts: a slice of one gathered buffer (base + v * stride), or -- peer mode -- an
-// entry of a device-resident pointer table whose entries may point into OTHER GPUs' memory (CUDA IPC mappings over
-// NVLink): the all-gather is then fused into this kernel's loads and no gathered copy exists.
-__device__ __forceinline__ const float *view_block(const float *base, size_t stride, const float *const *tab, int v)
-{
-    return tab ? tab[v] : base + (size_t)v * stride;
-}
-
-constexpr int SF_T = 256;  // 64 Gaussians per CTA, four threads each
-constexpr int SF_VB = 4;  // views whose factors a thread fetches before it uses any
-
-// Four threads per Gaussian: thread q owns SH coefficients 4q .. 4q+3, i.e. 48 contiguous bytes of the row
-// (three 16-byte stores; the four threads of a Gaussian cover its 192-byte row, a warp 1.5 KB without gaps), and
-// evaluates only those four basis functions per view -- 12 accumulators instead of 48 per thread, no shared-memory
-// transpose, 4x the threads in flight.  Rows with M != 16 use the generic path below (one thread per Gaussian).
-// `view_stride` is the distance in floats between two views' factor blocks (>= 3P: the exchange appends each view's
-// camera position to its block); campos[v] may live there too.
-__global__ void __launch_bounds__(SF_T) view_grad_finalize_m16_kernel(int p0, int p1, int deg, int nviews,
-                                                                       const float *__restrict__ means,
-                                                                       const float *__restrict__ campos, int campos_stride,
-                                                                       const float *__restrict__ dRGB, size_t view_stride,
-                                                                       const float *const *__restrict__ view_tab,
-                                                                       size_t campos_off, float *__restrict__ dsh,
-                                                                       const float *__restrict__ rec11, float scale,
-                                                                       float *__restrict__ dmeans3D,
-                                                                       float *__restrict__ dopacity,
-                                                                       float *__restrict__ dscales, float *__restrict__ drots)
-{
-    const int t = blockIdx.x * SF_T + threadIdx.x;
-    const int i = p0 + (t >> 2), q = t & 3;
-    if (i >= p1) return;
-    // Every load of the thread is issued before its first store or use: the kernel is a latency chain per thread
-    // (records -> stores, mean + factors -> rows), and what hides DRAM latency here is bytes in flight per thread.
-    float rv[4] = {0.f, 0.f, 0.f, 0.f};
-    if (rec11 && q < 3) {
-        // the 11 reduced floats of a Gaussian, split over its four threads: means3D | opacity + scales | rotations
-        const float *r = rec11 + (size_t)i * 11 + (q == 0 ? 0 : q == 1 ? 3 : 7);
-        rv[0] = __ldcs(r);
-        rv[1] = __ldcs(r + 1);
-        rv[2] = __ldcs(r + 2);
-        if (q) rv[3] = __ldcs(r + 3);
-    }
-    float mx = 0.f, my = 0.f, mz = 0.f;
-    float gv[SF_VB][3];
-    if (dsh) {
-        mx = __ldg(means + 3 * (size_t)i);
-        my = __ldg(means + 3 * (size_t)i + 1);
-        mz = __ldg(means + 3 * (size_t)i + 2);
-#pragma unroll
-        for (int u = 0; u < SF_VB; u++) {
-            const bool on = u < nviews;
-            const float *g = view_block(dRGB, view_stride, view_tab, on ? u : 0) + (size_t)i * 3;
-            gv[u][0] = on ? __ldcs(g) : 0.f;
-            gv[u][1] = on ? __ldcs(g + 1) : 0.f;
-            gv[u][2] = on ? __ldcs(g + 2) : 0.f;
-        }
-    }
-    if (rec11) {
-        if (q == 0) {
-            __stcs(dmeans3D + 3 * (size_t)i, rv[0] * scale);
-            __stcs(dmeans3D + 3 * (size_t)i + 1, rv[1] * scale);
-            __stcs(dmeans3D + 3 * (size_t)i + 2, rv[2] * scale);
-        } else if (q == 1) {
-            __stcs(dopacity + i, rv[0] * scale);
-            __stcs(dscales + 3 * (size_t)i, rv[1] * scale);
-            __stcs(dscales + 3 * (size_t)i + 1, rv[2] * scale);
-            __stcs(dscales + 3 * (size_t)i + 2, rv[3] * scale);
-        } else if (q == 2) {
-            __stcs((float4 *)(drots + 4 * (size_t)i), make_float4(rv[0] * scale, rv[1] * scale, rv[2] * scale, rv[3] * scale));
-        }
-    }
-    if (!dsh) return;
-    const int used = (deg + 1) * (deg + 1);
-    float acc[4][3];
-#pragma unroll
-    for (int k = 0; k < 4; k++) acc[k][0] = acc[k][1] = acc[k][2] = 0.f;
-    // The views' factors are independent 12-byte reads 3P floats apart: a thread fetches SF_VB views' worth at a time
-    // (the first batch above, with everything else), so 8 views cost 2 dependent DRAM round trips, not 8.
-    for (int v0 = 0; v0 < nviews; v0 += SF_VB) {
-        if (v0) {
-#pragma unroll
-            for (int u = 0; u < SF_VB; u++) {
-                const bool on = v0 + u < nviews;
-                const float *g = view_block(dRGB, view_stride, view_tab, on ? v0 + u : v0) + (size_t)i * 3;
-                gv[u][0] = on ? __ldcs(g) : 0.f;
-                gv[u][1] = on ? __ldcs(g + 1) : 0.f;
-                gv[u][2] = on ? __ldcs(g + 2) : 0.f;
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < SF_VB; u++) {
-            const float gr = gv[u][0] * scale, gg = gv[u][1] * scale, gb = gv[u][2] * scale;
-            if (gr == 0.f && gg == 0.f && gb == 0.f) continue;  // not visible in this view (or past the last view)
-            const float *cp = view_tab ? view_tab[v0 + u] + campos_off : campos + (size_t)(v0 + u) * campos_stride;
-            const f3 d = sh_dir(mx, my, mz, __ldg(cp), __ldg(cp + 1), __ldg(cp + 2));
-            float w[4] = {0.f, 0.f, 0.f, 0.f};  // basis functions 4q .. 4q + 3, zero at and above (deg + 1)^2
-            auto quad = [&](auto q4) {
-                constexpr int K0 = 4 * decltype(q4)::value;
-                sh_for<K0, K0 + 4>([&](auto k) {
-                    constexpr int K = decltype(k)::value;
-                    if (K < used) w[K - K0] = sh_basis<K>(d);
-                });
-            };
-            if (q == 0) quad(std::integral_constant<int, 0>{});
-            else if (q == 1) quad(std::integral_constant<int, 1>{});
-            else if (q == 2) quad(std::integral_constant<int, 2>{});
-            else quad(std::integral_constant<int, 3>{});
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                acc[k][0] = fmaf(w[k], gr, acc[k][0]);
-                acc[k][1] = fmaf(w[k], gg, acc[k][1]);
-                acc[k][2] = fmaf(w[k], gb, acc[k][2]);
-            }
-        }
-    }
-    // written once, 576 MB per backward at 3M Gaussians: streaming stores keep them from displacing the L2's contents
-    float4 *dst = (float4 *)(dsh + (size_t)i * 48 + q * 12);
-    __stcs(dst, make_float4(acc[0][0], acc[0][1], acc[0][2], acc[1][0]));
-    __stcs(dst + 1, make_float4(acc[1][1], acc[1][2], acc[2][0], acc[2][1]));
-    __stcs(dst + 2, make_float4(acc[2][2], acc[3][0], acc[3][1], acc[3][2]));
-}
-
-constexpr int SFG_T = 128;
-
-__global__ void __launch_bounds__(SFG_T) view_grad_finalize_kernel(int p0, int p1, int P, int M, int deg, int nviews,
-                                                                   const float *__restrict__ means,
-                                                                   const float *__restrict__ campos, int campos_stride,
-                                                                   const float *__restrict__ dRGB, size_t view_stride,
-                                                                   const float *const *__restrict__ view_tab,
-                                                                   size_t campos_off, float *__restrict__ dsh,
-                                                                   const float *__restrict__ rec11, float scale,
-                                                                   float *__restrict__ dmeans3D, float *__restrict__ dopacity,
-                                                                   float *__restrict__ dscales, float *__restrict__ drots)
-{
-    extern __shared__ __align__(16) float s_rows[];  // SFG_T rows x stride floats (SH half only)
-    const int tid = threadIdx.x, base = p0 + blockIdx.x * SFG_T, i = base + tid;
-    const int n = min(SFG_T, p1 - base);
-    if (rec11 && tid < n) {
-        const float *r = rec11 + (size_t)i * 11;
-        float v[11];
-#pragma unroll
-        for (int k = 0; k < 11; k++) v[k] = r[k] * scale;
-        dmeans3D[3 * (size_t)i] = v[0];
-        dmeans3D[3 * (size_t)i + 1] = v[1];
-        dmeans3D[3 * (size_t)i + 2] = v[2];
-        dopacity[i] = v[3];
-        dscales[3 * (size_t)i] = v[4];
-        dscales[3 * (size_t)i + 1] = v[5];
-        dscales[3 * (size_t)i + 2] = v[6];
-        drots[4 * (size_t)i] = v[7];
-        drots[4 * (size_t)i + 1] = v[8];
-        drots[4 * (size_t)i + 2] = v[9];
-        drots[4 * (size_t)i + 3] = v[10];
-    }
-    if (!dsh) return;
-    const int row_f = M * 3;
-    int vec;
-    const int stride = sh_row_stride(M, false, &vec);
-    float acc[48];
-#pragma unroll
-    for (int k = 0; k < 48; k++) acc[k] = 0.f;
-    if (tid < n) {
-        const float mx = means[3 * (size_t)i], my = means[3 * (size_t)i + 1], mz = means[3 * (size_t)i + 2];
-        for (int v = 0; v < nviews; v++) {
-            const float *g = view_block(dRGB, view_stride, view_tab, v) + (size_t)i * 3;
-            const float gr = g[0] * scale, gg = g[1] * scale, gb = g[2] * scale;
-            if (gr == 0.f && gg == 0.f && gb == 0.f) continue;  // not visible in this view
-            const float *cp = view_tab ? view_tab[v] + campos_off : campos + (size_t)v * campos_stride;
-            sh_accumulate(deg, acc, sh_dir(mx, my, mz, cp[0], cp[1], cp[2]), {gr, gg, gb});
-        }
-        float *row = s_rows + tid * stride;
-#pragma unroll
-        for (int k = 0; k < 48; k++)
-            if (k < row_f) row[k] = acc[k];
-        for (int k = 48; k < row_f; k++) row[k] = 0.f;
-    }
-    __syncthreads();
-    float *dst = dsh + (size_t)base * row_f;
-    sh_rows_walk<SFG_T, 1>(n, row_f, stride, [&](int g, int s) { dst[g] = s_rows[s]; });
-}
-
-static int finalize_impl(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree, int32_t num_views,
-                         const float *means3D, const float *campos, const float *dRGB, int64_t view_stride,
-                         int32_t campos_stride, const float *const *view_tab, float *dL_dsh, const float *reduced_records,
-                         float scale, float *dL_dmeans3D, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
-                         void *stream, const char *who);
-
-// CTA range [b0, b1) of chunk c of the per-Gaussian pass.  taper == 0: equal chunks.  taper != 0: every chunk half the size
-// of the one before it (weights 2^(n-1-c)), so that what a caller does with a finished chunk while the next one is
-// computed (the peer exchange: reduce + split) is matched by that next chunk's shorter run, and little is left after the
-// last, smallest chunk.
-static void chunk_blocks(int blocks, int nchunks, int c, int taper, int *b0, int *b1)
-{
-    if (!taper || nchunks > 30) {
-        *b0 = (int)((int64_t)blocks * c / nchunks);
-        *b1 = (int)((int64_t)blocks * (c + 1) / nchunks);
-        return;
-    }
-    const int64_t full = ((int64_t)1 << nchunks) - 1;
-    auto edge = [&](int k) { return (int)((int64_t)blocks * ((((int64_t)1 << nchunks) - ((int64_t)1 << (nchunks - k)))) / full); };
-    *b0 = edge(c);
-    *b1 = c + 1 == nchunks ? blocks : edge(c + 1);
-}
-
 static int set_backward_attributes()
 {
     SGR_CUDA(cudaFuncSetAttribute(blend_backward_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1153,26 +937,6 @@ static int set_backward_attributes()
     return SGR_OK;
 }
 static DeviceOnce g_backward_attributes;
-
-// The events that order the peer exchange's launches on the plan's signal stream (side = 0) and side stream (side = 1)
-// behind earlier work, per device and launch index, created on first use and kept.
-static int peer_event(int side, int index, cudaEvent_t *out)
-{
-    static std::mutex mu;
-    static cudaEvent_t evs[SGR_MAX_DEVICES][2][20] = {};
-    int dev = 0;
-    const int rc = current_device(&dev);
-    if (rc) return rc;
-    if (index < 0 || index >= 20) {
-        set_error("%s: chunk index out of range", side ? "peer_side_stream" : "peer_signal_stream");
-        return SGR_EINVAL;
-    }
-    std::lock_guard<std::mutex> lock(mu);
-    cudaEvent_t *ev = &evs[dev][side][index];
-    if (!*ev) SGR_CUDA(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
-    *out = *ev;
-    return SGR_OK;
-}
 
 static void launch_blend_backward(const ViewConsts &v, int P, const ImageState &img, const BinState &bin,
                                   const GeomState &geom, const float *dL_dout_color, float *gacc, float *dL_dcolors,
@@ -1202,6 +966,10 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     const SgrStageHook hook = plan ? plan->hook : nullptr;
     void *hook_ctx = plan ? plan->hook_ctx : nullptr;
     float *rec11 = plan ? plan->reduce_records : nullptr;
+    // the peer exchange (SgrPeerPlan); MULTI: the pass sums every rank's SH gradient into dL_dsh, see PreBwdArgs::view_tab
+    const SgrPeerPlan *pp = plan ? plan->peer : nullptr;
+    const bool multi = pp && pp->peer_view_blocks && dL_dsh && g->shs;
+    PeerBackward peer{pp, st, P, dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations};
     const ViewConsts v = view_consts(view, g->M);
     int rc = once_per_device(g_backward_attributes, set_backward_attributes);
     if (rc) return rc;
@@ -1213,37 +981,8 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
         SGR_LAUNCH(K_BLEND_BWD, st, launch_blend_backward(v, P, img, bin, geom, dL_dout_color, gacc, dL_dcolors, feat, st));
     // dL_dcolors is final here (with SH colours: the clamp-masked dL/dRGB, i.e. this view's SH factor)
     if (hook) hook(hook_ctx, SGR_STAGE_BLEND_DONE);
-    const bool peer = plan && plan->peer_flag_tab;
-    // this backward's own signals: on `st`, or on the plan's signal stream behind an event recorded on `st` (so that the
-    // next kernel on `st` does not queue behind the signal's launch)
-    auto signal = [&](int slot, int ev_index, bool on_main = false) -> int {
-        cudaStream_t sig = st;
-        if (plan->peer_signal_stream && !on_main) {
-            cudaEvent_t ev = nullptr;
-            const int rc = peer_event(0, ev_index, &ev);
-            if (rc) return rc;
-            sig = (cudaStream_t)plan->peer_signal_stream;
-            SGR_CUDA(cudaEventRecord(ev, st));
-            SGR_CUDA(cudaStreamWaitEvent(sig, ev, 0));
-        }
-        return sgr_peer_signal(plan->peer_flag_tab, plan->peer_nranks, slot, plan->peer_rank, plan->peer_seq, sig);
-    };
-    if (peer) {
-        // BLEND goes out on `st` itself: the wait right behind it spins, and a spinning kernel must never be dispatched
-        // ahead of a signal of its own rank that the peers need in order to answer
-        rc = signal(plan->peer_slot_blend, 0, true);
-        if (rc) return rc;
-        if (plan->peer_view_blocks && dL_dsh && g->shs) {
-            // the per-Gaussian pass sums every view's SH gradient into dL_dsh: the peers' factor blocks must be final
-            if (g->activations != 0 || !plan->peer_flags) {
-                set_error("peer_view_blocks: needs peer_flags and activated (not raw) parameters");
-                return SGR_EINVAL;
-            }
-            rc = sgr_peer_wait(plan->peer_flags, plan->peer_nranks, plan->peer_slot_blend, 1, plan->peer_seq,
-                               plan->peer_timeout_s, st);
-            if (rc) return rc;
-        }
-    }
+    rc = peer.blend_done(multi);
+    if (rc) return rc;
     PreBwdArgs a;
     a.means = g->means3D;
     a.scales = g->scales;
@@ -1263,31 +1002,15 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     a.dscales = dL_dscales;
     a.drots = dL_drotations;
     a.rec11 = rec11;
-    a.view_tab = nullptr;
-    a.stage_tab = nullptr;
-    a.pf_off = 0;
-    a.nviews = 1;
-    a.my_view = 0;
+    a.view_tab = multi ? (const float *const *)pp->peer_view_blocks : nullptr;
+    a.stage_tab = multi ? (float *const *)pp->peer_record_stages : nullptr;
+    a.nviews = multi ? pp->peer_nranks : 1;
+    a.my_view = multi ? pp->peer_rank : 0;
     a.campos_off = (size_t)3 * P;
-    a.dsh_scale = 1.0f;
+    a.dsh_scale = multi ? pp->peer_dsh_scale : 1.0f;
     const bool raw = g->activations != 0;
-    if (peer && plan->peer_view_blocks && dL_dsh && g->shs) {
-        a.view_tab = (const float *const *)plan->peer_view_blocks;
-        a.nviews = plan->peer_nranks;
-        a.my_view = plan->peer_rank;
-        a.dsh_scale = plan->peer_dsh_scale;
-        a.stage_tab = (float *const *)plan->peer_record_stages;
-        if (a.stage_tab && !rec11) {
-            set_error("peer_record_stages needs reduce_records (the local staging array)");
-            return SGR_EINVAL;
-        }
-    }
     a.rec = geom.rec;
     a.dsh_rest = plan ? plan->dL_dsh_rest : nullptr;
-    if (raw && g->shs && dL_dsh && g->M > 1 && !a.dsh_rest) {
-        set_error("raw-parameter mode needs SgrBackwardPlan.dL_dsh_rest");
-        return SGR_EINVAL;
-    }
     // (the SH arrays are not read; sh_jac is 256-byte aligned by GeomState::carve)
     a.in_bulk_ok = aligned16(gacc) && aligned16(dL_dcolors) && aligned16(g->means3D) &&
                    (!g->scales || aligned16(g->scales)) && (!g->rotations || aligned16(g->rotations)) &&
@@ -1309,27 +1032,10 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
     const size_t dyn = (size_t)(a.pf_off + pulled * PB_T * 3) * sizeof(float) + 16;
     // the per-Gaussian pass, in `num_chunks` Gaussian ranges (multiples of the CTA size) so that a caller
     // can start reducing a finished range while the next one is computed
-    int nchunks = plan && plan->num_chunks > 1 ? plan->num_chunks : 1;
+    const int nchunks = backward_chunks(P, plan ? plan->num_chunks : 1);
     const int blocks = (P + PB_T - 1) / PB_T;
-    if (nchunks > blocks) nchunks = blocks;
-    int split_c = -1, split_p0 = 0, split_p1 = 0;
     const auto preprocess = raw ? &preprocess_backward_kernel<true>
                                 : a.view_tab ? &preprocess_backward_kernel<false, true> : &preprocess_backward_kernel<false>;
-    auto split_chunk = [&](cudaStream_t B, int c, int p0, int p1) -> int {
-        int rc = sgr_peer_wait(plan->peer_flags, plan->peer_nranks, plan->peer_slot_reduced0 + c, 1, plan->peer_seq,
-                               plan->peer_timeout_s, B);
-        if (rc) return rc;
-        return finalize_impl(P, p0, p1, g->M, view->sh_degree, plan->peer_nranks, g->means3D, nullptr, nullptr, 0, 0, nullptr,
-                             nullptr, plan->peer_sums, plan->peer_dsh_scale, dL_dmeans3D, dL_dopacity, dL_dscales,
-                             dL_drotations, B, "peer exchange: bad arguments to the record split");
-    };
-    if (peer && plan->peer_side_stream &&
-        (!plan->peer_rec_tab || !plan->peer_sum_tab || !plan->peer_sums || !plan->peer_flags || !rec11 || !dL_dmeans3D ||
-         !dL_dopacity || !dL_dscales || !dL_drotations || nchunks > 16)) {
-        set_error("peer_side_stream needs peer_rec_tab / peer_sum_tab / peer_sums / peer_flags, reduce_records, the four "
-                  "record-bound gradient arrays and at most 16 chunks");
-        return SGR_EINVAL;
-    }
     for (int c = 0; c < nchunks; c++) {
         int b0, b1;
         chunk_blocks(blocks, nchunks, c, plan ? plan->chunk_taper : 0, &b0, &b1);
@@ -1337,155 +1043,14 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
         a.p1 = min(P, b1 * PB_T);
         if (b1 > b0) SGR_LAUNCH(K_PRE_BWD, st, preprocess<<<b1 - b0, PB_T, dyn, st>>>(a));
         if (hook) hook(hook_ctx, SGR_STAGE_CHUNK_DONE + c);
-        if (peer) {
-            int rc = signal(plan->peer_slot_chunk0 + c, 1 + c);
-            if (rc) return rc;
-            if (plan->peer_side_stream) {
-                // The records' exchange of this chunk, on the side stream.  Its kernels spin on flags: they may start
-                // only once THIS rank's own signal for the chunk is out (an event behind the signal kernel) -- a
-                // spinning kernel must never sit in front of a signal some rank is waiting for.
-                cudaStream_t B = (cudaStream_t)plan->peer_side_stream;
-                cudaStream_t sig = plan->peer_signal_stream ? (cudaStream_t)plan->peer_signal_stream : st;
-                cudaEvent_t e2 = nullptr;
-                rc = peer_event(1, c, &e2);
-                if (rc) return rc;
-                SGR_CUDA(cudaEventRecord(e2, sig));
-                SGR_CUDA(cudaStreamWaitEvent(B, e2, 0));
-                unsigned int *counters = (unsigned int *)plan->peer_flags + (size_t)(SGR_PEER_MAX_SLOTS - 1) * SGR_PEER_MAX_RANKS;
-                for (int r = 0; r < plan->peer_nranks; r++) {
-                    const bool me = r == plan->peer_rank;
-                    if (!me && !((plan->peer_emulate_ranks >> r) & 1)) continue;
-                    // one kernel: wait(CHUNK c, every rank) -> sum the owned slice -> its last CTA signals REDUCED c
-                    rc = sgr_peer_reduce_records_synced(plan->peer_rec_tab, plan->peer_sum_tab, plan->peer_nranks, r, a.p0, a.p1,
-                                                        plan->peer_flags, plan->peer_slot_chunk0 + c,
-                                                        me ? plan->peer_flag_tab : nullptr, plan->peer_slot_reduced0 + c,
-                                                        plan->peer_seq, me ? (void *)(counters + c) : nullptr,
-                                                        plan->peer_timeout_s, B);
-                    if (rc) return rc;
-                }
-                // the split of the chunk before runs behind this chunk's reduce: the other owners' slices of it have
-                // landed by then, and only the last (smallest) chunk's reduce + split is exposed
-                if (split_c >= 0) {
-                    rc = split_chunk(B, split_c, split_p0, split_p1);
-                    if (rc) return rc;
-                }
-                split_c = c;
-                split_p0 = a.p0;
-                split_p1 = a.p1;
-            }
-        }
-    }
-    if (peer && plan->peer_side_stream && split_c >= 0) {
-        const int rc = split_chunk((cudaStream_t)plan->peer_side_stream, split_c, split_p0, split_p1);
+        rc = peer.chunk_done(c, a.p0, a.p1);
         if (rc) return rc;
     }
+    rc = peer.finish();
+    if (rc) return rc;
     SGR_CUDA(cudaGetLastError());
     if (view->debug) SGR_CUDA(cudaStreamSynchronize(st));
     return SGR_OK;
 }
 
 }  // namespace sgr
-
-extern "C" int sgr_backward_chunk_range_tapered(int32_t P, int32_t num_chunks, int32_t chunk, int32_t taper, int32_t *p0,
-                                                int32_t *p1)
-{
-    using namespace sgr;
-    if (P < 0 || num_chunks < 1 || chunk < 0 || chunk >= num_chunks || !p0 || !p1) {
-        set_error("bad arguments to sgr_backward_chunk_range");
-        return SGR_EINVAL;
-    }
-    const int blocks = (P + PB_T - 1) / PB_T;
-    const int nchunks = num_chunks > blocks ? (blocks > 0 ? blocks : 1) : num_chunks;
-    if (chunk >= nchunks) {
-        *p0 = *p1 = P;
-        return SGR_OK;
-    }
-    int b0, b1;
-    chunk_blocks(blocks, nchunks, chunk, taper, &b0, &b1);
-    *p0 = b0 * PB_T;
-    *p1 = b1 * PB_T;
-    if (*p1 > P) *p1 = P;
-    if (*p0 > P) *p0 = P;
-    return SGR_OK;
-}
-
-extern "C" int sgr_backward_chunk_range(int32_t P, int32_t num_chunks, int32_t chunk, int32_t *p0, int32_t *p1)
-{
-    return sgr_backward_chunk_range_tapered(P, num_chunks, chunk, 0, p0, p1);
-}
-
-namespace sgr {
-static int finalize_impl(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree, int32_t num_views,
-                         const float *means3D, const float *campos, const float *dRGB, int64_t view_stride,
-                         int32_t campos_stride, const float *const *view_tab, float *dL_dsh, const float *reduced_records,
-                         float scale, float *dL_dmeans3D, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
-                         void *stream, const char *who)
-{
-    const bool sh = dL_dsh != nullptr, rec = reduced_records != nullptr;
-    const bool src_ok = view_tab ? true : (campos && dRGB && view_stride >= (int64_t)3 * P && campos_stride >= 3);
-    if (P < 0 || p0 < 0 || p1 < p0 || p1 > P || (!sh && !rec) ||
-        (sh && (M <= 0 || sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > M || num_views <= 0 ||
-                !means3D || !src_ok)) ||
-        (rec && (!dL_dmeans3D || !dL_dopacity || !dL_dscales || !dL_drotations))) {
-        set_error(who);
-        return SGR_EINVAL;
-    }
-    if (p1 == p0) return SGR_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t campos_off = (size_t)3 * P;  // peer mode: a view's camera position follows its [P,3] factors
-    const bool al16 = (((uintptr_t)dL_dsh | (uintptr_t)dL_drotations) & 15u) == 0;
-    if ((!sh || M == 16) && al16) {
-        const int threads = (p1 - p0) * 4;
-        SGR_LAUNCH(K_FINALIZE, st,
-                   view_grad_finalize_m16_kernel<<<(threads + SF_T - 1) / SF_T, SF_T, 0, st>>>(
-                       p0, p1, sh_degree, num_views, means3D, campos, campos_stride, dRGB, (size_t)view_stride, view_tab,
-                       campos_off, dL_dsh, reduced_records, scale, dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations));
-    } else {
-        int vec;
-        const size_t dyn = sh ? (size_t)SFG_T * sh_row_stride(M, false, &vec) * sizeof(float) : 0;
-        SGR_LAUNCH(K_FINALIZE, st,
-                   view_grad_finalize_kernel<<<(p1 - p0 + SFG_T - 1) / SFG_T, SFG_T, dyn, st>>>(
-                       p0, p1, P, M, sh_degree, num_views, means3D, campos, campos_stride, dRGB, (size_t)view_stride,
-                       view_tab, campos_off, dL_dsh, reduced_records, scale, dL_dmeans3D, dL_dopacity, dL_dscales,
-                       dL_drotations));
-    }
-    SGR_CUDA(cudaGetLastError());
-    return SGR_OK;
-}
-}  // namespace sgr
-
-extern "C" int sgr_view_grad_finalize(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree, int32_t num_views,
-                                      const float *means3D, const float *campos, const float *dRGB, int64_t view_stride,
-                                      int32_t campos_stride, float *dL_dsh, const float *reduced_records, float scale,
-                                      float *dL_dmeans3D, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
-                                      void *stream)
-{
-    return sgr::finalize_impl(P, p0, p1, M, sh_degree, num_views, means3D, campos, dRGB, view_stride, campos_stride, nullptr,
-                              dL_dsh, reduced_records, scale, dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations, stream,
-                              "bad arguments to sgr_view_grad_finalize");
-}
-
-extern "C" int sgr_view_grad_finalize_peers(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree,
-                                            int32_t num_views, const float *means3D, const float *const *view_blocks,
-                                            float *dL_dsh, const float *reduced_records, float scale, float *dL_dmeans3D,
-                                            float *dL_dopacity, float *dL_dscales, float *dL_drotations, void *stream)
-{
-    if (dL_dsh && !view_blocks) {
-        sgr::set_error("bad arguments to sgr_view_grad_finalize_peers");
-        return SGR_EINVAL;
-    }
-    return sgr::finalize_impl(P, p0, p1, M, sh_degree, num_views, means3D, nullptr, nullptr, 0, 0, view_blocks, dL_dsh,
-                              reduced_records, scale, dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations, stream,
-                              "bad arguments to sgr_view_grad_finalize_peers");
-}
-
-extern "C" int sgr_sh_grad_from_factors(int32_t P, int32_t M, int32_t sh_degree, int32_t num_views, const float *means3D,
-                                        const float *campos, const float *dRGB, float *dL_dsh, void *stream)
-{
-    if (!dL_dsh && P > 0) {
-        sgr::set_error("bad arguments to sgr_sh_grad_from_factors");
-        return SGR_EINVAL;
-    }
-    return sgr_view_grad_finalize(P, 0, P, M, sh_degree, num_views, means3D, campos, dRGB, (int64_t)3 * P, 3, dL_dsh, nullptr,
-                                  1.0f, nullptr, nullptr, nullptr, nullptr, stream);
-}

@@ -556,6 +556,36 @@ int launch_backward(const SgrView *view, const SgrGaussians *g, const int32_t *r
                     const float *dL_dout_color, float *dL_dmeans2D, float *dL_dcolors, float *dL_dopacity,
                     float *dL_dmeans3D, float *dL_dcov3D, float *dL_dsh, float *dL_dscales, float *dL_drotations,
                     void *grad_scratch, cudaStream_t stream, const SgrBackwardPlan *plan, const FeatureChannel *feat);
+
+// The per-Gaussian backward pass: PB_T Gaussians per CTA, in backward_chunks() chunks of whole CTAs (at least one, at
+// most one per CTA); chunk c covers the CTAs [b0, b1) (sgr_exchange.cu).
+constexpr int PB_T = 64;
+static inline int backward_chunks(int P, int num_chunks)
+{
+    const int n = num_chunks > 1 ? num_chunks : 1, blocks = (P + PB_T - 1) / PB_T;
+    return n > blocks ? blocks : n;
+}
+void chunk_blocks(int blocks, int nchunks, int c, int taper, int *b0, int *b1);
+
+// sgr_view_grad_finalize for the Gaussians [p0, p1) (sgr_exchange.cu); `who`: the message for bad arguments
+int finalize_impl(int32_t P, int32_t p0, int32_t p1, int32_t M, int32_t sh_degree, int32_t num_views,
+                  const float *means3D, const float *campos, const float *dRGB, int64_t view_stride, int32_t campos_stride,
+                  float *dL_dsh, const float *reduced_records, float scale, float *dL_dmeans3D, float *dL_dopacity,
+                  float *dL_dscales, float *dL_drotations, void *stream, const char *who);
+
+// The peer exchange's share of one backward (sgr_peer.cu), called by launch_backward next to the stage hook; with
+// plan == NULL nothing is enqueued.  rasterize_backward has checked the plan.
+struct PeerBackward {
+    const SgrPeerPlan *plan;
+    cudaStream_t st;
+    int P;
+    float *dmeans3D, *dopacity, *dscales, *drots;  // where the split puts the reduced records
+    int split_c = -1, split_p0 = 0, split_p1 = 0;  // the chunk whose split is still to be enqueued
+    int blend_done(bool views);             // signal BLEND; views (MULTI): wait until every rank has
+    int chunk_done(int c, int p0, int p1);  // signal CHUNK c; side stream: reduce chunk c, split chunk c - 1
+    int finish();                           // side stream: split the last chunk
+};
+
 // The reference's full per-tile list (dead instances included) of a forward's state, into `full`; `cursor`: T words
 int build_full_list(int P, int W, int H, const GeomState &geom, const ImageState &img, uint64_t num_rendered,
                     const BinState &full, uint32_t *cursor, cudaStream_t stream);

@@ -24,6 +24,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <mutex>
+
 #include "sgr_internal.cuh"
 
 namespace sgr {
@@ -304,7 +306,7 @@ int sgr_peer_reduce_records_synced(const void *const *rec_tab, void *const *sum_
     if (!rec_tab || !sum_tab || nranks < 1 || nranks > PEER_RANKS || my_rank < 0 || my_rank >= nranks || p0 < 0 ||
         p1 < p0 || (p0 & 63) || (flags && (wait_slot < 0 || wait_slot >= PEER_SLOTS)) ||
         (flag_tab && (signal_slot < 0 || signal_slot >= PEER_SLOTS || !counter))) {
-        set_error("bad arguments to sgr_peer_reduce_records (p0 must be a multiple of 64)");
+        set_error("bad arguments to sgr_peer_reduce_records_synced (p0 must be a multiple of 64)");
         return SGR_EINVAL;
     }
     // ownership follows the per-Gaussian pass (PreBwdArgs::stage_tab): block b of the chunk's nb 64-record blocks belongs
@@ -346,11 +348,109 @@ int sgr_peer_reduce_records_synced(const void *const *rec_tab, void *const *sum_
     return SGR_OK;
 }
 
-int sgr_peer_reduce_records(const void *const *rec_tab, void *const *sum_tab, int32_t nranks, int32_t my_rank, int32_t p0,
-                            int32_t p1, void *stream)
+}  // extern "C"
+
+namespace sgr {
+
+// The events that order the exchange's launches on the plan's signal stream (side = 0) and side stream (side = 1)
+// behind earlier work, per device and launch index (< 20: rasterize_backward bounds the chunks), kept once created.
+static int peer_event(int side, int index, cudaEvent_t *out)
 {
-    return sgr_peer_reduce_records_synced(rec_tab, sum_tab, nranks, my_rank, p0, p1, nullptr, 0, nullptr, 0, 0, nullptr, 0.0,
-                                          stream);
+    static std::mutex mu;
+    static cudaEvent_t evs[SGR_MAX_DEVICES][2][20] = {};
+    int dev = 0;
+    const int rc = current_device(&dev);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lock(mu);
+    cudaEvent_t *ev = &evs[dev][side][index];
+    if (!*ev) SGR_CUDA(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    *out = *ev;
+    return SGR_OK;
 }
 
-}  // extern "C"
+// This backward's own signals: on `st`, or on the plan's signal stream behind an event recorded on `st` (so that the
+// next kernel on `st` does not queue behind the signal's launch).
+static int signal(const SgrPeerPlan *pp, cudaStream_t st, int slot, int ev_index, bool on_main = false)
+{
+    cudaStream_t sig = st;
+    if (pp->peer_signal_stream && !on_main) {
+        cudaEvent_t ev = nullptr;
+        const int rc = peer_event(0, ev_index, &ev);
+        if (rc) return rc;
+        sig = (cudaStream_t)pp->peer_signal_stream;
+        SGR_CUDA(cudaEventRecord(ev, st));
+        SGR_CUDA(cudaStreamWaitEvent(sig, ev, 0));
+    }
+    return sgr_peer_signal(pp->peer_flag_tab, pp->peer_nranks, slot, pp->peer_rank, pp->peer_seq, sig);
+}
+
+// On the side stream: wait for every rank's REDUCED c, then split the sums of [p0, p1) into the gradient arrays.
+static int split_chunk(const PeerBackward &b, int c, int p0, int p1)
+{
+    const SgrPeerPlan *pp = b.plan;
+    cudaStream_t B = (cudaStream_t)pp->peer_side_stream;
+    const int rc = sgr_peer_wait(pp->peer_flags, pp->peer_nranks, pp->peer_slot_reduced0 + c, 1, pp->peer_seq,
+                                 pp->peer_timeout_s, B);
+    if (rc) return rc;
+    return finalize_impl(b.P, p0, p1, 0, 0, pp->peer_nranks, nullptr, nullptr, nullptr, 0, 0, nullptr, pp->peer_sums,
+                         pp->peer_dsh_scale, b.dmeans3D, b.dopacity, b.dscales, b.drots, B,
+                         "peer exchange: bad arguments to the record split");
+}
+
+int PeerBackward::blend_done(bool views)
+{
+    if (!plan) return SGR_OK;
+    // BLEND goes out on `st` itself: the wait right behind it spins, and a spinning kernel must never be dispatched
+    // ahead of a signal of its own rank that the peers need in order to answer
+    int rc = signal(plan, st, plan->peer_slot_blend, 0, true);
+    if (rc || !views) return rc;
+    // the per-Gaussian pass sums every view's SH gradient into dL_dsh: the peers' factor blocks must be final
+    return sgr_peer_wait(plan->peer_flags, plan->peer_nranks, plan->peer_slot_blend, 1, plan->peer_seq,
+                         plan->peer_timeout_s, st);
+}
+
+int PeerBackward::chunk_done(int c, int p0, int p1)
+{
+    if (!plan) return SGR_OK;
+    int rc = signal(plan, st, plan->peer_slot_chunk0 + c, 1 + c);
+    if (rc || !plan->peer_side_stream) return rc;
+    // The records' exchange of this chunk, on the side stream.  Its kernels spin on flags: they may start only once
+    // THIS rank's own signal for the chunk is out (an event behind the signal kernel) -- a spinning kernel must never
+    // sit in front of a signal some rank is waiting for.
+    cudaStream_t B = (cudaStream_t)plan->peer_side_stream;
+    cudaStream_t sig = plan->peer_signal_stream ? (cudaStream_t)plan->peer_signal_stream : st;
+    cudaEvent_t e2 = nullptr;
+    rc = peer_event(1, c, &e2);
+    if (rc) return rc;
+    SGR_CUDA(cudaEventRecord(e2, sig));
+    SGR_CUDA(cudaStreamWaitEvent(B, e2, 0));
+    unsigned int *counters = (unsigned int *)plan->peer_flags + (size_t)(PEER_SLOTS - 1) * PEER_RANKS;
+    for (int r = 0; r < plan->peer_nranks; r++) {
+        const bool me = r == plan->peer_rank;
+        if (!me && !((plan->peer_emulate_ranks >> r) & 1)) continue;
+        // one kernel: wait(CHUNK c, every rank) -> sum the owned slice -> its last CTA signals REDUCED c
+        rc = sgr_peer_reduce_records_synced(plan->peer_rec_tab, plan->peer_sum_tab, plan->peer_nranks, r, p0, p1,
+                                            plan->peer_flags, plan->peer_slot_chunk0 + c, me ? plan->peer_flag_tab : nullptr,
+                                            plan->peer_slot_reduced0 + c, plan->peer_seq,
+                                            me ? (void *)(counters + c) : nullptr, plan->peer_timeout_s, B);
+        if (rc) return rc;
+    }
+    // the split of the chunk before runs behind this chunk's reduce: the other owners' slices of it have landed by
+    // then, and only the last (smallest) chunk's reduce + split is exposed
+    if (split_c >= 0) {
+        rc = split_chunk(*this, split_c, split_p0, split_p1);
+        if (rc) return rc;
+    }
+    split_c = c;
+    split_p0 = p0;
+    split_p1 = p1;
+    return SGR_OK;
+}
+
+int PeerBackward::finish()
+{
+    if (!plan || !plan->peer_side_stream || split_c < 0) return SGR_OK;
+    return split_chunk(*this, split_c, split_p0, split_p1);
+}
+
+}  // namespace sgr

@@ -304,9 +304,7 @@ class ViewParallel:
                 failure.append(e)
 
         cb = STAGE_HOOK(on_stage)
-        plan = SgrBackwardPlan(cb, None, nchunks, bufs["records"].data_ptr(), None)
-        plan.chunk_taper = taper
-        launch(plan)
+        launch(SgrBackwardPlan(hook=cb, num_chunks=nchunks, chunk_taper=taper, reduce_records=bufs["records"].data_ptr()))
         if failure:
             raise failure[0]
         main = torch.cuda.current_stream(dev)
@@ -367,7 +365,7 @@ class ViewParallel:
         return self._peer_states[key]
 
     def _run_backward_peer(self, st, launch, bufs, P, means3D, campos):
-        from ._lib import STAGE_HOOK, SgrBackwardPlan
+        from ._lib import SgrBackwardPlan, SgrPeerPlan
         dev = means3D.device
         world, rank = st.world, st.rank
         nchunks = max(1, self.chunks)
@@ -384,11 +382,14 @@ class ViewParallel:
         emulate = 0
         for r in self._emulated:
             emulate |= 1 << r
-        plan = SgrBackwardPlan(STAGE_HOOK(0), None, nchunks, st.R_ptr, None, st.flag_tab.data_ptr(), world, rank,
-                               _SLOT_BLEND, _SLOT_CHUNK0, seq, st.F_tab[par].data_ptr(), st.flags_ptr, self.scale,
-                               self.peer_timeout_s, taper, st.stage_tab.data_ptr(),
-                               Csig.cuda_stream, B.cuda_stream, st.rec_tab.data_ptr(),
-                               st.S_tab.data_ptr(), st.S_ptr, _SLOT_REDUCED0, emulate)
+        peer = SgrPeerPlan(peer_flag_tab=st.flag_tab.data_ptr(), peer_nranks=world, peer_rank=rank,
+                           peer_slot_blend=_SLOT_BLEND, peer_slot_chunk0=_SLOT_CHUNK0, peer_seq=seq,
+                           peer_view_blocks=st.F_tab[par].data_ptr(), peer_flags=st.flags_ptr, peer_dsh_scale=self.scale,
+                           peer_timeout_s=self.peer_timeout_s, peer_record_stages=st.stage_tab.data_ptr(),
+                           peer_signal_stream=Csig.cuda_stream, peer_side_stream=B.cuda_stream,
+                           peer_rec_tab=st.rec_tab.data_ptr(), peer_sum_tab=st.S_tab.data_ptr(), peer_sums=st.S_ptr,
+                           peer_slot_reduced0=_SLOT_REDUCED0, peer_emulate_ranks=emulate)
+        plan = SgrBackwardPlan(num_chunks=nchunks, chunk_taper=taper, reduce_records=st.R_ptr, peer=C.pointer(peer))
         # ... and on the side stream, also enqueued by the C call, chunk by chunk underneath the per-Gaussian pass of the
         # later chunks: [wait(CHUNK c, every rank) -> sum the slice this rank owns over the staging arrays (local loads)
         # -> store the sums into every rank's S (posted NVLink writes) -> signal(REDUCED c)] as ONE kernel, then behind
@@ -422,7 +423,7 @@ class ViewParallel:
     @staticmethod
     def _range(lib, check, P, nchunks, c, taper=0):
         p0, p1 = C.c_int32(0), C.c_int32(0)
-        check(lib.sgr_backward_chunk_range_tapered(P, nchunks, c, taper, C.byref(p0), C.byref(p1)))
+        check(lib.sgr_backward_chunk_range(P, nchunks, c, taper, C.byref(p0), C.byref(p1)))
         return p0.value, p1.value
 
 
@@ -435,8 +436,9 @@ def sh_grad_from_factors(means3D: torch.Tensor, campos_all: torch.Tensor, dRGB_a
         out = torch.empty((P, M, 3), dtype=torch.float32, device=means3D.device)
     assert out.is_contiguous() and out.numel() == P * M * 3 and dRGB_all.is_contiguous() and campos_all.is_contiguous()
     with torch.cuda.device(means3D.device):
-        check(lib.sgr_sh_grad_from_factors(P, M, sh_degree, V, means3D.contiguous().data_ptr(), campos_all.data_ptr(),
-                                           dRGB_all.data_ptr(), out.data_ptr(), stream(means3D.device)))
+        check(lib.sgr_view_grad_finalize(P, 0, P, M, sh_degree, V, means3D.contiguous().data_ptr(), campos_all.data_ptr(),
+                                         dRGB_all.data_ptr(), 3 * P, 3, out.data_ptr(), None, 1.0, None, None, None, None,
+                                         stream(means3D.device)))
     return out
 
 

@@ -102,7 +102,7 @@ def _backward(f, dL, dD=None, sh_rest=None):
                                                            dDt.data_ptr(), *grads, dval.data_ptr(),
                                                            b["scratch"].data_ptr(), stream))
     else:
-        plan = _lib.SgrBackwardPlan(_lib.STAGE_HOOK(0), None, 1, None, b["sh_rest"].data_ptr() if M > 1 else None) \
+        plan = _lib.SgrBackwardPlan(num_chunks=1, dL_dsh_rest=b["sh_rest"].data_ptr() if M > 1 else None) \
             if raw else None
         _lib.check(_lib.lib.sgr_rasterize_backward_staged(*inputs, *grads, b["scratch"].data_ptr(), stream,
                                                           None if plan is None else C.byref(plan)))

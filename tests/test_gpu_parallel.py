@@ -151,8 +151,8 @@ def test_sh_factors_rebuild_the_summed_dsh_with_nine_stored_coefficients():
 
 
 def check_sh_factors_rebuild(M, deg):
-    """sgr_sh_grad_from_factors on the gathered factors of several views == the sum of the views' dL_dsh; the
-    factor of a view is the dL_dcolors the backward returns with SH colours (clamp-masked dL/dRGB).  Also against
+    """sh_grad_from_factors (sgr_view_grad_finalize) on the gathered factors of several views == the sum of the views'
+    dL_dsh; the factor of a view is the dL_dcolors the backward returns with SH colours (clamp-masked dL/dRGB).  Also against
     sum_v basis(normalize(mean - campos_v)) (x) factor_v evaluated in float64.  On one view's factor alone it gives
     that view's dL_dsh exactly: the backward and the factor kernels evaluate the same basis at the same direction."""
     import torch

@@ -128,7 +128,7 @@ def test_exchange_policy_without_a_process_group(monkeypatch):
 
 def test_record_ownership_of_producer_and_reducer_agree():
     """Peer exchange: the per-Gaussian pass sends CTA b of a chunk's nb CTAs to rank  b * N // nb  (sgr_backward.cu,
-    PreBwdArgs::stage_tab); sgr_peer_reduce_records lets rank r sum the blocks [ceil(r nb / N), ceil((r + 1) nb / N))
+    PreBwdArgs::stage_tab); sgr_peer_reduce_records_synced lets rank r sum the blocks [ceil(r nb / N), ceil((r + 1) nb / N))
     (sgr_peer.cu).  Both are restated here: every block has exactly one owner and the two formulas name the same one."""
     for N in (1, 2, 3, 4, 7, 8, 16, 64):
         for nb in (1, 2, 3, 5, 8, 63, 64, 65, 1000, 11719, 46875):
