@@ -445,6 +445,16 @@ SGR_API int sgr_knn(int32_t P, const float *points, int32_t Q, const float *quer
                     float *dist2, void *workspace, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * distCUDA2 (simple-knn, called by GaussianModel.create_from_pcd, gaussian_model.py:134): per point of
+ * points f32[P,3], mean_dist2 f32[P] <- (b0 + b1 + b2) / 3 of its three smallest squared distances to OTHER points
+ * (by index: a duplicate position counts as 0), each distance rounded as the reference build rounds it, so the result
+ * is the reference's to the bit.  P <= 3 keeps the reference's FLT_MAX sentinels in the sum: inf for P <= 2,
+ * (b0 + b1 + FLT_MAX) / 3 for P = 3.  The search is sgr_knn's cell grid, so `workspace` is the same buffer:
+ * sgr_knn_workspace_bytes(P) bytes.  P = 0 does nothing.  No host synchronisation.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API int sgr_dist_cuda2(int32_t P, const float *points, float *mean_dist2, void *workspace, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Photometric loss of the trainers, (1 - f) * l1_loss + f * (1 - ssim) (sugar_utils/loss_utils.py:17-62, used as
  * sugar_trainers/coarse_sdf.py:101-103, 452-457): per image b of img1, img2 f32[B,C,H,W] (contiguous planes), the
  * mean over its C*H*W elements of |x - y| and of the SSIM map
@@ -684,6 +694,9 @@ SGR_API int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *vert
  *   except in SGR_DENSIFY_ZERO_NEW columns (zeros: Adam moments); a child's SGR_DENSIFY_POINTS value is
  *   R(q / |q|) (normal * exp(scale)) + point with normals f32[2S,3] (copy k of the split row of rank r reads row
  *   k*S + r; R as pytorch3d's quaternion_to_matrix) and its SGR_DENSIFY_SCALES value log(exp(scale) * inv_split).
+ *   An SGR_DENSIFY_POINTS_VANILLA column is the same with R = build_rotation(q) of vanilla 3DGS
+ *   (utils/general_utils.py:78-99: norm = sqrt(((r*r + x*x) + y*y) + z*z), q / norm, no epsilon, then its nine
+ *   entries as written).
  *   points / scales f32[P,3] and quaternions f32[P,4] (16-byte aligned) are the parents'.  src_row i32[P'] scratch.
  *   Pruning by a mask is the same call with only the keep row set.
  * ------------------------------------------------------------------------------------------ */
@@ -692,6 +705,7 @@ SGR_API int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *vert
 #define SGR_DENSIFY_ZERO_NEW 1  /* new rows are zero */
 #define SGR_DENSIFY_POINTS 2    /* children compute their position */
 #define SGR_DENSIFY_SCALES 3    /* children compute their log-scale */
+#define SGR_DENSIFY_POINTS_VANILLA 4 /* SGR_DENSIFY_POINTS with vanilla 3DGS's build_rotation for R */
 typedef struct SgrDensifyColumn {
     const float *src;
     float *dst;

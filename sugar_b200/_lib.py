@@ -130,6 +130,7 @@ PROTOTYPES = {
     "sgr_knn_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "sgr_knn": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                           C.c_void_p]),
+    "sgr_dist_cuda2": (C.c_int, [C.c_int32] + [C.c_void_p] * 4),
     "sgr_l1_ssim_scratch_bytes": (C.c_size_t, [C.c_int32] * 4),
     "sgr_l1_ssim_forward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 6),
     "sgr_l1_ssim_backward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 7),

@@ -14,7 +14,8 @@
 // densify_emit_kernel      one launch over every column, flattened [P' x width] per column so the stores are coalesced
 //                          whatever the row width (sh_rest rows are 180 B).  Rows tagged clone or child copy the
 //                          parameter and zero the moments; a child's position and log-scale come from its parent and
-//                          normal k*S + rank_in_split.
+//                          normal k*S + rank_in_split; a SGR_DENSIFY_POINTS_VANILLA column takes R from vanilla
+//                          3DGS's build_rotation instead of pytorch3d's quaternion_to_matrix.
 #include <math.h>
 
 #include "sgr_internal.cuh"
@@ -103,19 +104,58 @@ __global__ void __launch_bounds__(DNS_THREADS) densify_map_kernel(int P, const i
     }
 }
 
-// position (d) of child copy k of parent p: R(q^) (normal * scale) + point, R as pytorch3d's quaternion_to_matrix
+// R . (normal * exp(scale)) + point for row R of the child's rotation (the bmm's dot product as an fma chain)
+__device__ __forceinline__ float child_offset(int p, int d, int copy, int S, const int *__restrict__ split_scan,
+                                              const float *__restrict__ points, const float *__restrict__ scales,
+                                              const float *__restrict__ normals, const float R[3])
+{
+    const size_t z = 3 * ((size_t)copy * S + (split_scan[p] - 1));
+    float x = 0.0f;
+#pragma unroll
+    for (int c = 0; c < 3; c++) x = fmaf(R[c], __fmul_rn(normals[z + c], expf(scales[3 * (size_t)p + c])), x);
+    return __fadd_rn(x, points[3 * (size_t)p + d]);
+}
+
+// row d of vanilla 3DGS's build_rotation(q) (utils/general_utils.py:78-99), each torch op rounded on its own:
+// norm = sqrt(((r*r + x*x) + y*y) + z*z), no epsilon; q / norm a true division; then the entries as written
+__device__ void vanilla_rotation_row(float4 q, int d, float R[3])
+{
+    const float n = sqrtf(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q.x, q.x), __fmul_rn(q.y, q.y)), __fmul_rn(q.z, q.z)),
+                                    __fmul_rn(q.w, q.w)));
+    const float r = __fdiv_rn(q.x, n), x = __fdiv_rn(q.y, n), y = __fdiv_rn(q.z, n), z = __fdiv_rn(q.w, n);
+    if (d == 0) {
+        R[0] = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, y), __fmul_rn(z, z))));
+        R[1] = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, y), __fmul_rn(r, z)));
+        R[2] = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, z), __fmul_rn(r, y)));
+    } else if (d == 1) {
+        R[0] = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, y), __fmul_rn(r, z)));
+        R[1] = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(z, z))));
+        R[2] = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(y, z), __fmul_rn(r, x)));
+    } else {
+        R[0] = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, z), __fmul_rn(r, y)));
+        R[1] = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, z), __fmul_rn(r, x)));
+        R[2] = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))));
+    }
+}
+
+// position (d) of child copy k of parent p: R(q^) (normal * scale) + point, R as pytorch3d's quaternion_to_matrix, or
+// as vanilla 3DGS's build_rotation when `vanilla`
 __device__ float child_position(int p, int d, int copy, int S, const int *__restrict__ split_scan,
                                 const float *__restrict__ points, const float *__restrict__ scales,
-                                const float *__restrict__ quats, const float *__restrict__ normals)
+                                const float *__restrict__ quats, const float *__restrict__ normals, bool vanilla)
 {
     const float4 q = reinterpret_cast<const float4 *>(quats)[p];
+    float R[3];
+    if (vanilla) {
+        vanilla_rotation_row(q, d, R);
+        return child_offset(p, d, copy, S, split_scan, points, scales, normals, R);
+    }
     // F.normalize: q / max(|q|, 1e-12), |q| summed pairwise as torch's reduction does
     const float n = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(q.x, q.x), __fmul_rn(q.y, q.y)),
                                           __fadd_rn(__fmul_rn(q.z, q.z), __fmul_rn(q.w, q.w)))), 1e-12f);
     const float r = __fdiv_rn(q.x, n), qi = __fdiv_rn(q.y, n), qj = __fdiv_rn(q.z, n), qk = __fdiv_rn(q.w, n);
     const float two_s = __fdiv_rn(2.0f, __fadd_rn(__fadd_rn(__fmul_rn(r, r), __fmul_rn(qi, qi)),
                                                   __fadd_rn(__fmul_rn(qj, qj), __fmul_rn(qk, qk))));
-    float R[3];
     if (d == 0) {
         R[0] = __fsub_rn(1.0f, __fmul_rn(two_s, __fadd_rn(__fmul_rn(qj, qj), __fmul_rn(qk, qk))));
         R[1] = __fmul_rn(two_s, __fsub_rn(__fmul_rn(qi, qj), __fmul_rn(qk, r)));
@@ -129,11 +169,7 @@ __device__ float child_position(int p, int d, int copy, int S, const int *__rest
         R[1] = __fmul_rn(two_s, __fadd_rn(__fmul_rn(qj, qk), __fmul_rn(qi, r)));
         R[2] = __fsub_rn(1.0f, __fmul_rn(two_s, __fadd_rn(__fmul_rn(qi, qi), __fmul_rn(qj, qj))));
     }
-    const size_t z = 3 * ((size_t)copy * S + (split_scan[p] - 1));
-    float x = 0.0f;
-#pragma unroll
-    for (int c = 0; c < 3; c++) x = fmaf(R[c], __fmul_rn(normals[z + c], expf(scales[3 * (size_t)p + c])), x);
-    return __fadd_rn(x, points[3 * (size_t)p + d]);
+    return child_offset(p, d, copy, S, split_scan, points, scales, normals, R);
 }
 
 __global__ void __launch_bounds__(DNS_THREADS) densify_emit_kernel(DensifyColumns cols, int P_out, int S,
@@ -158,9 +194,9 @@ __global__ void __launch_bounds__(DNS_THREADS) densify_emit_kernel(DensifyColumn
         const unsigned row = e / w, d = e - row * w;
         const unsigned code = (unsigned)src_row[row], p = code & ((1u << TAG_SHIFT) - 1), tag = code >> TAG_SHIFT;
         if (tag != TAG_ORIG && col.kind == SGR_DENSIFY_ZERO_NEW) continue;
-        if (tag >= TAG_CHILD0 && col.kind == SGR_DENSIFY_POINTS)
+        if (tag >= TAG_CHILD0 && (col.kind == SGR_DENSIFY_POINTS || col.kind == SGR_DENSIFY_POINTS_VANILLA))
             v[u] = child_position((int)p, (int)d, (int)(tag - TAG_CHILD0), S, split_scan, points, scales, quats,
-                                  normals);
+                                  normals, col.kind == SGR_DENSIFY_POINTS_VANILLA);
         else if (tag >= TAG_CHILD0 && col.kind == SGR_DENSIFY_SCALES)
             v[u] = logf(__fmul_rn(expf(col.src[(size_t)p * 3 + d]), inv_split));
         else
@@ -243,7 +279,7 @@ int sgr_densify_emit(int32_t P, int32_t n_keep, int32_t n_clone, int32_t S, int3
     long long blocks = 0;
     for (int c = 0; c < n_cols; c++) {
         const SgrDensifyColumn &k = cols[c];
-        if (k.width <= 0 || k.kind < SGR_DENSIFY_COPY || k.kind > SGR_DENSIFY_SCALES ||
+        if (k.width <= 0 || k.kind < SGR_DENSIFY_COPY || k.kind > SGR_DENSIFY_POINTS_VANILLA ||
             (k.kind >= SGR_DENSIFY_POINTS && k.width != 3) || P_out * k.width > INT32_MAX) {
             set_error("sgr_densify_emit: column %d: width=%d kind=%d (width > 0, 3 for points and scales, "
                       "P' * width <= 2^31 - 1 with P'=%lld)", c, k.width, k.kind, P_out);

@@ -14,6 +14,7 @@
 // own cell with a K-entry insertion list in local memory; after shell r every unvisited point is
 // farther than r * (cell edge), which bounds the search exactly.  Everything (bounding box, cell
 // size) stays on the device: no host synchronisation.
+#include <float.h>
 #include <math.h>
 
 #include "sgr_knn.cuh"
@@ -299,6 +300,69 @@ __global__ void __launch_bounds__(128) knn_query_kernel(int Q, int K, int P, con
     }
 }
 
+// distCUDA2 (simple-knn, gaussian_model.py:134): per point, the mean squared distance to its 3 nearest OTHER points
+// (other by index: a duplicate position is a neighbour at distance 0).  The walk and shell bound are knn_query_kernel's;
+// the three best stay in registers with updateKBest's ascending swap chain, and the per-pair distance is its
+// contraction in the reference build's SASS: FMUL dy*dy, FFMA dx*dx + that, FFMA dz*dz + that (nvcc contracted
+// dx*dx + dy*dy into the x product, not the y one).  The three smallest
+// distances as a sorted multiset do not depend on the visiting order, so an exact 3-NN gives the reference's bits.  With
+// fewer than 3 other points the FLT_MAX sentinels enter the sum, as in the reference: P <= 2 gives inf, P = 3 gives
+// (d1 + d2 + FLT_MAX) / 3 (FLT_MAX / 3 for ordinary clouds).
+__global__ void __launch_bounds__(128) dist_cuda2_kernel(int P, const KnnGrid *__restrict__ gp,
+                                                          const uint32_t *__restrict__ starts,
+                                                          const float4 *__restrict__ sorted, float *__restrict__ out)
+{
+    const int q = blockIdx.x * 128 + threadIdx.x;
+    if (q >= P) return;
+    const KnnGrid g = *gp;
+    const int nx = g.n[0], ny = g.n[1], nz = g.n[2];
+    const uint32_t ncell = (uint32_t)nx * ny * nz;
+    // the query in sorted order: the same warp walks neighbouring cells
+    const float4 me = __ldg(sorted + q);
+    const int self = __float_as_int(me.w);
+    const float qx = me.x, qy = me.y, qz = me.z;
+    const int cx = cell_coord(qx, g.lo[0], g.inv_h, nx), cy = cell_coord(qy, g.lo[1], g.inv_h, ny),
+              cz = cell_coord(qz, g.lo[2], g.inv_h, nz);
+    const int rmax = max(nx, max(ny, nz));
+    float b0 = FLT_MAX, b1 = FLT_MAX, b2 = FLT_MAX;
+    int have = 0;
+    for (int r = 0; r < rmax; r++) {
+        const int z0 = max(cz - r, 0), z1 = min(cz + r, nz - 1);
+        const int y0 = max(cy - r, 0), y1 = min(cy + r, ny - 1);
+        const int x0 = max(cx - r, 0), x1 = min(cx + r, nx - 1);
+        for (int z = z0; z <= z1; z++) {
+            const bool zface = (z == cz - r) || (z == cz + r);
+            for (int y = y0; y <= y1; y++) {
+                const bool yface = (y == cy - r) || (y == cy + r);
+                const int step = (zface || yface || r == 0) ? 1 : max(1, 2 * r);
+                for (int x = cx - r; x <= cx + r; x += step) {
+                    if (x < x0 || x > x1) continue;
+                    const uint32_t c = ((uint32_t)z * ny + y) * nx + x;
+                    const uint32_t s = starts[c];
+                    const uint32_t e = (c + 1 < ncell) ? starts[c + 1] : (uint32_t)P;
+                    for (uint32_t k = s; k < e; k++) {
+                        const float4 p = __ldg(sorted + k);
+                        if (__float_as_int(p.w) == self) continue;
+                        const float dx = __fsub_rn(p.x, qx), dy = __fsub_rn(p.y, qy), dz = __fsub_rn(p.z, qz);
+                        float d = fmaf(dz, dz, fmaf(dx, dx, __fmul_rn(dy, dy)));
+                        have++;
+                        // updateKBest<3>: walk the list from the front, swapping the carried value into place
+                        float t;
+                        if (b0 > d) { t = b0; b0 = d; d = t; }
+                        if (b1 > d) { t = b1; b1 = d; d = t; }
+                        if (b2 > d) b2 = d;
+                    }
+                }
+            }
+        }
+        // every unvisited point is farther than r cell edges (knn_query_kernel's bound, shrunk by a thousandth of an
+        // edge so that a coordinate rounded into a neighbouring cell cannot end the walk early)
+        const float bound = fmaxf((float)r - 1e-3f, 0.0f) * g.h;
+        if (have >= 3 && b2 <= bound * bound) break;
+    }
+    out[self] = __fdiv_rn(__fadd_rn(__fadd_rn(b0, b1), b2), 3.0f);
+}
+
 static int knn_axis_cells(int P)
 {
     // about 4 points per cell on a volume-filling cloud; surface-like clouds leave most cells empty,
@@ -374,6 +438,25 @@ int sgr_knn(int32_t P, const float *points, int32_t Q, const float *queries, int
     SGR_LAUNCH(K_KNN_QUERY, st,
                knn_query_kernel<<<(Q + 127) / 128, 128, 0, st>>>(Q, K, P, queries, cells.grid, cells.starts,
                                                                  cells.sorted, idx, dist2));
+    SGR_CUDA(cudaGetLastError());
+    return SGR_OK;
+}
+
+int sgr_dist_cuda2(int32_t P, const float *points, float *mean_dist2, void *workspace, void *stream)
+{
+    if (P < 0 || (P > 0 && (!points || !mean_dist2 || !workspace))) {
+        set_error("sgr_dist_cuda2: need P >= 0 and non-null pointers (P=%d)", P);
+        return SGR_EINVAL;
+    }
+    if (P == 0) return SGR_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    Layout l(workspace);
+    KnnCells cells;
+    int rc = knn_build_cells(P, points, knn_cells_scratch(l, P), st, &cells);
+    if (rc) return rc;
+    SGR_LAUNCH(K_KNN_QUERY, st,
+               dist_cuda2_kernel<<<(P + 127) / 128, 128, 0, st>>>(P, cells.grid, cells.starts, cells.sorted,
+                                                                  mean_dist2));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }

@@ -22,8 +22,11 @@ sums accum and denom and takes the maximum of max_radii2D over the ranks before 
 drawn on the group's first rank and broadcast, so every rank makes the same decisions.  The per-step statistics stay
 local between densifications and are never part of the gradient exchange.
 
-Mesh-bound models are out of scope (the refinement never densifies), as is vanilla 3DGS's GaussianModel, whose
-build_rotation normalises differently.
+`rotation="vanilla"` makes it vanilla 3DGS's GaussianModel densification (gaussian_splatting/scene/gaussian_model.py:
+273-410, as train.train_3dgs uses it).  Every statement there is SuGaRDensifier's except the split's rotation, which is
+build_rotation of the raw quaternion (norm = sqrt(((r*r + x*x) + y*y) + z*z), no epsilon, a true division, then the
+nine entries as written) instead of pytorch3d's quaternion_to_matrix of the normalised one; oracle/densify_oracle_vanilla.py
+restates it.  Mesh-bound models are out of scope (the refinement never densifies).
 """
 import numpy as np
 import torch
@@ -31,7 +34,8 @@ import torch
 from ._lib import SgrDensifyColumn, SgrDensifyGates, check, lib, ptr, require_cuda, stream, tensor
 
 KEYS = ("points", "densities", "scales", "quaternions", "sh_dc", "sh_rest")
-COPY, ZERO_NEW, POINTS, SCALES = 0, 1, 2, 3
+COPY, ZERO_NEW, POINTS, SCALES, POINTS_VANILLA = 0, 1, 2, 3, 4
+ROTATIONS = {"sugar": POINTS, "vanilla": POINTS_VANILLA}   # the split's R: quaternion_to_matrix / build_rotation
 INV_SPLIT = float(np.float32(1.0) / np.float32(0.8 * 2))   # torch's scalar division on CUDA: x * (1 / float(1.6))
 
 
@@ -56,12 +60,16 @@ def split_normals(S, device, generator=None, group=None):
 
 
 class Densifier:
-    """SuGaRDensifier over `raw` and `optimizer` (see the module docstring)."""
+    """SuGaRDensifier over `raw` and `optimizer`, or vanilla 3DGS's with rotation="vanilla" (see the module
+    docstring)."""
 
     def __init__(self, raw, optimizer, max_grad=2e-4, min_opacity=0.005, max_screen_size=20, scene_extent=None,
-                 percent_dense=0.01, group=None):
+                 percent_dense=0.01, group=None, rotation="sugar"):
         if scene_extent is None:
             raise ValueError("scene_extent is required (the reference's get_cameras_spatial_extent())")
+        if rotation not in ROTATIONS:
+            raise ValueError(f"rotation must be 'sugar' or 'vanilla', got {rotation!r}")
+        self.points_kind = ROTATIONS[rotation]
         self.raw, self.optimizer, self.group = raw, optimizer, group
         self.max_grad, self.min_opacity, self.max_screen_size = max_grad, min_opacity, max_screen_size
         self.scene_extent, self.percent_dense = scene_extent, percent_dense
@@ -110,7 +118,7 @@ class Densifier:
             alive.append(src)
             dst = torch.empty((P_out,) + tuple(src.shape[1:]), device=dev)
             width = int(np.prod(src.shape[1:]))
-            kind = POINTS if k == "points" else SCALES if k == "scales" else COPY
+            kind = self.points_kind if k == "points" else SCALES if k == "scales" else COPY
             cols.append((src, dst, width, kind))
             st = self.optimizer.state.get(self.raw[k], None)
             mom = None

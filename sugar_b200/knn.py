@@ -3,6 +3,7 @@ SuGaR uses it (sugar_scene/sugar_model.py:1013-1030 reset_neighbors, :1335-1343)
 
     dists, idx = knn_points(queries, points, K)     # [Q,K] squared distances (ascending), [Q,K] int64
     knn_dists, knn_idx = reset_neighbors(points, K=16)   # the tables SuGaR keeps (self is neighbour 0)
+    dist2 = dist_cuda2(points)                       # simple-knn's distCUDA2: vanilla 3DGS's initial scales
 """
 import torch
 
@@ -36,3 +37,20 @@ def reset_neighbors(points: torch.Tensor, K: int = 16):
     """SuGaR.reset_neighbors: (knn_dists [P,K], knn_idx [P,K]) of the cloud against itself, no grad."""
     with torch.no_grad():
         return knn_points(points, points, K)
+
+
+def dist_cuda2(points: torch.Tensor) -> torch.Tensor:
+    """simple-knn's distCUDA2 (vanilla 3DGS's create_from_pcd): float32 [P], per point the mean of the squared
+    distances to its 3 nearest other points (other by index, so a duplicate position is a neighbour at 0), the
+    reference's value to the bit.  With P <= 3 its FLT_MAX sentinels stay in the mean: inf for P <= 2, about
+    FLT_MAX / 3 for P = 3.  `points`: [P,3] CUDA tensor (converted to float32).  No host synchronisation."""
+    r = _cloud(points, "points")
+    require_cuda("knn", r)
+    dev, P = r.device, r.shape[0]
+    out = torch.empty((P,), dtype=torch.float32, device=dev)
+    if P == 0:
+        return out
+    with torch.cuda.device(dev):
+        ws = scratch(lib.sgr_knn_workspace_bytes(P), dev)
+        check(lib.sgr_dist_cuda2(P, ptr(r), ptr(out), ptr(ws), stream(dev)))
+    return out
