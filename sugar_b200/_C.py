@@ -82,7 +82,7 @@ class _Arena:
         self.used = 0
         self.parts = {}
         self.error = None   # an exception raised inside a callback (e.g. torch OOM): re-raised after the C call returns
-        self.cbs = {name: _lib.ALLOC_FN(lambda _ctx, n, name=name: self._alloc(name, n)) for name in ("geom", "binning", "img")}
+        self.cbs = {name: _lib.SgrAlloc(lambda _ctx, n, name=name: self._alloc(name, n)) for name in ("geom", "binning", "img")}
 
     def _alloc(self, name, nbytes):
         try:
@@ -129,7 +129,7 @@ def _view_struct(bg, scale_modifier, viewmatrix, projmatrix, tan_fovx, tan_fovy,
 
 def _gauss_struct(P, M, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp, sh_rest=None) -> SgrGaussians:
     g = SgrGaussians()
-    g.activations = 1 if sh_rest is not None else 0   # SGR_ACT_RAW: raw SuGaR parameters, (dc, rest) SH arrays
+    g.activations = _lib.SGR_ACT_RAW if sh_rest is not None else 0   # raw SuGaR parameters, (dc, rest) SH arrays
     g.sh_rest = f32_ptr(sh_rest, "sh_rest") if sh_rest is not None else None
     g.P, g.M = int(P), int(M)
     g.means3D = f32_ptr(means3D, "means3D")

@@ -1,185 +1,96 @@
-"""ctypes binding of libsugar_b200.so (the C ABI declared in include/sugar_b200.h).
+"""ctypes binding of libsugar_b200.so.
+
+The C header include/sugar_b200.h is the binding's only statement of the ABI: its structs, callback types, integer
+SGR_* constants and SGR_API prototypes are read from it at import (parse_header) and exported here under their C names.
 
 There is no CPU fallback: if the CUDA library is missing this module raises at import, and every
 call raises on a non-zero status with the library's own message.
 """
 import ctypes as C
 import os
+import re
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SGR_LIB_PATH", os.path.join(_HERE, "lib", "libsugar_b200.so"))  # override: the stats build (scripts/blend_stats.py)
+HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "sugar_b200.h")
+
+# sgr_struct_bytes(i) is the library's sizeof of _STRUCT_ORDER[i] (the index order of its switch)
+_STRUCT_ORDER = ("SgrView", "SgrGaussians", "SgrBackwardPlan", "SgrFieldParams", "SgrSsimParams", "SgrDensifyGates",
+                 "SgrDensifyColumn", "SgrAdamSegment", "SgrPeerPlan")
+
+# The header's types by value; a pointer may point to one of these, to a header struct, or to _POINTEES.
+_SCALARS = {"int32_t": C.c_int32, "int": C.c_int32, "int64_t": C.c_int64, "uint32_t": C.c_uint32,
+            "uint64_t": C.c_uint64, "unsigned long long": C.c_ulonglong, "size_t": C.c_size_t, "float": C.c_float,
+            "double": C.c_double}
+_POINTEES = ("void", "char", "uint8_t")
 
 
 class SgrError(RuntimeError):
     pass
 
 
-class SgrView(C.Structure):
-    _fields_ = [
-        ("image_height", C.c_int32), ("image_width", C.c_int32),
-        ("tanfovx", C.c_float), ("tanfovy", C.c_float),
-        ("bg", C.c_void_p), ("scale_modifier", C.c_float),
-        ("viewmatrix", C.c_void_p), ("projmatrix", C.c_void_p),
-        ("sh_degree", C.c_int32), ("campos", C.c_void_p),
-        ("prefiltered", C.c_int32), ("debug", C.c_int32),
-    ]
+def parse_header(text: str):
+    """-> (names, prototypes) of the C header `text`.  names: its integer `#define SGR_*` constants, its structs as
+    ctypes.Structure classes and its function-pointer typedefs as CFUNCTYPEs, by their C names; prototypes: every
+    SGR_API function as name -> (restype, argtypes).  A pointer to a header struct is POINTER(struct), a returned
+    `const char *` c_char_p, any other pointer c_void_p.  Raises SgrError naming any declaration it cannot map."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    names = {m[1]: int(m[2]) for m in
+             re.finditer(r"^[ \t]*#[ \t]*define[ \t]+(SGR_\w+)[ \t]+\(?[ \t]*(-?\d+)[ \t]*\)?[ \t]*$", text, re.M)}
+    text = re.sub(r"^[ \t]*#.*$", "", text, flags=re.M)   # the other preprocessor lines, SGR_API's definition among them
+    structs = {s: type(s, (C.Structure,), {"__module__": __name__}) for s in re.findall(r"\bstruct\s+(\w+)", text)}
+    callbacks = {}
+
+    def ctype(spec, what, ret=False):
+        base, stars = " ".join(w for w in re.findall(r"\w+", spec) if w != "const"), spec.count("*")
+        if not stars and (base in _SCALARS or base in callbacks):
+            return _SCALARS.get(base) or callbacks[base]
+        if ret and (base, stars) in (("void", 0), ("char", 1)):
+            return None if base == "void" else C.c_char_p
+        if stars == 1 and base in structs:
+            return C.POINTER(structs[base])
+        if stars and (base in _SCALARS or base in structs or base in _POINTEES):
+            return C.c_void_p
+        raise SgrError(f"{HEADER_PATH}: {what}: no ctypes type for '{' '.join(spec.split())}'")
+
+    def declarator(decl, what):   # 'const float *x' -> ('const float *', 'x', None); 'float w[11]' -> (.., 'w', 11)
+        m = re.fullmatch(r"\s*(.*?)(\w+)\s*(?:\[(\d+)\])?\s*", decl, re.S)
+        if m is None:
+            raise SgrError(f"{HEADER_PATH}: {what}: cannot parse '{' '.join(decl.split())}'")
+        return m[1], m[2], m[3] and int(m[3])
+
+    def params(arglist, fn):
+        if arglist.strip() in ("", "void"):
+            return []
+        return [ctype(declarator(a, fn)[0], f"{fn}({' '.join(a.split())})") for a in arglist.split(",")]
+
+    for m in re.finditer(r"typedef\s+([^;{}()]+?)\(\s*\*\s*(\w+)\s*\)\s*\(([^()]*)\)\s*;", text):
+        callbacks[m[2]] = C.CFUNCTYPE(ctype(m[1], m[2], ret=True), *params(m[3], m[2]))
+    for m in re.finditer(r"\bstruct\s+(\w+)\s*\{([^{}]*)\}", text):
+        fields = []
+        for decl in filter(str.strip, m[2].split(";")):
+            first, *more = decl.split(",")   # int32_t N, K, P;
+            spec, name, n = declarator(first, m[1])
+            for spec, name, n in [(spec, name, n)] + [declarator(spec.split("*")[0] + d, m[1]) for d in more]:
+                t = ctype(spec, f"{m[1]}.{name}")
+                fields.append((name, t * n if n else t))
+        structs[m[1]]._fields_ = fields   # after the class exists: SgrPeerPlan is used by pointer before its body
+    prototypes = {m[2]: (ctype(m[1], m[2], ret=True), params(m[3], m[2]))
+                  for m in re.finditer(r"\bSGR_API\s+([^;{}()]*?)(\w+)\s*\(([^()]*)\)\s*;", text)}
+    if len(prototypes) != len(re.findall(r"\bSGR_API\b", text)):
+        raise SgrError(f"{HEADER_PATH}: an SGR_API declaration is not of the form `SGR_API <ret> <name>(<args>);`")
+    return {**names, **structs, **callbacks}, prototypes
 
 
-class SgrGaussians(C.Structure):
-    _fields_ = [
-        ("P", C.c_int32), ("M", C.c_int32),
-        ("means3D", C.c_void_p), ("opacities", C.c_void_p), ("shs", C.c_void_p),
-        ("colors_precomp", C.c_void_p), ("scales", C.c_void_p), ("rotations", C.c_void_p),
-        ("cov3D_precomp", C.c_void_p), ("activations", C.c_int32), ("sh_rest", C.c_void_p),
-    ]
-
-
-class SgrFieldParams(C.Structure):
-    _fields_ = [("N", C.c_int32), ("K", C.c_int32), ("P", C.c_int32), ("density_factor", C.c_float),
-                ("density_threshold", C.c_float), ("opacity_min_clamp", C.c_float), ("samples_per_idx_row", C.c_int32)]
-
-
-class SgrSsimParams(C.Structure):
-    _fields_ = [("B", C.c_int32), ("C", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("c1", C.c_float),
-                ("c2", C.c_float), ("window", C.c_float * 11)]
-
-
-class SgrDensifyGates(C.Structure):
-    _fields_ = [("max_grad", C.c_float), ("clone_scale", C.c_float), ("big_scale", C.c_float),
-                ("min_opacity", C.c_float), ("screen_size", C.c_float), ("inv_split", C.c_float),
-                ("use_screen", C.c_int32)]
-
-
-class SgrDensifyColumn(C.Structure):
-    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("width", C.c_int32), ("kind", C.c_int32)]
-
-
-class SgrAdamSegment(C.Structure):
-    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
-                ("n", C.c_int64), ("one_minus_beta1", C.c_float), ("beta2", C.c_float), ("one_minus_beta2", C.c_float),
-                ("bias_correction2_sqrt", C.c_float), ("eps", C.c_float), ("step_size", C.c_float)]
-
-
-ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
-STAGE_HOOK = C.CFUNCTYPE(None, C.c_void_p, C.c_int32)
-
-
-class SgrPeerPlan(C.Structure):
-    _fields_ = [("peer_flag_tab", C.c_void_p), ("peer_nranks", C.c_int32), ("peer_rank", C.c_int32),
-                ("peer_slot_blend", C.c_int32), ("peer_slot_chunk0", C.c_int32), ("peer_seq", C.c_uint32),
-                ("peer_view_blocks", C.c_void_p), ("peer_flags", C.c_void_p), ("peer_dsh_scale", C.c_float),
-                ("peer_timeout_s", C.c_double), ("peer_record_stages", C.c_void_p), ("peer_signal_stream", C.c_void_p),
-                ("peer_side_stream", C.c_void_p), ("peer_rec_tab", C.c_void_p), ("peer_sum_tab", C.c_void_p),
-                ("peer_sums", C.c_void_p), ("peer_slot_reduced0", C.c_int32), ("peer_emulate_ranks", C.c_uint64)]
-
-
-class SgrBackwardPlan(C.Structure):
-    _fields_ = [("hook", STAGE_HOOK), ("hook_ctx", C.c_void_p), ("num_chunks", C.c_int32),
-                ("reduce_records", C.c_void_p), ("dL_dsh_rest", C.c_void_p), ("chunk_taper", C.c_int32),
-                ("peer", C.POINTER(SgrPeerPlan))]
-
-
-# name -> (restype, argtypes); kept in one table so tests can check it against the header
-PROTOTYPES = {
-    "sgr_rasterize_forward": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians), ALLOC_FN, C.c_void_p, ALLOC_FN,
-                                        C.c_void_p, ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
-                                        C.POINTER(C.c_int64), C.c_void_p]),
-    "sgr_rasterize_backward": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians)] + [C.c_void_p] * 4 +
-                               [C.c_int64] + [C.c_void_p] * 11),
-    "sgr_rasterize_backward_staged": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians)] + [C.c_void_p] * 4 +
-                                      [C.c_int64] + [C.c_void_p] * 11 + [C.POINTER(SgrBackwardPlan)]),
-    "sgr_rasterize_forward_feature": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians), ALLOC_FN, C.c_void_p,
-                                                ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p] + [C.c_void_p] * 5 +
-                                      [C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
-    "sgr_rasterize_backward_feature": (C.c_int, [C.POINTER(SgrView), C.POINTER(SgrGaussians)] + [C.c_void_p] * 4 +
-                                       [C.c_int64] + [C.c_void_p] * 15),
-    "sgr_backward_chunk_range": (C.c_int, [C.c_int32] * 4 + [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
-    "sgr_view_grad_finalize": (C.c_int, [C.c_int32] * 6 + [C.c_void_p] * 3 + [C.c_int64, C.c_int32] + [C.c_void_p] * 2 +
-                               [C.c_float] + [C.c_void_p] * 5),
-    "sgr_peer_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p)]),
-    "sgr_peer_free": (C.c_int, [C.c_void_p]),
-    "sgr_peer_export": (C.c_int, [C.c_void_p, C.c_void_p]),
-    "sgr_peer_import": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
-    "sgr_peer_close": (C.c_int, [C.c_void_p]),
-    "sgr_peer_flag_bytes": (C.c_size_t, []),
-    "sgr_peer_signal": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32, C.c_void_p]),
-    "sgr_peer_wait": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint32, C.c_double, C.c_void_p]),
-    "sgr_peer_reduce_records_synced": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                                 C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_uint32, C.c_void_p,
-                                                 C.c_double, C.c_void_p]),
-    "sgr_mark_visible": (C.c_int, [C.c_int32] + [C.c_void_p] * 5),
-    "sgr_geometry_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_binning_bytes": (C.c_size_t, [C.c_int64]),
-    "sgr_image_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
-    "sgr_backward_scratch_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_inspect_state": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 16),
-    "sgr_field_scratch_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_normal_scratch_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_normal_loss_forward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 10),
-    "sgr_normal_loss_backward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 11),
-    "sgr_field_forward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 12),
-    "sgr_field_backward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 17),
-    "sgr_density_estimation_forward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 11),
-    "sgr_density_estimation_backward": (C.c_int, [C.POINTER(SgrFieldParams)] + [C.c_void_p] * 15),
-    "sgr_meshbind_forward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 5 + [C.c_float] + [C.c_void_p] * 4),
-    "sgr_meshbind_backward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 12),
-    "sgr_meshbind_edited_forward": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 6 + [C.c_float] + [C.c_void_p] * 5),
-    "sgr_sh_colors_rotated": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 4),
-    "sgr_knn_workspace_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_knn": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                          C.c_void_p]),
-    "sgr_dist_cuda2": (C.c_int, [C.c_int32] + [C.c_void_p] * 4),
-    "sgr_l1_ssim_scratch_bytes": (C.c_size_t, [C.c_int32] * 4),
-    "sgr_l1_ssim_forward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 6),
-    "sgr_l1_ssim_backward": (C.c_int, [C.POINTER(SgrSsimParams)] + [C.c_void_p] * 7),
-    "sgr_mesh_nc_forward_scratch_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_mesh_nc_backward_scratch_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_mesh_nc_forward": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 5),
-    "sgr_mesh_nc_backward": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 8),
-    "sgr_border_peel": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 6),
-    "sgr_splat_mesh": (C.c_int, [C.c_int32] + [C.c_void_p] * 5 + [C.c_float, C.c_void_p, C.c_void_p]),
-    "sgr_mesh_raster_scratch_bytes": (C.c_size_t, [C.c_int32] * 3),
-    "sgr_mesh_raster": (C.c_int, [C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32, C.c_int32] +
-                        [C.c_void_p] * 4),
-    "sgr_texture_init": (C.c_int, [C.c_int32] * 5 + [C.c_void_p] * 8),
-    "sgr_texture_bake_view": (C.c_int, [C.c_int32] * 4 + [C.c_void_p] * 6 + [C.c_int32, C.c_int32] +
-                              [C.c_void_p] * 8),
-    "sgr_texture_render": (C.c_int, [C.c_int32] * 5 + [C.c_void_p] * 7 + [C.c_int32] * 2 + [C.c_void_p] * 2 +
-                           [C.c_int32] + [C.c_float] * 3 + [C.c_double] * 2 + [C.c_void_p] * 2),
-    "sgr_density_grid_workspace_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_density_grid": (C.c_int, [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32, C.c_float] + [C.c_int32] * 3 +
-                         [C.c_void_p] * 3 + [C.c_float] + [C.c_void_p] * 3),
-    "sgr_mcubes_scratch_bytes": (C.c_size_t, [C.c_int32] * 3),
-    "sgr_mcubes_count": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double] + [C.c_void_p] * 4),
-    "sgr_mcubes_emit": (C.c_int, [C.c_int32] * 3 + [C.c_void_p, C.c_double, C.c_int64, C.c_int64] + [C.c_void_p] * 4),
-    "sgr_poisson_bin": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32] + [C.c_float] * 4 + [C.c_void_p] * 8),
-    "sgr_poisson_splat": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
-                                    C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "sgr_poisson_coarsen": (C.c_int, [C.c_int32] + [C.c_void_p] * 3),
-    "sgr_poisson_residual_norm": (C.c_int, [C.c_int32, C.c_float] + [C.c_void_p] * 6),
-    "sgr_poisson_vcycle": (C.c_int, [C.c_int32] + [C.c_void_p] * 6),
-    "sgr_poisson_interpolate": (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_float] +
-                                [C.c_void_p] * 4),
-    "sgr_decimate_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
-    "sgr_decimate": (C.c_int, [C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 11),
-    "sgr_densify_stats": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 6),
-    "sgr_densify_classify": (C.c_int, [C.c_int32] + [C.c_void_p] * 4 + [C.POINTER(SgrDensifyGates)] +
-                             [C.c_void_p] * 2),
-    "sgr_densify_emit": (C.c_int, [C.c_int32] * 5 + [C.c_void_p, C.c_int32, C.POINTER(SgrDensifyColumn)] +
-                         [C.c_void_p] * 4 + [C.c_float, C.c_void_p, C.c_void_p]),
-    "sgr_adam_step": (C.c_int, [C.c_int32, C.POINTER(SgrAdamSegment), C.c_void_p]),
-    "sgr_struct_bytes": (C.c_size_t, [C.c_int32]),
-    "sgr_launch_count": (C.c_ulonglong, []),
-    "sgr_num_kernel_kinds": (C.c_int, []),
-    "sgr_kernel_name": (C.c_char_p, [C.c_int]),
-    "sgr_profile_enable": (C.c_int, [C.c_int]),
-    "sgr_profile_read": (C.c_int, [C.c_void_p, C.c_void_p]),
-    "sgr_profile_timeline": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "sgr_last_error": (C.c_char_p, []),
-    "sgr_version": (C.c_char_p, []),
-}
+with open(HEADER_PATH) as _f:
+    _names, PROTOTYPES = parse_header(_f.read())
+globals().update(_names)
+_structs = {n for n, t in _names.items() if isinstance(t, type) and issubclass(t, C.Structure)}
+if _structs != set(_STRUCT_ORDER):
+    raise SgrError(f"{HEADER_PATH}: structs {sorted(_structs ^ set(_STRUCT_ORDER))} are not both in the header and in "
+                   "_lib._STRUCT_ORDER, the index order of sgr_struct_bytes")
 
 
 def _load():
@@ -196,11 +107,10 @@ def _load():
 
 
 lib = _load()
-for _i, _t in enumerate((SgrView, SgrGaussians, SgrBackwardPlan, SgrFieldParams, SgrSsimParams, SgrDensifyGates,
-                          SgrDensifyColumn, SgrAdamSegment, SgrPeerPlan)):
-    if lib.sgr_struct_bytes(_i) != C.sizeof(_t):   # a stale library or a binding edited without the header
-        raise SgrError(f"{LIB_PATH}: struct {_t.__name__} is {lib.sgr_struct_bytes(_i)} bytes in the library, "
-                       f"{C.sizeof(_t)} in this binding -- rebuild with `python sugar_b200/build.py`")
+for _i, _n in enumerate(_STRUCT_ORDER):
+    if lib.sgr_struct_bytes(_i) != C.sizeof(_names[_n]):   # a library built from another version of the header
+        raise SgrError(f"{LIB_PATH}: struct {_n} is {lib.sgr_struct_bytes(_i)} bytes in the library, "
+                       f"{C.sizeof(_names[_n])} in {HEADER_PATH} -- rebuild with `python sugar_b200/build.py`")
 
 
 def check(status: int) -> None:

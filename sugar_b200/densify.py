@@ -31,11 +31,13 @@ restates it.  Mesh-bound models are out of scope (the refinement never densifies
 import numpy as np
 import torch
 
-from ._lib import SgrDensifyColumn, SgrDensifyGates, check, lib, ptr, require_cuda, stream, tensor
+from ._lib import (SGR_DENSIFY_COPY, SGR_DENSIFY_POINTS, SGR_DENSIFY_POINTS_VANILLA, SGR_DENSIFY_SCALES,
+                   SGR_DENSIFY_ZERO_NEW, SgrDensifyColumn, SgrDensifyGates, check, lib, ptr, require_cuda, stream,
+                   tensor)
 
 KEYS = ("points", "densities", "scales", "quaternions", "sh_dc", "sh_rest")
-COPY, ZERO_NEW, POINTS, SCALES, POINTS_VANILLA = 0, 1, 2, 3, 4
-ROTATIONS = {"sugar": POINTS, "vanilla": POINTS_VANILLA}   # the split's R: quaternion_to_matrix / build_rotation
+# the split's R: quaternion_to_matrix / build_rotation
+ROTATIONS = {"sugar": SGR_DENSIFY_POINTS, "vanilla": SGR_DENSIFY_POINTS_VANILLA}
 INV_SPLIT = float(np.float32(1.0) / np.float32(0.8 * 2))   # torch's scalar division on CUDA: x * (1 / float(1.6))
 
 
@@ -118,7 +120,7 @@ class Densifier:
             alive.append(src)
             dst = torch.empty((P_out,) + tuple(src.shape[1:]), device=dev)
             width = int(np.prod(src.shape[1:]))
-            kind = self.points_kind if k == "points" else SCALES if k == "scales" else COPY
+            kind = self.points_kind if k == "points" else SGR_DENSIFY_SCALES if k == "scales" else SGR_DENSIFY_COPY
             cols.append((src, dst, width, kind))
             st = self.optimizer.state.get(self.raw[k], None)
             mom = None
@@ -128,7 +130,7 @@ class Densifier:
                     m = st[name].contiguous()
                     alive.append(m)
                     md = torch.empty_like(dst)
-                    cols.append((m, md, width, ZERO_NEW))
+                    cols.append((m, md, width, SGR_DENSIFY_ZERO_NEW))
                     mom.append(md)
             new[k] = (dst, mom)
         stats = None
@@ -136,7 +138,7 @@ class Densifier:
             stats = (torch.empty((P_out, 1), device=dev), torch.empty((P_out, 1), device=dev),
                      torch.empty((P_out,), device=dev))
             for s, d in zip((self.accum, self.denom, self.max_radii2D), stats):
-                cols.append((s, d, 1, COPY))
+                cols.append((s, d, 1, SGR_DENSIFY_COPY))
         tab = (SgrDensifyColumn * len(cols))(*[SgrDensifyColumn(ptr(s), ptr(d), w, kd) for s, d, w, kd in cols])
         src_row = torch.empty((P_out,), dtype=torch.int32, device=dev)
         pts, scl, q = (self.raw[k].detach().contiguous() for k in ("points", "scales", "quaternions"))

@@ -16,9 +16,7 @@ float32 CUDA tensors.
 import numpy as np
 import torch
 
-from ._lib import SgrAdamSegment, check, lib, stream
-
-MAX_SEGMENTS = 8   # SGR_ADAM_MAX_SEGMENTS: tensors per launch
+from ._lib import SGR_ADAM_MAX_SEGMENTS, SgrAdamSegment, check, lib, stream
 
 
 def _check_param(p, name="params"):
@@ -123,8 +121,8 @@ class Adam(torch.optim.Optimizer):
         if segs:
             with torch.cuda.device(dev):
                 st = stream(dev)
-                for i in range(0, len(segs), MAX_SEGMENTS):
-                    chunk = segs[i:i + MAX_SEGMENTS]
+                for i in range(0, len(segs), SGR_ADAM_MAX_SEGMENTS):
+                    chunk = segs[i:i + SGR_ADAM_MAX_SEGMENTS]
                     check(lib.sgr_adam_step(len(chunk), (SgrAdamSegment * len(chunk))(*chunk), st))
         return loss
 

@@ -247,7 +247,7 @@ class ViewParallel:
         """`launch(plan, *, dL_dcolors=ptr, dL_dsh=ptr)` enqueues this view's sgr_rasterize_backward_staged under
         `plan`, with the two gradient outputs optionally redirected; `bufs`: dict of the gradient tensors +
         "records" f32[P,11].  Returns nothing: bufs hold the reduced gradients when the enqueued work completes."""
-        from ._lib import STAGE_HOOK, SgrBackwardPlan, check, lib
+        from ._lib import SGR_STAGE_BLEND_DONE, SGR_STAGE_CHUNK_DONE, SgrBackwardPlan, SgrStageHook, check, lib
         if self.uses_peer_memory(M, has_cov_precomp):
             st = self._peer_state(lib, check, P, means3D.device)
             if st is not None:
@@ -283,16 +283,17 @@ class ViewParallel:
 
         def on_stage(_ctx, stage):
             try:
-                if stage == 1:  # SGR_STAGE_BLEND_DONE: dL_dcolors is final
+                if stage == SGR_STAGE_BLEND_DONE:  # dL_dcolors is final
                     if factor and multi:
                         early.append(dist.all_gather_into_tensor(d_all, bufs["colors_block"], group=self.group,
                                                                  async_op=True))
                     elif not M and multi:  # colours were precomputed: their gradient is an ordinary sum
                         early.append(dist.all_reduce(bufs["colors"], group=self.group, async_op=True))
-                elif stage >= 16 and side is not None and not multi:
-                    chunk_done[stage - 16].record()   # what the side stream's finalize of this range waits for
-                elif stage >= 16 and multi:  # SGR_STAGE_CHUNK_DONE + c
-                    c = stage - 16
+                elif stage >= SGR_STAGE_CHUNK_DONE and side is not None and not multi:
+                    # what the side stream's finalize of this range waits for
+                    chunk_done[stage - SGR_STAGE_CHUNK_DONE].record()
+                elif stage >= SGR_STAGE_CHUNK_DONE and multi:
+                    c = stage - SGR_STAGE_CHUNK_DONE
                     p0, p1 = ranges[c]
                     if p1 > p0:
                         pending[c].append(dist.all_reduce(bufs["records"][p0:p1], group=self.group, async_op=True))
@@ -303,7 +304,7 @@ class ViewParallel:
             except BaseException as e:  # never unwind through the C frame
                 failure.append(e)
 
-        cb = STAGE_HOOK(on_stage)
+        cb = SgrStageHook(on_stage)
         launch(SgrBackwardPlan(hook=cb, num_chunks=nchunks, chunk_taper=taper, reduce_records=bufs["records"].data_ptr()))
         if failure:
             raise failure[0]

@@ -42,11 +42,12 @@ from types import SimpleNamespace
 
 import torch
 
-from ._lib import check, check_ids, lib, require_cuda, same_device, stream, tensor
+from ._lib import (SGR_SAMPLE_BILINEAR, SGR_SAMPLE_NEAREST, check, check_ids, lib, require_cuda, same_device, stream,
+                   tensor)
 from .splatmesh import cam_matrix
 
 INT32_MAX = 2 ** 31 - 1
-SAMPLING_MODES = {"bilinear": 0, "nearest": 1}   # SGR_SAMPLE_BILINEAR, SGR_SAMPLE_NEAREST
+SAMPLING_MODES = {"bilinear": SGR_SAMPLE_BILINEAR, "nearest": SGR_SAMPLE_NEAREST}
 SH_C0 = 0.28209479177387814
 
 

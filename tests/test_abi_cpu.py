@@ -34,7 +34,7 @@ def test_sizes_and_errors_without_gpu():
     v = _lib.SgrView(); g = _lib.SgrGaussians()
     v.image_width, v.image_height, g.P = 0, 0, 5
     n = ctypes.c_int64(0)
-    cb = _lib.ALLOC_FN(lambda ctx, n: 0)
+    cb = _lib.SgrAlloc(lambda ctx, n: 0)
     rc = L.sgr_rasterize_forward(ctypes.byref(v), ctypes.byref(g), cb, None, cb, None, cb, None, None, None, 0,
                                  ctypes.byref(n), None)
     assert rc == -1 and b"bad sizes" in L.sgr_last_error()
@@ -82,7 +82,7 @@ def test_entry_points_validate_arguments_without_gpu():
     # the staged backward shares the plain one's validation
     v = _lib.SgrView(); g = _lib.SgrGaussians()
     v.image_width, v.image_height, g.P = 0, 0, 5
-    hook = _lib.STAGE_HOOK(lambda ctx, stage: None)
+    hook = _lib.SgrStageHook(lambda ctx, stage: None)
     plan = _lib.SgrBackwardPlan(hook=hook, num_chunks=4)
     assert L.sgr_rasterize_backward_staged(ctypes.byref(v), ctypes.byref(g), *([None] * 4), 0, *([None] * 11),
                                            ctypes.byref(plan)) == -1
@@ -103,12 +103,33 @@ def test_entry_points_validate_arguments_without_gpu():
 def test_struct_layouts_match_the_library():
     """The ctypes structs of the binding have the sizes the library was compiled with (sgr_struct_bytes)."""
     from sugar_b200 import _lib
-    for i, t in enumerate((_lib.SgrView, _lib.SgrGaussians, _lib.SgrBackwardPlan, _lib.SgrFieldParams)):
+    for i, t in enumerate((_lib.SgrView, _lib.SgrGaussians, _lib.SgrBackwardPlan, _lib.SgrFieldParams,
+                           _lib.SgrSsimParams, _lib.SgrDensifyGates, _lib.SgrDensifyColumn, _lib.SgrAdamSegment,
+                           _lib.SgrPeerPlan)):
         assert _lib.lib.sgr_struct_bytes(i) == ctypes.sizeof(t), t.__name__
-    assert _lib.lib.sgr_struct_bytes(8) == ctypes.sizeof(_lib.SgrPeerPlan)
     assert [f for f, _ in _lib.SgrBackwardPlan._fields_] == ["hook", "hook_ctx", "num_chunks", "reduce_records",
                                                               "dL_dsh_rest", "chunk_taper", "peer"]
-    assert _lib.lib.sgr_struct_bytes(99) == 0
+    assert _lib.lib.sgr_struct_bytes(9) == 0 and _lib.lib.sgr_struct_bytes(99) == 0
+
+
+def test_every_integer_define_is_exported():
+    from sugar_b200 import _lib
+    text = open(os.path.join(ROOT, "include", "sugar_b200.h")).read()
+    defines = re.findall(r"^#define[ \t]+(SGR_\w+)[ \t]+\(?(-?\d+)\)?", text, re.M)
+    assert len(defines) >= 15
+    for name, value in defines:
+        assert getattr(_lib, name, None) == int(value), name
+
+
+def test_header_parser_rejects_unknown_types():
+    """A type outside the binding's vocabulary is an import error that names its declaration, not a guessed width."""
+    import pytest
+    from sugar_b200 import _lib
+    for decl, what in (("SGR_API int sgr_bad(int32_t n, half_t *x);", "sgr_bad(half_t *x)"),
+                       ("typedef struct SgrBad { float a; bfloat16 b; } SgrBad;", "SgrBad.b"),
+                       ("SGR_API long sgr_long(void);", "sgr_long")):
+        with pytest.raises(_lib.SgrError, match=re.escape(what)):
+            _lib.parse_header(decl)
 
 
 def test_chunk_ranges_cover_and_halve():

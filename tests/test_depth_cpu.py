@@ -16,7 +16,7 @@ sys.path.insert(0, ROOT)
 def test_feature_entry_points_validate_arguments_without_gpu():
     from sugar_b200 import _lib
     L = _lib.lib
-    cb = _lib.ALLOC_FN(lambda ctx, n: 0)
+    cb = _lib.SgrAlloc(lambda ctx, n: 0)
     n = ctypes.c_int64(0)
     nz = ctypes.c_void_p(16)   # never dereferenced: every case below fails validation first
 
