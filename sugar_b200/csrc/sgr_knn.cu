@@ -4,8 +4,10 @@
 // tree; call sites: sugar_scene/sugar_model.py:1013-1030 `reset_neighbors` = knn_points(points,
 // points, K=16) every 500 iterations, and :1335-1343 `get_gaussians_closest_to_samples`).
 // Semantics kept: exact K nearest by squared Euclidean distance, results ordered by increasing
-// distance, int64 indices, a point is its own neighbour 0 when queries == points.  Ties may be
-// returned in a different order than pytorch3d (which does not define one).
+// distance, int64 indices.  Equal distances are ordered by index (pytorch3d defines no tie order), so
+// the result is a function of the input alone: with queries == points, neighbour 0 is the smallest
+// index at distance 0, the point itself unless it is duplicated.  The distance is knn_dist2's
+// (sgr_knn.cuh), rounded step by step, so a float32 brute force reproduces every row to the bit.
 //
 // Method: counting sort of the reference points into a grid of CUBIC cells over their bounding box
 // (per-axis cell counts nx x ny x nz <= N^3, the edge chosen on the device so that the cell count
@@ -253,6 +255,7 @@ __global__ void __launch_bounds__(128) knn_query_kernel(int Q, int K, int P, con
     int best_i[KNN_MAXK];
     int have = 0;
     float kth = 3.0e38f;
+    int kth_i = 0;
     const uint32_t total = (uint32_t)P;
     for (int r = 0; r < rmax; r++) {
         const int z0 = max(cz - r, 0), z1 = min(cz + r, nz - 1);
@@ -271,28 +274,31 @@ __global__ void __launch_bounds__(128) knn_query_kernel(int Q, int K, int P, con
                     const uint32_t e = (c + 1 < ncell) ? starts[c + 1] : total;
                     for (uint32_t k = s; k < e; k++) {
                         const float4 p = __ldg(sorted + k);
-                        const float dx = p.x - qx, dy = p.y - qy, dz = p.z - qz;
-                        const float d2 = dx * dx + dy * dy + dz * dz;
-                        if (have < K || d2 < kth) {
+                        const float d2 = knn_dist2(p.x, p.y, p.z, qx, qy, qz);
+                        const int id = __float_as_int(p.w);
+                        if (have < K || knn_before(d2, id, kth, kth_i)) {
                             int j = have < K ? have : K - 1;  // insertion position search from the back
-                            while (j > 0 && best_d[j - 1] > d2) {
+                            while (j > 0 && knn_before(d2, id, best_d[j - 1], best_i[j - 1])) {
                                 best_d[j] = best_d[j - 1];
                                 best_i[j] = best_i[j - 1];
                                 j--;
                             }
                             best_d[j] = d2;
-                            best_i[j] = __float_as_int(p.w);
+                            best_i[j] = id;
                             if (have < K) have++;
-                            if (have == K) kth = best_d[K - 1];
+                            if (have == K) {
+                                kth = best_d[K - 1];
+                                kth_i = best_i[K - 1];
+                            }
                         }
                     }
                 }
             }
         }
-        // every unvisited point lies beyond shell r: farther than r cell edges from the query's cell, hence
-        // from the query if it is inside the box; outside the box the query is even farther from them
-        const float bound = (float)r * g.h;
-        if (have == K && kth <= bound * bound) break;
+        // every unvisited point lies beyond shell r: farther than r cell edges from the query's cell (less the rounding
+        // margin), hence from the query if it is inside the box; outside the box the query is even farther from them
+        const float bound = knn_shell_radius(r, g.h);
+        if (have == K && kth < bound * bound) break;
     }
     for (int j = 0; j < K; j++) {
         idx_out[(size_t)q * K + j] = j < have ? (int64_t)best_i[j] : (int64_t)-1;
@@ -355,8 +361,8 @@ __global__ void __launch_bounds__(128) dist_cuda2_kernel(int P, const KnnGrid *_
                 }
             }
         }
-        // every unvisited point is farther than r cell edges (knn_query_kernel's bound, shrunk by a thousandth of an
-        // edge so that a coordinate rounded into a neighbouring cell cannot end the walk early)
+        // every unvisited point is farther than r cell edges less the rounding margin (knn_shell_radius's radius, spelt
+        // out here; only the three distances are returned, so their ties need no order)
         const float bound = fmaxf((float)r - 1e-3f, 0.0f) * g.h;
         if (have >= 3 && b2 <= bound * bound) break;
     }

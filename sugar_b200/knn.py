@@ -2,8 +2,12 @@
 SuGaR uses it (sugar_scene/sugar_model.py:1013-1030 reset_neighbors, :1335-1343).
 
     dists, idx = knn_points(queries, points, K)     # [Q,K] squared distances (ascending), [Q,K] int64
-    knn_dists, knn_idx = reset_neighbors(points, K=16)   # the tables SuGaR keeps (self is neighbour 0)
+    knn_dists, knn_idx = reset_neighbors(points, K=16)   # the tables SuGaR keeps (neighbour 0 is the smallest index
+                                                         # at distance 0: self unless the point is duplicated)
     dist2 = dist_cuda2(points)                       # simple-knn's distCUDA2: vanilla 3DGS's initial scales
+
+Equal distances come in index order, so every row is a function of the input alone; the distances are float32
+((dx*dx + dy*dy) + dz*dz) with d = point - query, each step rounded, which a float32 brute force reproduces to the bit.
 """
 import torch
 

@@ -1,6 +1,10 @@
 """Point clouds for the distCUDA2 goldens and tests, built from seeded CPU torch generators (the same values on every
 machine): a uniform cloud, a clustered one with exact duplicates, a planar one (a zero-extent axis), the sizes around
-simple-knn's 1024-point boxes, and the P <= 3 clouds whose FLT_MAX sentinels stay in the mean."""
+simple-knn's 1024-point boxes, the P <= 3 clouds whose FLT_MAX sentinels stay in the mean, a Gaussian bulk with 1%
+floaters 6 sigma to 1e4 sigma out on both sides of every axis (beyond the K-NN grid's 4-sigma clip), and a unit cloud
+centred far from the origin (coordinates quantised at 2^-13)."""
+import math
+
 import torch
 
 
@@ -20,6 +24,13 @@ def clouds():
     out["planar"] = plane
     for P in (4, 1023, 1024, 1025, 2049):
         out[f"p{P}"] = torch.randn(P, 3, generator=_g(100 + P))
+    bulk = torch.randn(30_000, 3, generator=_g(8))
+    F = 300
+    mag = 6.0 * torch.exp(torch.rand(F, generator=_g(9)) * math.log(1e4 / 6.0))
+    sign = torch.where((torch.arange(F) // 3) % 2 == 0, 1.0, -1.0)
+    bulk[torch.arange(F), torch.arange(F) % 3] = sign * mag
+    out["floaters"] = bulk[torch.randperm(30_000, generator=_g(10))].contiguous()
+    out["offset"] = torch.rand(30_000, 3, generator=_g(11)) - 0.5 + torch.tensor([3e3, -2e3, 1e3])
     for P in (1, 2, 3):
         out[f"p{P}"] = torch.randn(P, 3, generator=_g(200 + P))
     return out

@@ -47,25 +47,53 @@ def _far_cloud(P, seed):
     return [t.float().cuda() for t in (pts, sc, q, st)]
 
 
-def test_grid_density_equals_knn_plus_field_far_outside_the_cloud():
+def _far_grid():
     import torch
-    from sugar_b200 import field, knn, mcubes
-    pts, sc, q, st = _far_cloud(200_000, 3)
     R = 128
     X = torch.linspace(-1, 1, R) * 12.0
     Y = torch.linspace(-1, 1, R) * 9.0
     Z = torch.linspace(-1, 1, R) * 10.0 + 1.5
-    got = mcubes.density_grid(pts, sc, q, st, X, Y, Z).reshape(-1)
     xx, yy, zz = torch.meshgrid(X, Y, Z, indexing="ij")
-    grid = torch.stack([xx.reshape(-1), yy.reshape(-1), zz.reshape(-1)], -1).cuda()
-    d2, idx = knn.knn_points(grid, pts, 17)
-    want = field.compute_density(grid, idx[:, :16].contiguous(), pts, sc, q, st)
-    diff = got != want
-    tie = (d2[:, 1:] == d2[:, :-1]).any(1)      # equal distances within the 16 or at the 16th / 17th boundary
-    assert int((diff & ~tie).sum()) == 0
-    assert int(diff.sum()) <= 1e-4 * grid.shape[0]
-    rel = ((got - want).abs() / want.abs().clamp(min=1e-30))[diff]
-    assert rel.numel() == 0 or float(rel.max()) < 1e-5
+    return (X, Y, Z), torch.stack([xx.reshape(-1), yy.reshape(-1), zz.reshape(-1)], -1).cuda()
+
+
+def test_grid_density_equals_knn_plus_field_far_outside_the_cloud():
+    """The density grid's walk and knn_points share the distance, the (distance, index) order and the stop radius, so
+    every voxel, inside the grid's box or far outside it, equals compute_density over knn_points' neighbours to the
+    bit."""
+    import torch
+    from sugar_b200 import field, knn, mcubes
+    pts, sc, q, st = _far_cloud(200_000, 3)
+    axes, grid = _far_grid()
+    got = mcubes.density_grid(pts, sc, q, st, *axes).reshape(-1)
+    want = field.compute_density(grid, knn.knn_points(grid, pts, 16)[1], pts, sc, q, st)
+    diff = (got.view(torch.int32) != want.view(torch.int32)).nonzero()[:, 0]
+    assert diff.numel() == 0, (diff.numel(), diff[:5].tolist())
+
+
+def test_grid_density_equals_the_field_over_brute_force_neighbours():
+    """The same grid against neighbours that come from no grid walk: the float32 brute force (oracle/knn_oracle.py) on
+    voxels well inside the 4-sigma box, far outside it, and next to each floater."""
+    import torch
+    from oracle import knn_oracle as ko
+    from sugar_b200 import field, mcubes
+    pts, sc, q, st = _far_cloud(200_000, 3)
+    axes, grid = _far_grid()
+    got = mcubes.density_grid(pts, sc, q, st, *axes).reshape(-1)
+    p64 = pts.double()
+    mean, sd = p64.mean(0), p64.std(0)
+    z = ((grid.double() - mean) / sd).abs()
+    gen = torch.Generator(device="cuda").manual_seed(5)
+    pick = lambda m, k: m.nonzero()[:, 0][torch.randperm(int(m.sum()), generator=gen, device="cuda")[:k]]
+    inside, outside = pick((z < 3.5).all(1), 3000), pick((z > 5.0).any(1), 3000)
+    floaters = ((pts.double() - mean) / sd).abs().gt(4.0).any(1).nonzero()[:, 0]
+    near = ko.knn_f32(pts[floaters], grid, 8)[1].reshape(-1)      # the voxels around each floater
+    assert inside.numel() == outside.numel() == 3000 and floaters.numel() >= 10
+    sel = torch.cat([inside, outside, near]).unique()
+    idx = ko.knn_f32(grid[sel], pts, 16)[1]
+    want = field.compute_density(grid[sel], idx, pts, sc, q, st)
+    bad = (got[sel].view(torch.int32) != want.view(torch.int32)).nonzero()[:, 0]
+    assert bad.numel() == 0, (bad.numel(), sel[bad[:5]].tolist())
 
 
 def test_exclusion_box_writes_exact_zeros():
