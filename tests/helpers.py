@@ -74,9 +74,10 @@ def assert_digests(gold, got):
             assert np.array_equal(digest(got[field]), gold[k]), f"{field} not bit-identical to the reference build"
 
 
-def scene_kwargs(sc, use_sh=True, use_cov_precomp=False, sh_degree=3, cov3D=None):
+def scene_kwargs(sc, use_sh=True, use_cov_precomp=False, sh_degree=3, cov3D=None, scale_modifier=1.0):
     kw = dict(means3D=sc.means3D, opacities=sc.opacities, viewmatrix=sc.viewmatrix, projmatrix=sc.projmatrix,
-              campos=sc.campos, W=sc.width, H=sc.height, tanfovx=sc.tanfovx, tanfovy=sc.tanfovy, sh_degree=sh_degree)
+              campos=sc.campos, W=sc.width, H=sc.height, tanfovx=sc.tanfovx, tanfovy=sc.tanfovy, sh_degree=sh_degree,
+              scale_modifier=scale_modifier)
     if use_sh:
         kw["shs"] = sc.shs
     else:
@@ -183,7 +184,7 @@ def pad_culled(t, names, pad_to=PACKED_MAX_P):
 
 
 def run_module(mod, sc, bg, dL=None, use_sh=True, use_cov_precomp=False, sh_degree=3, cov3D=None, device="cuda",
-               debug=False, pad_to=None):
+               debug=False, pad_to=None, scale_modifier=1.0):
     """Run GaussianRasterizer of `mod` (ours or the reference build).  Returns dict with image, radii, grads and
     the saved opaque buffers.  pad_to: the Gaussians of `sc` followed by culled ones up to pad_to (pad_culled)."""
     import torch
@@ -196,8 +197,9 @@ def run_module(mod, sc, bg, dL=None, use_sh=True, use_cov_precomp=False, sh_degr
     means2D = torch.zeros_like(means3D, requires_grad=True)
     settings = mod.GaussianRasterizationSettings(
         image_height=sc.height, image_width=sc.width, tanfovx=sc.tanfovx, tanfovy=sc.tanfovy,
-        bg=torch.from_numpy(np.asarray(bg, np.float32)).to(device), scale_modifier=1.0, viewmatrix=t["viewmatrix"],
-        projmatrix=t["projmatrix"], sh_degree=sh_degree, campos=t["campos"], prefiltered=False, debug=debug)
+        bg=torch.from_numpy(np.asarray(bg, np.float32)).to(device), scale_modifier=scale_modifier,
+        viewmatrix=t["viewmatrix"], projmatrix=t["projmatrix"], sh_degree=sh_degree, campos=t["campos"],
+        prefiltered=False, debug=debug)
     rast = mod.GaussianRasterizer(raster_settings=settings)
     kw = {}
     leaves = dict(means3D=means3D, means2D=means2D, opacities=opac)

@@ -475,12 +475,17 @@ def test_raw_parameter_mode():
     the same blend accumulators against ref64, and the raw chain's rows against the activated chain (the oracle's,
     fed with the GPU's accumulators, on the activations evaluated in float64) taken through the activations'
     derivatives in float64: d sigmoid = o (1 - o), d exp = scale, normalisation as dnormvdv."""
+    from sugar_b200 import scenes
+    W, H = 200, 120
+    run_raw_mode("raw", scenes.make_scene(4000, W, H, seed=12, camera="posed"), (0.1, 0.2, 0.3),
+                 scenes.upstream_grad(W, H, seed=3))
+
+
+def run_raw_mode(label, sc, bg, dL, deg=3):
+    """test_raw_parameter_mode's checks on the scene `sc` (SH of degree `deg`, 16 coefficients)."""
     import torch
-    from sugar_b200 import _C, scenes
-    P, W, H, deg, M = 4000, 200, 120, 3, 16
-    bg = (0.1, 0.2, 0.3)
-    sc = scenes.make_scene(P, W, H, seed=12, camera="posed")
-    dL = scenes.upstream_grad(W, H, seed=3)
+    from sugar_b200 import _C
+    P, W, H, M = sc.means3D.shape[0], sc.width, sc.height, 16
     t = h.to_torch(sc)
     dens = torch.logit(t["opacities"].clamp(1e-4, 1 - 1e-4)).contiguous()
     s_raw = t["scales"].log().contiguous()
@@ -494,9 +499,9 @@ def test_raw_parameter_mode():
     f = dict(args=args, Pt=P, M=M, R=R, radii=radii, geom=geom, binning=binning, img=img)
     grads, gacc = _backward(f, dL, sh_rest=sh_rest)
     o32 = st["conic_opacity"][:, 3]
-    _check_record_copies("raw", gacc, grads, P, opacity_factor=o32 * (np.float32(1) - o32))
+    _check_record_copies(label, gacc, grads, P, opacity_factor=o32 * (np.float32(1) - o32))
     r = b64.blend_backward64(st, bg, dL, st["rgb"], clamped=st["clamped"])
-    rep = check_accumulators("raw", st, b64.gpu_accumulators(gacc, grads["colors"]), r)
+    rep = check_accumulators(label, st, b64.gpu_accumulators(gacc, grads["colors"]), r)
 
     # the activated counterpart, in float64, as the oracle's inputs
     d64, s64, q64 = (x.double().cpu().numpy() for x in (dens, s_raw, q_raw))
@@ -521,6 +526,7 @@ def test_raw_parameter_mode():
     nm, nc, no = _noisy(dm2d, dconic, gacc[:, 5])
     pert = raw_chain(nm, nc, no.astype(np.float64), op64 * (1 + 2.0 ** -23))
     rows = same & (rad > 0)
-    rep["chain"] = compare_rows("raw", want, pert, {k: grads[k] for k in want}, rows=rows)
+    rep["chain"] = compare_rows(label, want, pert, {k: grads[k] for k in want}, rows=rows)
     assert not any(grads[k][rad == 0].any() for k in want), "a culled Gaussian has raw gradients"
-    print(f"\n[grad_rows] raw_mode: {rep}")
+    print(f"\n[grad_rows] {label}: {rep}")
+    return rep
