@@ -76,6 +76,13 @@ def _forward(sc, bg, use_sh=False, sh_degree=0, use_cov_precomp=False, cov3D=Non
                 sh_degree=sh_degree)
 
 
+def scratch_accumulators(b, P):
+    """The blend accumulators [P, 8] in the scratch of _C._alloc_backward's buffers `b`, after a backward."""
+    base = b["scratch"].data_ptr()
+    off = ((base + 255) // 256 * 256 - base) // 4           # launch_backward: gacc = align_up(scratch, SGR_ALIGN)
+    return b["scratch"][off:off + 8 * P].view(P, 8)
+
+
 def _backward(f, dL, dD=None, sh_rest=None):
     """The backward on f's forward buffers, through the C entry point, with the test's scratch: (grads, gacc [P,8]).
     sh_rest: raw-parameter mode (sugar_b200/fused.py), the plan carries the second SH gradient array."""
@@ -107,9 +114,7 @@ def _backward(f, dL, dD=None, sh_rest=None):
         _lib.check(_lib.lib.sgr_rasterize_backward_staged(*inputs, *grads, b["scratch"].data_ptr(), stream,
                                                           None if plan is None else C.byref(plan)))
     torch.cuda.synchronize()
-    base = b["scratch"].data_ptr()
-    off = ((base + 255) // 256 * 256 - base) // 4           # launch_backward: gacc = align_up(scratch, SGR_ALIGN)
-    gacc = b["scratch"][off:off + 8 * Pt].view(Pt, 8)
+    gacc = scratch_accumulators(b, Pt)
     out = {k: b[k].cpu().numpy() for k in ("means2D", "colors", "opacity", "means3D", "cov3D", "scales", "rotations")}
     if M:
         out["sh"] = b["sh"].cpu().numpy()

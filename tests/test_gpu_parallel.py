@@ -207,72 +207,31 @@ def test_peer_exchange_with_three_emulated_ranks_and_nine_stored_coefficients():
 def check_peer_exchange_with_three_emulated_ranks(M, deg):
     """The peer-memory exchange (csrc/sgr_peer.cu) as rank 0 of THREE, on one GPU: ranks 1 and 2 are static stand-ins --
     their factor blocks and record arrays are filled from plain backwards of their views, their flag words are preset,
-    and this process reduces their record slices as well.  Everything the real multi-rank run executes runs here: the
-    flag waits, the per-Gaussian pass summing three views' SH gradients through the pointer table, the two-shot reduce
-    over three record arrays, the split.  The result must be scale x (sum of the three views' plain gradients)."""
-    import ctypes as C
+    and this process reduces their record slices as well (test_gpu_exchange_rows.emulate_peers).  Everything the real
+    multi-rank run executes runs here: the flag waits, the per-Gaussian pass summing three views' SH gradients through the
+    pointer table, the two-shot reduce over three record arrays, the split.  The result must be scale x (sum of the three
+    views' plain gradients)."""
     import torch
-    from sugar_b200 import _C, _lib, diff_gaussian_rasterization as mod
-    from sugar_b200 import parallel, scenes
-    P, W, H, scale = 6001, 160, 96, 0.25
-    base = scenes.make_scene(P, W, H, seed=41, camera="posed")
-    views = [base, scenes.with_camera_offset(base, 0.15, (0.3, -0.1, 0.2)),
-             scenes.with_camera_offset(base, -0.2, (-0.4, 0.2, 0.5))]
+    from sugar_b200 import diff_gaussian_rasterization as mod
+    import test_gpu_exchange_rows as ex
+    P, scale = 6001, 0.25
     names = ("means3D", "opacities", "shs", "scales", "rotations")
-    E = torch.Tensor([])
-    plain, factors, records = [], [], []
-
-    def to_torch(sc):
-        t = h.to_torch(sc)
-        t["shs"] = t["shs"][:, :M].contiguous()
-        return t
-    for v, sc in enumerate(views):
-        t = to_torch(sc)
-        dL = torch.from_numpy(scenes.upstream_grad(W, H, seed=5 + v)).cuda()
-        bg = torch.zeros(3, device="cuda")
-        R, color, radii, geom, binning, img = _C.rasterize_gaussians(
-            bg, t["means3D"], E, t["opacities"], t["scales"], t["rotations"], 1.0, E, t["viewmatrix"], t["projmatrix"],
-            sc.tanfovx, sc.tanfovy, H, W, t["shs"], deg, t["campos"], False, False)
-        g = _C.rasterize_gaussians_backward(bg, t["means3D"], radii, E, t["scales"], t["rotations"], 1.0, E,
-                                            t["viewmatrix"], t["projmatrix"], sc.tanfovx, sc.tanfovy, dL, t["shs"], deg,
-                                            t["campos"], geom, R, binning, img, False)
-        plain.append({"means3D": g[3].double(), "opacities": g[2].double(), "shs": g[5].double(), "scales": g[6].double(),
-                      "rotations": g[7].double()})
-        factors.append(torch.cat([g[1].reshape(-1), t["campos"].reshape(3), torch.zeros(1, device="cuda")]).contiguous())
-        records.append(torch.cat([g[3], g[2], g[6], g[7]], dim=1).contiguous())     # the 44-byte record layout
-    want = {k: scale * sum(p[k] for p in plain) for k in names}
-
-    vp = parallel.ViewParallel(chunks=3, scale=scale, force=True, peer=True)
-    vp._nstage = 3      # staging arrays for three source ranks in this (single) rank's buffer
-    st = vp._peer_state(_lib.lib, _lib.check, P, torch.device("cuda", torch.cuda.current_device()))
-    # stand-ins for ranks 1 and 2: their records sit in this rank's staging arrays 1 and 2 (as if their per-Gaussian
-    # passes had stored them), their sum arrays are plain local tensors, their factor blocks are static
-    stage = lambda j: torch.as_tensor(parallel._DevMem(st.base + st.off["STAGE"] + j * st.stage_stride, 11 * P),
-                                      device="cuda")
-    stage(1).copy_(records[1].reshape(-1))
-    stage(2).copy_(records[2].reshape(-1))
-    S_fake = [torch.zeros(11 * P + 16, device="cuda"), torch.zeros(11 * P + 16, device="cuda")]
-    tab = lambda own, others: torch.tensor([int(own)] + [o.data_ptr() for o in others], dtype=torch.int64, device="cuda")
-    st.world = 3
-    st.F_tab = [tab(st.F_tab[0][0], factors[1:]), tab(st.F_tab[1][0], factors[1:])]
-    st.S_tab = tab(st.S_tab[0], S_fake)
-    st.stage_tab = torch.tensor([st.R_ptr] * 3, dtype=torch.int64, device="cuda")   # every owner's array for OUR records = ours
-    st.flag_tab = torch.tensor([st.base] * 3, dtype=torch.int64, device="cuda")   # "every rank's flags" = ours
-    flags = torch.as_tensor(type("M", (), {"__cuda_array_interface__": {
-        "shape": (64, 64), "typestr": "<i4", "data": (st.base, False), "version": 2}})(), device="cuda")
-    flags[:63, 1:3] = 1 << 30   # ranks 1 and 2 have "already signalled" every slot of every step (row 63: CTA counters)
-    vp._emulated = (1, 2)
-    t0, sc0 = to_torch(views[0]), views[0]
-    dL0 = torch.from_numpy(scenes.upstream_grad(W, H, seed=5)).cuda()
-    for step in range(2):       # both factor-block parities
-        ps = {k: t0[k].clone().requires_grad_(True) for k in names}
-        with vp.context():
-            loss, _ = _render_loss(mod, t0, sc0, dL0, deg, ps, bg=(0.0, 0.0, 0.0))
-            loss.backward()
-        for k in names:
-            assert _err(ps[k].grad, want[k].float()) <= 1e-4, (step, k)
-        for S in S_fake:        # every rank's sum array received every slice
-            assert _err(S[:11 * P], (records[0].double() + records[1].double() + records[2].double()).float().reshape(-1)) <= 1e-4
-    torch.cuda.synchronize()
-    st.world = 1
-    vp.close()
+    em = ex.emulate_peers(3, 0, M, deg, chunks=3, taper=True, scale=scale, P=P, seed=41)
+    try:
+        plain = [{"means3D": g[3].double(), "opacities": g[2].double(), "shs": g[5].double(), "scales": g[6].double(),
+                  "rotations": g[7].double()} for g in em.plain]
+        want = {k: scale * sum(p[k] for p in plain) for k in names}
+        records = em.records
+        t0, sc0 = h.to_torch(em.views[0]), em.views[0]
+        dL0 = torch.from_numpy(em.dL[0]).cuda()
+        for step in range(2):       # both factor-block parities
+            ps = {k: t0[k].clone().requires_grad_(True) for k in names}
+            with em.vp.context():
+                loss, _ = _render_loss(mod, t0, sc0, dL0, deg, ps, bg=(0.0, 0.0, 0.0))
+                loss.backward()
+            for k in names:
+                assert _err(ps[k].grad, want[k].float()) <= 1e-4, (step, k)
+            for S in em.S_others.values():        # every rank's sum array received every slice
+                assert _err(S[:11 * P], (records[0].double() + records[1].double() + records[2].double()).float().reshape(-1)) <= 1e-4
+    finally:
+        em.close()
