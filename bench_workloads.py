@@ -35,6 +35,7 @@ def reference_ops(torch, ref_mod):
     from oracle import densest_oracle as deo
     from oracle import field_oracle as fo
     from oracle import meshbind_oracle as mo
+    from oracle import meshlap_oracle as lo
     from oracle import meshloss_oracle as mlo
     from oracle import ssim_oracle as so
 
@@ -49,7 +50,10 @@ def reference_ops(torch, ref_mod):
         better_normal_loss=fo.better_normal_loss_torch, bind_to_mesh=bind, l1_dssim=so.l1_dssim_torch,
         density_estimation_loss=deo.density_estimation_loss_torch,
         # pytorch3d's cost: a new Meshes every call (edges rebuilt) and its Python pair loop; no cached topology
-        mesh_normal_consistency=lambda verts, faces, topology=None: mlo.mesh_normal_consistency_torch(verts, faces))
+        mesh_normal_consistency=lambda verts, faces, topology=None: mlo.mesh_normal_consistency_torch(verts, faces),
+        # a new Meshes every call: the sparse Laplacian rebuilt from the faces (and the moving vertices for cot)
+        mesh_laplacian_smoothing=lambda verts, faces, method, topology=None:
+            lo.mesh_laplacian_smoothing_torch(verts, faces, method))
 
 
 def run(args, scenes, load_peaks, ClockSampler, cpu_density_baseline):

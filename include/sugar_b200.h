@@ -502,6 +502,40 @@ SGR_API int sgr_mesh_nc_backward(int32_t Q, int32_t V, const float *verts, const
                                  void *scratch, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Mesh Laplacian smoothing of the refinement stage (sugar_trainers/refine.py:163-171, 778-780: pytorch3d 0.7.4
+ * mesh_laplacian_smoothing of the one surface mesh, off by default there): loss = sum_v |y_v| / V over every vertex,
+ *   uniform  y = L x                                L[i,j] = 1 / deg_i per unique-edge entry, L[i,i] -= 1
+ *   cot      y = (L x) norm_w - x                   L the cotangent Laplacian, norm_w = 1 / rowsum(L) where > 0
+ *   cotcurv  y = (L x - rowsum(L) x) 0.25 inv_area  inv_area = 1 / (the areas of the faces on v) where > 0, else 0
+ * L is a constant (no gradient through it), computed from a topology built once (sugar_b200/meshloss.py:
+ * laplacian_topology):
+ *   verts    f32[V,3]
+ *   faces    i32[F,3]                          (cot / cotcurv; not read for uniform)
+ *   vert_ptr i32[V+1], vert_inc               uniform: the neighbours of each vertex, i32[2E] over the E unique
+ *                                              edges, a self-loop (v, v) listed twice; cot / cotcurv: the entries
+ *                                              3 f + k of the face corners at each vertex, i32[3F]; ascending (CSR)
+ *   face_w   f32[F,4]   (cot / cotcurv) written by the forward, read by the backward: (cot_a, cot_b, cot_c) / 4 and
+ *                        the clamped Heron area of each face, in pytorch3d's float32 order
+ *   vert_ys  f32[V,4]   written by the forward, read by the backward: y_v and the row's scale (1 / deg, norm_w or
+ *                        0.25 inv_area)
+ *   partials f64[SGR_MESH_LAP_PARTIALS]   scratch
+ *   loss     f32[1]     the mean; summed in double in a fixed order (run-to-run identical)
+ * Backward: g_loss f32[1] (DEVICE: the upstream gradient) -> g_verts f32[V,3], fully written; each vertex gathers its
+ * CSR list in order (run-to-run identical); rows with y_v = 0 contribute no gradient.  No host synchronisation.
+ * Limits: V > 0, 0 < F <= (2^31 - 1) / 3.
+ * ------------------------------------------------------------------------------------------ */
+#define SGR_MESH_LAP_UNIFORM 0
+#define SGR_MESH_LAP_COT 1
+#define SGR_MESH_LAP_COTCURV 2
+#define SGR_MESH_LAP_PARTIALS 1024
+SGR_API int sgr_mesh_lap_forward(int32_t method, int32_t V, int32_t F, const float *verts, const int32_t *faces,
+                                 const int32_t *vert_ptr, const int32_t *vert_inc, float *face_w, float *vert_ys,
+                                 double *partials, float *loss, void *stream);
+SGR_API int sgr_mesh_lap_backward(int32_t method, int32_t V, int32_t F, const int32_t *faces, const int32_t *vert_ptr,
+                                  const int32_t *vert_inc, const float *face_w, const float *vert_ys,
+                                  const float *g_loss, float *g_verts, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Border-face erosion of the refined mesh (postprocess_mesh, sugar_extractors/refined_mesh.py:140-147): `iterations`
  * rounds, each one launch on `stream`, no host synchronisation.  Entry 3 f + m is edge m of face f, (0,1), (1,2),
  * (2,0); the entries are grouped in runs of equal (unordered) edges, built once per call by the caller

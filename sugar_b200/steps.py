@@ -30,6 +30,8 @@ fused kernels and over the reference's own building blocks (its CUDA rasterizer 
                                 return_closest_gaussian_opacities=True) -> ([N], [N,K])   (coarse_density_step)
     ops.l1_dssim(pred, gt, dssim_factor) -> scalar   (only called with dssim_factor > 0)
     ops.mesh_normal_consistency(verts, faces, topology) -> scalar   (only called with normal_consistency_factor > 0)
+    ops.mesh_laplacian_smoothing(verts, faces, method, topology) -> scalar   (only called with
+                               laplacian_smoothing_factor > 0)
     ops.rasterize_with_depth   sugar_b200.depth.rasterize_with_depth (only called with fused_depth=True; the
                                reference has no counterpart)
 
@@ -219,20 +221,28 @@ def coarse_density_step(raw, cam, gt_rgb, knn_idx, ops, n_samples=1_000_000, den
     return loss.detach(), stats
 
 
-def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0, normal_consistency_factor=0.0, sh_deg=3):
+def refine_step(raw, mesh, cam, gt_rgb, ops, backward=True, dssim_factor=0.0, normal_consistency_factor=0.0, sh_deg=3,
+                laplacian_smoothing_factor=0.0, laplacian_smoothing_method="uniform"):
     """One refinement iteration's render for mesh-bound Gaussians (sugar_trainers/refine.py; model properties
     sugar_model.py:384-398 points, :415-441 scaling, :443-479 quaternions).  `raw`: verts [V,3], sh_dc, sh_rest,
     densities [P,1], scales [P,2] (in-plane), quaternions [P,2] (the learned 2-D rotation as a complex number);
     `mesh`: faces [F,3] int64, bary [n,3,1], thickness, optionally `topology` (meshloss.mesh_topology of the faces,
     built once); P = F * n.  normal_consistency_factor > 0 adds the surface mesh's normal consistency
-    (refine.py:775-783, 0.1 in the trainers) through ops.mesh_normal_consistency.  `sh_deg`: the SH degree rendered
-    (the refinement's warm-up raises it from 0 to 3, train.refine_sh_degree)."""
+    (refine.py:775-783, 0.1 in the trainers) through ops.mesh_normal_consistency.  laplacian_smoothing_factor > 0 adds
+    the surface mesh's Laplacian smoothing with `laplacian_smoothing_method` ("uniform", "cot" or "cotcurv"; refine.py:
+    163-171, 778-780, off in the trainers, factor 5 when on) through ops.mesh_laplacian_smoothing, before the normal
+    consistency term as refine.py orders them, reading the optional `mesh.laplacian_topology`
+    (meshloss.laplacian_topology of the faces).  `sh_deg`: the SH degree rendered (the refinement's warm-up raises it
+    from 0 to 3, train.refine_sh_degree)."""
     a = ops.bind_to_mesh(raw["verts"], mesh.faces, mesh.bary, raw["scales"], raw["quaternions"], mesh.thickness)
     b = SimpleNamespace(points=a.points, scaling=a.scaling, quaternions=a.quaternions,
                         strengths=torch.sigmoid(raw["densities"]).view(-1, 1),
                         sh=torch.cat([raw["sh_dc"], raw["sh_rest"]], dim=1))
     image, radii, _ = render(ops, b, cam, torch.zeros(3, device=b.points.device), sh_deg=sh_deg)
     loss = photometric_loss(ops, image, gt_rgb, dssim_factor)
+    if laplacian_smoothing_factor > 0.0:
+        loss = loss + laplacian_smoothing_factor * ops.mesh_laplacian_smoothing(
+            raw["verts"], mesh.faces, laplacian_smoothing_method, getattr(mesh, "laplacian_topology", None))
     if normal_consistency_factor > 0.0:
         loss = loss + normal_consistency_factor * ops.mesh_normal_consistency(raw["verts"], mesh.faces,
                                                                               getattr(mesh, "topology", None))
@@ -250,7 +260,8 @@ def camera_from_scene(sc, device):
 
 def ours_ops():
     """This package's operators: in-kernel SH colours, fused field / normal-loss / density-estimation kernels, fused
-    mesh binding, fused L1 + D-SSIM loss, fused mesh normal consistency, colour + depth in one rasterizer call."""
+    mesh binding, fused L1 + D-SSIM loss, fused mesh normal consistency and Laplacian smoothing, colour + depth in one
+    rasterizer call."""
     from . import diff_gaussian_rasterization as dgr
     from . import depth, field, loss, meshbind, meshloss
     return SimpleNamespace(rasterizer=dgr, colors=lambda points, sh, campos, deg: None,
@@ -258,4 +269,5 @@ def ours_ops():
                            field_values=field.field_values, better_normal_loss=field.better_normal_loss,
                            density_estimation_loss=field.density_estimation_loss,
                            bind_to_mesh=meshbind.bind_to_mesh, l1_dssim=loss.l1_dssim_loss,
-                           mesh_normal_consistency=meshloss.mesh_normal_consistency)
+                           mesh_normal_consistency=meshloss.mesh_normal_consistency,
+                           mesh_laplacian_smoothing=meshloss.mesh_laplacian_smoothing)

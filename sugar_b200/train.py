@@ -178,11 +178,14 @@ def train_coarse(raw, views, knn_idx, mode="sdf", spatial_extent=None, num_itera
 
 def train_refined(raw, mesh, views, spatial_lr_scale, num_iterations=15_000, dssim_factor=0.2,
                   normal_consistency_factor=0.1, sh_warmup_every=1000, generator=None, on_iteration=None,
-                  first_iteration=1, optimizer=None):
+                  first_iteration=1, optimizer=None, laplacian_smoothing_factor=0.0,
+                  laplacian_smoothing_method="uniform"):
     """The refinement's loop (see the module docstring).  `raw`: steps.refine_step's dict (verts, sh_dc, sh_rest,
     densities, scales [P,2], quaternions [P,2]; leaf tensors, updated in place); `mesh` as refine_step takes it (give it
-    a `topology` to build the edge table once); `spatial_lr_scale` from refine_spatial_lr_scale; `first_iteration` and
-    `optimizer` (a bound SugarOptimizer over `raw`) as train_coarse takes them.  -> the SugarOptimizer (bound)."""
+    a `topology` to build the edge table once, a `laplacian_topology` for the Laplacian lists); `spatial_lr_scale` from
+    refine_spatial_lr_scale; `first_iteration` and `optimizer` (a bound SugarOptimizer over `raw`) as train_coarse takes
+    them; laplacian_smoothing_factor / _method as refine_step takes them (refine.py's switch, off by default).
+    -> the SugarOptimizer (bound)."""
     if len(views) == 0:
         raise ValueError("views is empty")
     if not spatial_lr_scale > 0:
@@ -197,7 +200,9 @@ def train_refined(raw, mesh, views, spatial_lr_scale, num_iterations=15_000, dss
         optimizer.update_learning_rate(it)
         ev = refine_phase(it, sh_warmup_every)
         loss, _ = steps.refine_step(raw, mesh, cam, gt, ops, dssim_factor=dssim_factor,
-                                    normal_consistency_factor=normal_consistency_factor, sh_deg=ev["sh_degree"])
+                                    normal_consistency_factor=normal_consistency_factor, sh_deg=ev["sh_degree"],
+                                    laplacian_smoothing_factor=laplacian_smoothing_factor,
+                                    laplacian_smoothing_method=laplacian_smoothing_method)
         optimizer.step()
         optimizer.zero_grad(set_to_none=True)
         if on_iteration is not None:
