@@ -24,7 +24,8 @@
 // After the loop the vertices that a face references are compacted in order and written as float32.
 #include <math.h>
 
-#include "sgr_knn.cuh"
+#include "sgr_reduce.cuh"
+#include "sgr_scan.cuh"
 
 namespace sgr {
 
@@ -419,7 +420,7 @@ __global__ void __launch_bounds__(256) dec_pass_list_kernel(int V, const uint8_t
 
 __device__ unsigned long long block_sum_u64(unsigned long long x, unsigned long long *s_w)
 {
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    x = warp_sum(x);
     __syncthreads();
     if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = x;
     __syncthreads();
@@ -621,7 +622,7 @@ static int build_csr(int V, int F, const DecScratch &s, const int *fc, cudaStrea
 {
     SGR_CUDA(cudaMemsetAsync(s.vcnt, 0, ((size_t)V + 1) * 4, st));
     if (F) SGR_LAUNCH(K_MISC, st, dec_count_kernel<<<grid(3 * (size_t)F, 256), 256, 0, st>>>(3 * F, fc, s.vcnt));
-    exclusive_scan_u32(K_MISC, V + 1, s.vcnt, s.vstart, s.bsums, s.vcnt, st);
+    exclusive_scan(K_MISC, V + 1, s.vcnt, s.vstart, s.bsums, s.vcnt, st);
     if (F) SGR_LAUNCH(K_MISC, st, dec_scatter_kernel<<<grid(3 * (size_t)F, 256), 256, 0, st>>>(3 * F, fc, s.vcnt, s.csr));
     SGR_LAUNCH(K_MISC, st, dec_sort_kernel<<<grid(V, 256), 256, 0, st>>>(V, s.vstart, s.csr));
     return SGR_OK;
@@ -701,7 +702,7 @@ int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *verts, const
         const bool cutoff = ctr[2] >= need;
         if (cutoff) {
             SGR_LAUNCH(K_MISC, st, dec_pass_flags_kernel<<<grid(V, 256), 256, 0, st>>>(V, s.state, s.fflag));
-            exclusive_scan_u32(K_MISC, V, s.fflag, s.fflag, s.bsums, s.fflag, st);
+            exclusive_scan(K_MISC, V, s.fflag, s.fflag, s.bsums, s.fflag, st);
             SGR_LAUNCH(K_MISC, st, dec_pass_list_kernel<<<grid(V, 256), 256, 0, st>>>(V, s.state, s.fflag, s.vmin, s.removed,
                                                                                      s.list));
             SGR_LAUNCH(K_MISC, st, dec_cutoff_kernel<<<1, 1024, 0, st>>>((uint32_t)ctr[1], s.list, need, s.ctr));
@@ -712,7 +713,7 @@ int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *verts, const
                            s.pos, s.Q, col, nrm};
         SGR_LAUNCH(K_MISC, st, dec_apply_kernel<<<grid(V, 256), 256, 0, st>>>(aa));
         SGR_LAUNCH(K_MISC, st, dec_face_flags_kernel<<<grid(Fc, 256), 256, 0, st>>>(Fc, s.fc[cur], s.fflag));
-        exclusive_scan_u32(K_MISC, Fc, s.fflag, s.fflag, s.bsums, s.fflag, st);
+        exclusive_scan(K_MISC, Fc, s.fflag, s.fflag, s.bsums, s.fflag, st);
         SGR_LAUNCH(K_MISC, st, dec_face_scatter_kernel<<<grid(Fc, 256), 256, 0, st>>>(Fc, s.fc[cur], s.blk[cur], s.fflag,
                                                                                       s.fc[cur ^ 1], s.blk[cur ^ 1]));
         cur ^= 1;
@@ -727,7 +728,7 @@ int sgr_decimate(int32_t V, int32_t F, int64_t target, const float *verts, const
     // the vertices that a face references, in order
     SGR_CUDA(cudaMemsetAsync(s.vcnt, 0, ((size_t)V + 1) * 4, st));
     if (Fc) SGR_LAUNCH(K_MISC, st, dec_mark_kernel<<<grid(3 * (size_t)Fc, 256), 256, 0, st>>>(3 * Fc, s.fc[cur], s.vcnt));
-    exclusive_scan_u32(K_MISC, V + 1, s.vcnt, s.vstart, s.bsums, s.vcnt, st);
+    exclusive_scan(K_MISC, V + 1, s.vcnt, s.vstart, s.bsums, s.vcnt, st);
     SGR_LAUNCH(K_MISC, st, dec_out_verts_kernel<<<grid(V, 256), 256, 0, st>>>(V, s.vstart, s.pos, col, nrm, verts_out,
                                                                              colors_out, normals_out));
     if (Fc) SGR_LAUNCH(K_MISC, st, dec_out_faces_kernel<<<grid(3 * (size_t)Fc, 256), 256, 0, st>>>(3 * Fc, s.fc[cur], s.vstart,

@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "sgr_internal.cuh"
+#include "sgr_reduce.cuh"
 #include "sgr_sh.cuh"
 
 namespace sgr {
@@ -309,21 +310,11 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(const uint32_t *__restr
             v[k] = (i0 + k < T) ? count[i0 + k] : 0u;
             sum += v[k];
         }
-        uint32_t inc = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
+        const uint32_t inc = warp_inclusive_scan(sum);
         if (lane == 31) s_warp[wid] = inc;
         __syncthreads();
         if (wid == 0) {
-            uint32_t w = s_warp[lane], winc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc += t;
-            }
+            const uint32_t w = s_warp[lane], winc = warp_inclusive_scan(w);
             s_warp[lane] = winc - w;  // exclusive
         }
         __syncthreads();
@@ -352,21 +343,11 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(const uint32_t *__restr
     __syncthreads();
     {
         const uint32_t c = s_class[tid];
-        uint32_t inc = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
+        const uint32_t inc = warp_inclusive_scan(c);
         if (lane == 31) s_warp[wid] = inc;
         __syncthreads();
         if (wid == 0) {
-            uint32_t w = s_warp[lane], winc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc += t;
-            }
+            const uint32_t w = s_warp[lane], winc = warp_inclusive_scan(w);
             s_warp[lane] = winc - w;
         }
         __syncthreads();
@@ -577,12 +558,7 @@ __global__ void __launch_bounds__(GSORT_T) tile_sort_global_kernel(const uint32_
 #pragma unroll 4
                 for (int w = 0; w < NW; w++) tot += s_hist[w][tid];
             }
-            uint32_t inc = tot;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-                if (lane >= o) inc += t;
-            }
+            const uint32_t inc = warp_inclusive_scan(tot);
             if (tid < 256 && lane == 31) s_wsum[wid] = inc;
             __syncthreads();
             if (tid < 256) {
@@ -799,12 +775,7 @@ __global__ void __launch_bounds__(BK_T) tile_sort_bucket_kernel(const uint32_t *
                 cm = max(cm, c[k]);
             }
             cm = __reduce_max_sync(0xffffffffu, cm);
-            uint32_t inc = sum;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-                if (lane >= o) inc += t;
-            }
+            const uint32_t inc = warp_inclusive_scan(sum);
             if (lane == 31) s_wsum[wid] = inc;
             if (lane == 0) atomicMax(&s_red[2], cm);
             __syncthreads();

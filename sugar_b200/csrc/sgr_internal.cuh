@@ -414,16 +414,6 @@ __device__ __forceinline__ uint32_t block_mask_of_record(float x, float y, float
 // strict: id 0xffffff with mask 0xff would read as the "no record" word
 inline bool ids_packed(int P) { return P < SGR_PACKED_MAX_P; }
 
-__device__ __forceinline__ float warp_sum(float v)
-{
-    v += __shfl_xor_sync(0xffffffffu, v, 16);
-    v += __shfl_xor_sync(0xffffffffu, v, 8);
-    v += __shfl_xor_sync(0xffffffffu, v, 4);
-    v += __shfl_xor_sync(0xffffffffu, v, 2);
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    return v;
-}
-
 // one 16-byte vector reduction into global memory (SASS REDG.E.ADD.F32x4)
 __device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d)
 {

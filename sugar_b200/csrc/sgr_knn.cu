@@ -20,6 +20,8 @@
 #include <math.h>
 
 #include "sgr_knn.cuh"
+#include "sgr_reduce.cuh"
+#include "sgr_scan.cuh"
 
 namespace sgr {
 
@@ -57,11 +59,8 @@ __global__ void __launch_bounds__(256) knn_bbox_kernel(int P, const float *__res
     for (int a = 0; a < 3; a++) {
         const int lo = __reduce_min_sync(0xffffffffu, float_flip(mn[a]));
         const int hi = __reduce_max_sync(0xffffffffu, float_flip(mx[a]));
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            s1[a] += __shfl_xor_sync(0xffffffffu, s1[a], o);
-            s2[a] += __shfl_xor_sync(0xffffffffu, s2[a], o);
-        }
+        s1[a] = warp_sum(s1[a]);
+        s2[a] = warp_sum(s2[a]);
         if ((threadIdx.x & 31) == 0) {
             atomicMin(&bb[a], lo);
             atomicMax(&bb[3 + a], hi);
@@ -131,98 +130,6 @@ __global__ void __launch_bounds__(256) knn_count_kernel(int P, const float *__re
     const uint32_t c = ((uint32_t)cz * g.n[1] + cy) * g.n[0] + cx;
     cell_of[i] = c;
     atomicAdd(&counts[c], 1u);
-}
-
-// three-kernel exclusive scan over the cell counts (block = 1024 threads x 4 cells); in place is safe: a thread loads
-// its four counts before the block barrier and stores their offsets after it
-__global__ void __launch_bounds__(1024) knn_scan_blocks_kernel(int ncell, const uint32_t *__restrict__ counts,
-                                                               uint32_t *__restrict__ starts, uint32_t *__restrict__ block_sums)
-{
-    __shared__ uint32_t s_w[32];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int i0 = (blockIdx.x * 1024 + tid) * 4;
-    uint32_t v[4], sum = 0;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        v[k] = (i0 + k < ncell) ? counts[i0 + k] : 0u;
-        sum += v[k];
-    }
-    uint32_t inc = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-    }
-    if (lane == 31) s_w[wid] = inc;
-    __syncthreads();
-    if (wid == 0) {
-        uint32_t w = s_w[lane], wi = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xffffffffu, wi, o);
-            if (lane >= o) wi += t;
-        }
-        s_w[lane] = wi - w;
-        if (lane == 31) block_sums[blockIdx.x] = wi;
-    }
-    __syncthreads();
-    uint32_t ex = s_w[wid] + inc - sum;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        if (i0 + k < ncell) starts[i0 + k] = ex;
-        ex += v[k];
-    }
-}
-
-__global__ void __launch_bounds__(1024) knn_scan_sums_kernel(int nblocks, uint32_t *block_sums)
-{
-    // single CTA, serial over chunks of 1024 (nblocks <= 4096 for 2^24 cells)
-    __shared__ uint32_t s_w[32];
-    __shared__ uint32_t s_carry;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (tid == 0) s_carry = 0;
-    __syncthreads();
-    for (int base = 0; base < nblocks; base += 1024) {
-        const uint32_t v = (base + tid < nblocks) ? block_sums[base + tid] : 0u;
-        uint32_t inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
-        if (lane == 31) s_w[wid] = inc;
-        __syncthreads();
-        if (wid == 0) {
-            uint32_t w = s_w[lane], wi = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, wi, o);
-                if (lane >= o) wi += t;
-            }
-            s_w[lane] = wi - w;
-        }
-        __syncthreads();
-        const uint32_t ex = s_carry + s_w[wid] + inc - v;
-        if (base + tid < nblocks) block_sums[base + tid] = ex;
-        __syncthreads();
-        if (tid == 1023) s_carry = ex + v;
-        __syncthreads();
-    }
-}
-
-__global__ void __launch_bounds__(1024) knn_scan_add_kernel(int ncell, uint32_t *__restrict__ starts,
-                                                            const uint32_t *__restrict__ block_sums,
-                                                            uint32_t *__restrict__ cursor)
-{
-    const int i0 = (blockIdx.x * 1024 + threadIdx.x) * 4;
-    const uint32_t add = block_sums[blockIdx.x];
-#pragma unroll
-    for (int k = 0; k < 4; k++)
-        if (i0 + k < ncell) {
-            const uint32_t s = starts[i0 + k] + add;
-            starts[i0 + k] = s;
-            cursor[i0 + k] = s;
-        }
 }
 
 __global__ void __launch_bounds__(256) knn_scatter_kernel(int P, const float *__restrict__ pts,
@@ -393,15 +300,6 @@ KnnCellsScratch knn_cells_scratch(Layout &l, int P)
     return s;
 }
 
-void exclusive_scan_u32(int kind, int n, const uint32_t *counts, uint32_t *starts, uint32_t *block_sums,
-                        uint32_t *cursor, cudaStream_t st)
-{
-    const int nblocks = (int)(((size_t)n + 4095) / 4096);
-    SGR_LAUNCH(kind, st, knn_scan_blocks_kernel<<<(unsigned)nblocks, 1024, 0, st>>>(n, counts, starts, block_sums));
-    SGR_LAUNCH(kind, st, knn_scan_sums_kernel<<<1, 1024, 0, st>>>(nblocks, block_sums));
-    SGR_LAUNCH(kind, st, knn_scan_add_kernel<<<(unsigned)nblocks, 1024, 0, st>>>(n, starts, block_sums, cursor));
-}
-
 int knn_build_cells(int P, const float *points, const KnnCellsScratch &ws, cudaStream_t st, KnnCells *out)
 {
     const int n = knn_axis_cells(P);
@@ -411,7 +309,7 @@ int knn_build_cells(int P, const float *points, const KnnCellsScratch &ws, cudaS
     SGR_LAUNCH(K_KNN, st, knn_grid_setup_kernel<<<1, 32, 0, st>>>(ws.bbox, n, P, ws.grid));
     SGR_CUDA(cudaMemsetAsync(ws.cursor, 0, ncell * 4, st));  // cursor doubles as the count array first
     SGR_LAUNCH(K_KNN, st, knn_count_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, ws.grid, ws.cell_of, ws.cursor));
-    exclusive_scan_u32(K_KNN, (int)ncell, ws.cursor, ws.starts, ws.bsums, ws.cursor, st);
+    exclusive_scan(K_KNN, ncell, ws.cursor, ws.starts, ws.bsums, ws.cursor, st);
     SGR_LAUNCH(K_KNN, st, knn_scatter_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, points, ws.cell_of, ws.cursor, ws.sorted));
     out->grid = ws.grid;
     out->starts = ws.starts;

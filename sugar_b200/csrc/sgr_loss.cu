@@ -18,6 +18,7 @@
 // away from float64.  The passes read their double operands from shared memory once per tap, which (not HBM)
 // bounds both kernels; DESIGN sections 3 and 9 have the numbers and the next steps.
 #include "sgr_internal.cuh"
+#include "sgr_reduce.cuh"
 
 namespace sgr {
 
@@ -32,13 +33,6 @@ struct LossConsts {
 };
 
 constexpr size_t LOSS_FWD_SMEM = (size_t)(2 * LSY * LSX + 5 * LSY * LT_X) * sizeof(double);
-
-__device__ __forceinline__ double warp_sum_d(double v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 __global__ void __launch_bounds__(L_THREADS) loss_forward_kernel(const LossConsts k, const float *__restrict__ img1,
                                                                  const float *__restrict__ img2,
@@ -119,19 +113,9 @@ __global__ void __launch_bounds__(L_THREADS) loss_forward_kernel(const LossConst
         sum_s += S;
         sum_l1 += fabs(sx[so] - sy[so]);
     }
-    sum_s = warp_sum_d(sum_s);
-    sum_l1 = warp_sum_d(sum_l1);
-    if (tx == 0) {
-        red[0][ty] = sum_l1;
-        red[1][ty] = sum_s;
-    }
-    __syncthreads();
+    const double l = cta_sum_by_warps<L_THREADS>(sum_l1, red[0]);
+    const double s = cta_sum_by_warps<L_THREADS>(sum_s, red[1]);
     if (tid == 0) {
-        double l = 0.0, s = 0.0;
-        for (int w = 0; w < L_THREADS / 32; w++) {
-            l += red[0][w];
-            s += red[1][w];
-        }
         const size_t tile = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
         partials[tile] = make_double2(l, s);
     }
@@ -142,27 +126,12 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(int pairs_per_image, d
                                                           const double2 *__restrict__ partials, float *__restrict__ out)
 {
     __shared__ double r0[256], r1[256];
-    const int t = threadIdx.x;
-    const double2 *p = partials + (size_t)blockIdx.x * pairs_per_image;
-    double l = 0.0, s = 0.0;
-    for (int i = t; i < pairs_per_image; i += 256) {
-        const double2 v = p[i];
-        l += v.x;
-        s += v.y;
-    }
-    r0[t] = l;
-    r1[t] = s;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if (t < o) {
-            r0[t] += r0[t + o];
-            r1[t] += r1[t + o];
-        }
-        __syncthreads();
-    }
-    if (t == 0) {
-        out[2 * blockIdx.x] = (float)(r0[0] * inv_n);
-        out[2 * blockIdx.x + 1] = (float)(r1[0] * inv_n);
+    const double *p = (const double *)(partials + (size_t)blockIdx.x * pairs_per_image);
+    const double l = cta_sum_partials<256>(pairs_per_image, p, 2, r0);
+    const double s = cta_sum_partials<256>(pairs_per_image, p + 1, 2, r1);
+    if (threadIdx.x == 0) {
+        out[2 * blockIdx.x] = (float)(l * inv_n);
+        out[2 * blockIdx.x + 1] = (float)(s * inv_n);
     }
 }
 

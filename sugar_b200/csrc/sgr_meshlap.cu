@@ -24,6 +24,7 @@
 #include <math.h>
 
 #include "sgr_internal.cuh"
+#include "sgr_reduce.cuh"
 
 // The per-face and per-vertex arithmetic is plain C++: tests/test_meshlap_cpu.py compiles this file with
 // -DSGR_MESHLAP_HOST_TEST and runs the same functions on the host against the oracle in float64.
@@ -180,13 +181,6 @@ __global__ void __launch_bounds__(LAP_THREADS) mesh_lap_face_kernel(int F, const
     face_w[f] = lap_face(verts, __ldg(fv), __ldg(fv + 1), __ldg(fv + 2));
 }
 
-__device__ __forceinline__ double lap_warp_sum(double v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // grid-stride over the vertices; per CTA the sum of |y_v| in double
 __global__ void __launch_bounds__(LAP_THREADS) mesh_lap_row_kernel(int method, int V, const float *__restrict__ verts,
                                                                     const int *__restrict__ faces,
@@ -203,32 +197,8 @@ __global__ void __launch_bounds__(LAP_THREADS) mesh_lap_row_kernel(int method, i
         ys[v] = make_float4((float)y.x, (float)y.y, (float)y.z, (float)s);
         t += sqrt(y.x * y.x + y.y * y.y + y.z * y.z);
     }
-    t = lap_warp_sum(t);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = t;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-#pragma unroll
-        for (int w = 0; w < LAP_THREADS / 32; w++) s += red[w];
-        partials[blockIdx.x] = s;
-    }
-}
-
-// one CTA: the per-CTA sums in a fixed order, times 1 / V
-__global__ void __launch_bounds__(1024) mesh_lap_reduce_kernel(int n, double inv_v, const double *__restrict__ partials,
-                                                               float *__restrict__ out)
-{
-    __shared__ double r[1024];
-    const int t = threadIdx.x;
-    double s = 0.0;
-    for (int i = t; i < n; i += 1024) s += partials[i];
-    r[t] = s;
-    __syncthreads();
-    for (int o = 512; o > 0; o >>= 1) {
-        if (t < o) r[t] += r[t + o];
-        __syncthreads();
-    }
-    if (t == 0) out[0] = (float)(r[0] * inv_v);
+    const double s = cta_sum_by_warps<LAP_THREADS>(t, red);
+    if (threadIdx.x == 0) partials[blockIdx.x] = s;
 }
 
 __global__ void __launch_bounds__(LAP_THREADS) mesh_lap_backward_kernel(int method, int V, double inv_v,
@@ -311,7 +281,7 @@ int sgr_mesh_lap_forward(int32_t method, int32_t V, int32_t F, const float *vert
     SGR_LAUNCH(K_MISC, st,
                mesh_lap_row_kernel<<<nb, LAP_THREADS, 0, st>>>(method, V, verts, faces, (const float4 *)face_w,
                                                                 vert_ptr, vert_inc, (float4 *)vert_ys, partials));
-    SGR_LAUNCH(K_MISC, st, mesh_lap_reduce_kernel<<<1, 1024, 0, st>>>(nb, 1.0 / (double)V, partials, loss));
+    SGR_LAUNCH(K_MISC, st, sum_partials_kernel<1024><<<1, 1024, 0, st>>>(nb, 1.0 / (double)V, partials, loss));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }

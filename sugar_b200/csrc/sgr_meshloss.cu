@@ -21,6 +21,7 @@
 #include <math.h>
 
 #include "sgr_internal.cuh"
+#include "sgr_reduce.cuh"
 
 // The per-pair arithmetic is plain C++: tests/test_meshloss_cpu.py compiles this file with
 // -DSGR_MESHLOSS_HOST_TEST and runs the same function on the host against the oracle's float64 autograd.
@@ -90,13 +91,6 @@ SGR_HD double nc_pair(const float *__restrict__ verts, int v0, int v1, int a, in
 
 constexpr int NC_THREADS = 256;
 
-__device__ __forceinline__ double nc_warp_sum(double v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 __global__ void __launch_bounds__(NC_THREADS) mesh_nc_forward_kernel(int Q, const float *__restrict__ verts,
                                                                      const int4 *__restrict__ pairs,
                                                                      double *__restrict__ partials)
@@ -108,32 +102,8 @@ __global__ void __launch_bounds__(NC_THREADS) mesh_nc_forward_kernel(int Q, cons
         const int4 r = __ldg(pairs + q);
         t = nc_pair(verts, r.x, r.y, r.z, r.w, 0.0, nullptr);
     }
-    t = nc_warp_sum(t);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = t;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-#pragma unroll
-        for (int w = 0; w < NC_THREADS / 32; w++) s += red[w];
-        partials[blockIdx.x] = s;
-    }
-}
-
-// one CTA: the per-CTA sums in a fixed order, times 1 / Q
-__global__ void __launch_bounds__(1024) mesh_nc_reduce_kernel(int n, double inv_q, const double *__restrict__ partials,
-                                                              float *__restrict__ out)
-{
-    __shared__ double r[1024];
-    const int t = threadIdx.x;
-    double s = 0.0;
-    for (int i = t; i < n; i += 1024) s += partials[i];
-    r[t] = s;
-    __syncthreads();
-    for (int o = 512; o > 0; o >>= 1) {
-        if (t < o) r[t] += r[t + o];
-        __syncthreads();
-    }
-    if (t == 0) out[0] = (float)(r[0] * inv_q);
+    const double s = cta_sum_by_warps<NC_THREADS>(t, red);
+    if (threadIdx.x == 0) partials[blockIdx.x] = s;
 }
 
 __global__ void __launch_bounds__(NC_THREADS) mesh_nc_pair_grad_kernel(int Q, const float *__restrict__ verts,
@@ -238,7 +208,7 @@ int sgr_mesh_nc_forward(int32_t Q, int32_t V, const float *verts, const int32_t 
     const int nb = nc_blocks(Q);
     SGR_LAUNCH(K_MESH_NC_FWD, st,
                mesh_nc_forward_kernel<<<nb, NC_THREADS, 0, st>>>(Q, verts, (const int4 *)pairs, partials));
-    SGR_LAUNCH(K_MESH_NC_FWD, st, mesh_nc_reduce_kernel<<<1, 1024, 0, st>>>(nb, 1.0 / (double)Q, partials, loss));
+    SGR_LAUNCH(K_MESH_NC_FWD, st, sum_partials_kernel<1024><<<1, 1024, 0, st>>>(nb, 1.0 / (double)Q, partials, loss));
     SGR_CUDA(cudaGetLastError());
     return SGR_OK;
 }

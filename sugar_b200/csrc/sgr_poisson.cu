@@ -20,7 +20,8 @@
 // order; the host reads one scalar per call.
 #include <math.h>
 
-#include "sgr_knn.cuh"
+#include "sgr_reduce.cuh"
+#include "sgr_scan.cuh"
 
 namespace sgr {
 
@@ -303,20 +304,8 @@ __global__ void __launch_bounds__(64) poi_coarsest_kernel(float coeff, float *__
     u[t] = su[t];
 }
 
-// Fixed-order sums: thread (block, tid) takes items block * 256 + tid + m * POI_RED_BLOCKS * 256, a shared-memory tree
-// per block, then one CTA sums the POI_RED_BLOCKS partials by the same tree.
-__device__ __forceinline__ double block_tree_sum(double v, double *sh)
-{
-    const int t = threadIdx.x;
-    sh[t] = v;
-    __syncthreads();
-    for (int w = blockDim.x / 2; w > 0; w >>= 1) {
-        if (t < w) sh[t] += sh[t + w];
-        __syncthreads();
-    }
-    return sh[0];
-}
-
+// Fixed-order sums: thread (block, tid) takes items block * 256 + tid + m * POI_RED_BLOCKS * 256, cta_tree_sum per
+// block, then one CTA sums the POI_RED_BLOCKS partials by the same tree.
 __global__ void __launch_bounds__(256) poi_residual_sq_kernel(int N, float coeff, const float *__restrict__ u,
                                                               const float *__restrict__ b, const float *__restrict__ q,
                                                               double *__restrict__ partial)
@@ -328,14 +317,14 @@ __global__ void __launch_bounds__(256) poi_residual_sq_kernel(int N, float coeff
         const float r = residual_at(u, b, q, N, coeff, (int)(at / ((size_t)N * N)), (int)(at / N % N), (int)(at % N));
         acc += (double)r * r;
     }
-    const double s = block_tree_sum(acc, sh);
+    const double s = cta_tree_sum<256>(acc, sh);
     if (threadIdx.x == 0) partial[blockIdx.x] = s;
 }
 
 __global__ void __launch_bounds__(POI_RED_BLOCKS) poi_final_sum_kernel(double *__restrict__ partial)
 {
     __shared__ double sh[POI_RED_BLOCKS];
-    const double s = block_tree_sum(partial[threadIdx.x], sh);
+    const double s = cta_sum_partials<POI_RED_BLOCKS>(POI_RED_BLOCKS, partial, 1, sh);
     if (threadIdx.x == 0) partial[0] = s;
 }
 
@@ -367,7 +356,7 @@ __global__ void __launch_bounds__(256) poi_interpolate_kernel(int N, const float
         acc += v;
     }
     if (partial) {
-        const double total = block_tree_sum(acc, sh);
+        const double total = cta_tree_sum<256>(acc, sh);
         if (threadIdx.x == 0) partial[blockIdx.x] = total;
     }
 }
@@ -424,11 +413,11 @@ int sgr_poisson_bin(int32_t n, const float *points, int32_t N, float ox, float o
     SGR_CUDA(cudaMemsetAsync(starts, 0, nbins * 4, st));
     SGR_LAUNCH(K_MISC, st, poi_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(n, points, ox, oy, oz, inv_h, N, key[0],
                                                                                 rec[0], starts));
-    exclusive_scan_u32(K_MISC, (int)nbins, starts, starts, block_sums, starts, st);
+    exclusive_scan(K_MISC, nbins, starts, starts, block_sums, starts, st);
     for (int p = 0; p < passes; p++) {
         const int a = p & 1;
         SGR_LAUNCH(K_MISC, st, poi_radix_hist_kernel<<<ntiles, POI_RADIX_TILE, 0, st>>>(n, key[a], 8 * p, ntiles, hist));
-        exclusive_scan_u32(K_MISC, 256 * ntiles, hist, hist, block_sums, hist, st);
+        exclusive_scan(K_MISC, 256 * ntiles, hist, hist, block_sums, hist, st);
         SGR_LAUNCH(K_MISC, st, poi_radix_scatter_kernel<<<ntiles, POI_RADIX_TILE, 0, st>>>(
                                    n, key[a], rec[a], 8 * p, ntiles, hist, key[a ^ 1], rec[a ^ 1]));
     }

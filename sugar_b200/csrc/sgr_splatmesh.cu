@@ -19,7 +19,7 @@
 //                         z < 0, |area| <= pytorch3d's 1e-8 in its NDC units, an empty clipped box) and stores a
 //                         64-byte record: the three barycentric planes relative to the box's corner, the view z's,
 //                         the clipped pixel box and the face id; plus the box's count of 8x8-pixel pieces;
-//   mesh_scan_*_kernel    exclusive scan of the piece counts (three launches, 64-bit offsets);
+//   exclusive_scan        of the piece counts (sgr_scan.cu, three launches, 64-bit offsets);
 //   mesh_fragment_kernel  grid-stride over the pieces, one thread per piece (at most 64 candidate pixels, so a
 //                         background splat that covers half the image is spread over many threads): the piece's face by
 //                         binary search over the offsets, the per-pixel test, and a 64-bit atomicMin of
@@ -36,14 +36,12 @@
 #include <math.h>
 
 #include "sgr_internal.cuh"
+#include "sgr_scan.cuh"
 
 namespace sgr {
 
 constexpr int SPM_THREADS = 256;
 constexpr int PIECE = 8;              // pieces are PIECE x PIECE pixels of a face's clipped box
-constexpr int SCAN_THREADS = 256;
-constexpr int SCAN_ITEMS = 8;         // per thread: one scan block covers 2048 faces
-constexpr int SCAN_BLOCK = SCAN_THREADS * SCAN_ITEMS;
 
 // row-vector transform p @ M[:3,:3] + M[3,:3] of a transposed 4x4 (the rasterizer's viewmatrix convention)
 __device__ __forceinline__ double3 xf_point(const float *__restrict__ m, double x, double y, double z)
@@ -178,85 +176,7 @@ __global__ void __launch_bounds__(SPM_THREADS) mesh_setup_kernel(int F, int V, c
         }
     }
     npieces[f] = n;
-}
-
-// ---- exclusive scan of the piece counts: block sums, one CTA over the block sums, block rescans ----
-__device__ __forceinline__ unsigned long long block_exclusive_scan(unsigned long long v, unsigned long long *warp_tot,
-                                                                   unsigned long long &total)
-{
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned long long incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    if (lane == 31) warp_tot[w] = incl;
-    __syncthreads();
-    unsigned long long before = 0, all = 0;
-#pragma unroll
-    for (int k = 0; k < SCAN_THREADS / 32; k++) {
-        const unsigned long long t = warp_tot[k];
-        before += k < w ? t : 0ull;
-        all += t;
-    }
-    __syncthreads();
-    total = all;
-    return before + incl - v;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) mesh_scan_reduce_kernel(int F, const unsigned *__restrict__ n,
-                                                                        unsigned long long *__restrict__ block_sums)
-{
-    __shared__ unsigned long long warp_tot[SCAN_THREADS / 32];
-    const size_t base = (size_t)blockIdx.x * SCAN_BLOCK + (size_t)threadIdx.x * SCAN_ITEMS;
-    unsigned long long s = 0;
-#pragma unroll
-    for (int k = 0; k < SCAN_ITEMS; k++)
-        if (base + k < (size_t)F) s += n[base + k];
-    unsigned long long total;
-    block_exclusive_scan(s, warp_tot, total);
-    if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
-}
-
-// one CTA: block sums -> exclusive block offsets in place, the grand total into off[F]
-__global__ void __launch_bounds__(SCAN_THREADS) mesh_scan_blocks_kernel(int nb, int F,
-                                                                        unsigned long long *__restrict__ block_sums,
-                                                                        unsigned long long *__restrict__ off)
-{
-    __shared__ unsigned long long warp_tot[SCAN_THREADS / 32];
-    unsigned long long carry = 0;
-    for (int b0 = 0; b0 < nb; b0 += SCAN_THREADS) {
-        const int b = b0 + threadIdx.x;
-        const unsigned long long v = b < nb ? block_sums[b] : 0ull;
-        unsigned long long total;
-        const unsigned long long ex = block_exclusive_scan(v, warp_tot, total);
-        if (b < nb) block_sums[b] = carry + ex;
-        carry += total;
-    }
-    if (threadIdx.x == 0) off[F] = carry;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) mesh_scan_apply_kernel(int F, const unsigned *__restrict__ n,
-                                                                       const unsigned long long *__restrict__ block_offs,
-                                                                       unsigned long long *__restrict__ off)
-{
-    __shared__ unsigned long long warp_tot[SCAN_THREADS / 32];
-    const size_t base = (size_t)blockIdx.x * SCAN_BLOCK + (size_t)threadIdx.x * SCAN_ITEMS;
-    unsigned v[SCAN_ITEMS];
-    unsigned long long s = 0;
-#pragma unroll
-    for (int k = 0; k < SCAN_ITEMS; k++) {
-        v[k] = base + k < (size_t)F ? n[base + k] : 0u;
-        s += v[k];
-    }
-    unsigned long long total;
-    unsigned long long run = block_offs[blockIdx.x] + block_exclusive_scan(s, warp_tot, total);
-#pragma unroll
-    for (int k = 0; k < SCAN_ITEMS; k++) {
-        if (base + k < (size_t)F) off[base + k] = run;
-        run += v[k];
-    }
+    if (f == 0) npieces[F] = 0;
 }
 
 __global__ void __launch_bounds__(SPM_THREADS) mesh_fragment_kernel(int F, int W, const unsigned long long *__restrict__ off,
@@ -319,14 +239,13 @@ struct RasterScratch {
     FaceSetup *rec;
     unsigned *npieces;
     unsigned long long *off, *block_sums, *keys;
-    static int scan_blocks(int F) { return (F + SCAN_BLOCK - 1) / SCAN_BLOCK; }
     static RasterScratch carve(Layout &l, int F, int W, int H)
     {
         RasterScratch s;
         s.rec = l.take<FaceSetup>(F);
-        s.npieces = l.take<unsigned>(F);
+        s.npieces = l.take<unsigned>((size_t)F + 1);  // a zero count past the last face: off[F] is the total
         s.off = l.take<unsigned long long>((size_t)F + 1);
-        s.block_sums = l.take<unsigned long long>((size_t)scan_blocks(F) + 1);
+        s.block_sums = l.take<unsigned long long>(scan_block_sums((size_t)F + 1));
         s.keys = l.take<unsigned long long>((size_t)W * H);
         return s;
     }
@@ -396,14 +315,10 @@ int sgr_mesh_raster(int32_t V, int32_t F, const float *verts, const int64_t *fac
         // pytorch3d drops |area| <= 1e-8 in its NDC units, 2 / min(W, H) per pixel
         const double half = 0.5 * (double)(W < H ? W : H);
         const double area_eps = 1e-8 * half * half;
-        const int nb = RasterScratch::scan_blocks(F);
         SGR_LAUNCH(K_MISC, st,
                    mesh_setup_kernel<<<spm_blocks(F, SPM_THREADS), SPM_THREADS, 0, st>>>(
                        F, V, verts, (const long long *)faces, viewmatrix, projmatrix, W, H, area_eps, s.rec, s.npieces));
-        SGR_LAUNCH(K_MISC, st, mesh_scan_reduce_kernel<<<nb, SCAN_THREADS, 0, st>>>(F, s.npieces, s.block_sums));
-        SGR_LAUNCH(K_MISC, st, mesh_scan_blocks_kernel<<<1, SCAN_THREADS, 0, st>>>(nb, F, s.block_sums, s.off));
-        SGR_LAUNCH(K_MISC, st,
-                   mesh_scan_apply_kernel<<<nb, SCAN_THREADS, 0, st>>>(F, s.npieces, s.block_sums, s.off));
+        exclusive_scan(K_MISC, (size_t)F + 1, s.npieces, s.off, s.block_sums, s.off, st);
         SGR_LAUNCH(K_MISC, st,
                    mesh_fragment_kernel<<<device_sm_count() * 8, SPM_THREADS, 0, st>>>(F, W, s.off, s.rec, s.keys));
     }

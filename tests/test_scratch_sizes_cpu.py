@@ -23,8 +23,8 @@ SIZES = {
     "sgr_l1_ssim_scratch_bytes": [((1, 1, 1, 1), 512), ((2, 3, 17, 9), 512), ((1, 3, 1080, 1920), 196096)],
     "sgr_mesh_nc_forward_scratch_bytes": [((0,), 0), ((1,), 512), ((7,), 512), ((3000000,), 94208)],
     "sgr_mesh_nc_backward_scratch_bytes": [((0,), 0), ((1,), 512), ((7,), 768), ((3000000,), 144000256)],
-    "sgr_mesh_raster_scratch_bytes": [((0, 1, 1), 1024), ((1, 1, 1), 1536), ((7, 17, 9), 2816),
-                                      ((6000000, 1920, 1080), 472612864), ((5, 0, 7), 1536)],
+    "sgr_mesh_raster_scratch_bytes": [((0, 1, 1), 1280), ((1, 1, 1), 1536), ((7, 17, 9), 2816),
+                                      ((6000000, 1920, 1080), 472601344), ((5, 0, 7), 1536)],
 }
 
 REJECTED = {
