@@ -793,6 +793,35 @@ typedef struct SgrAdamSegment {
 } SgrAdamSegment;
 SGR_API int sgr_adam_step(int32_t n_segs, const SgrAdamSegment *segs, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Ground-truth image preparation (sugar_b200/dataset.py): a host-decoded image to the float32 [3,H,W] image the
+ * trainers compare against, byte for byte as the reference prepares it with Pillow and numpy (PILtoTorch after
+ * Image.resize, gaussian_splatting/utils/general_utils.py:21-27; the composites of dataset_readers.py:204-210 and
+ * sugar_scene/cameras.py:102-107):
+ *   src      u8[H_in, W_in, C]   C = 3 (RGB) or 4 (RGBA)
+ *   mode     SGR_IMAGE_PLAIN        the RGB channels as they are (C = 4: only at an unchanged size, the alpha dropped)
+ *            SGR_IMAGE_COMPOSITE    C = 4 over a white (white = 1) or black background in float64:
+ *                                   byte = trunc((c/255 a/255 + bg (1 - a/255)) 255)
+ *            SGR_IMAGE_PREMULTIPLY  C = 4 resized through premultiplied RGBa (Pillow's RGBA resize); the alpha is
+ *                                   resized with the colour and then dropped
+ *   x_bounds i32[W_out, 2], x_coeffs i32[W_out, kx]   Pillow's bicubic tables (xmin, count) and 22-bit fixed-point
+ *   y_bounds i32[H_out, 2], y_coeffs i32[H_out, ky]   weights, as sugar_b200/dataset.py: resample_coeffs builds
+ *                                   them; read only for an axis whose size changes (W_out != W_in, H_out != H_in)
+ *   tmp      u8[H_in, W_out, 4]  the horizontal pass's output when both axes change (3 bytes per pixel used unless
+ *                                   mode is SGR_IMAGE_PREMULTIPLY); not read otherwise and may be NULL
+ *   out      f32[3, H_out, W_out]  u / 255 of each prepared byte (a correctly rounded float32 division)
+ * The horizontal pass runs first, as in Pillow; each pass accumulates in int32 from 1 << 21, shifts by 22 and clamps
+ * to [0, 255].  One launch per pass, none when both sizes are unchanged but a conversion pass.
+ * Limits: every size >= 1, kx, ky >= 1 where their tables are read.
+ * ------------------------------------------------------------------------------------------ */
+#define SGR_IMAGE_PLAIN 0
+#define SGR_IMAGE_COMPOSITE 1
+#define SGR_IMAGE_PREMULTIPLY 2
+SGR_API int sgr_image_prepare(int32_t H_in, int32_t W_in, int32_t C, int32_t mode, int32_t white, int32_t W_out,
+                              int32_t kx, const int32_t *x_bounds, const int32_t *x_coeffs, int32_t H_out, int32_t ky,
+                              const int32_t *y_bounds, const int32_t *y_coeffs, const uint8_t *src, uint8_t *tmp,
+                              float *out, void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */

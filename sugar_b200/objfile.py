@@ -78,8 +78,9 @@ def _unfilter(raw, H, W, bpp):
     return out[1:, 1:].astype(np.uint8)
 
 
-def read_png(path):
-    """-> uint8 [H,W,3]: an 8-bit RGB or RGBA (alpha dropped) PNG without interlacing."""
+def read_png(path, keep_alpha=False):
+    """-> uint8 [H,W,3]: an 8-bit RGB or RGBA (alpha dropped) PNG without interlacing.  With `keep_alpha` an RGBA
+    PNG gives uint8 [H,W,4]."""
     with open(path, "rb") as f:
         buf = f.read()
     if buf[:8] != PNG_SIGNATURE:
@@ -114,7 +115,8 @@ def read_png(path):
     raw = zlib.decompress(b"".join(idat))
     if len(raw) != H * (1 + W * bpp):
         raise ValueError(f"{path}: PNG image data of {len(raw)} bytes, {H * (1 + W * bpp)} expected for {W}x{H}")
-    return np.ascontiguousarray(_unfilter(raw, H, W, bpp)[..., :3])
+    px = _unfilter(raw, H, W, bpp)
+    return np.ascontiguousarray(px if keep_alpha else px[..., :3])
 
 
 # ------------------------------------------------------------------------------------------------------------- .obj I/O
