@@ -41,9 +41,13 @@ optimizer step with the loss as a device tensor and `events`, the dict that coar
 Nothing is read back to the host beyond what the reference reads: the prune's scan and the sampled-Gaussian counts
 the steps read.  `generator` (a CPU torch.Generator, or None for the default one) draws the view order; the SDF
 samples come from the default CUDA generator, as in the reference.
+
+`init_refined_from_mesh` builds refine.py's starting model from an extracted mesh (SuGaR's bound constructor), the
+(raw, mesh) pair train_refined takes.
 """
 import random
 
+import numpy as np
 import torch
 
 from . import knn, steps
@@ -258,6 +262,49 @@ def init_from_points(points, colors, sh_degree=3):
     return dict(points=leaf(xyz.detach().clone()), sh_dc=leaf(features[:, :, 0:1].transpose(1, 2)),
                 sh_rest=leaf(features[:, :, 1:].transpose(1, 2)), densities=leaf(densities), scales=leaf(scales),
                 quaternions=leaf(rots))
+
+
+# surface_triangle_circle_radius of SuGaR's constructor (sugar_model.py:172-212), float64 as numpy computes it
+CIRCLE_RADIUS = {1: 1.0 / 2.0 / np.sqrt(3.0), 3: 1.0 / 2.0 / (np.sqrt(3.0) + 1.0), 4: 1.0 / (4.0 * np.sqrt(3.0)),
+                 6: 1.0 / (4.0 + 2.0 * np.sqrt(3.0))}
+
+
+def init_refined_from_mesh(verts, faces, vertex_colors, n_gaussians_per_surface_triangle, thickness, sh_degree=3):
+    """The refined model bound to a mesh, as SuGaR's constructor builds it for refine.py (sugar_model.py:149-361,
+    learning positions, opacities and scales) -> (raw, mesh): `raw` refine_step's dict of float32 leaf tensors on the
+    vertices' device, `mesh` checkpoint.mesh_namespace's (faces int64, bary, thickness, n, topology).
+
+    verts [V,3] (rounded to float32), faces [F,3] integer, vertex_colors [V,3] in [0, 1] (mcubes.read_mesh_ply's uint8
+    / 255); n Gaussians per face, 1, 3, 4 or 6 (ValueError otherwise); thickness the camera extent / 1e6 in the
+    reference.  In its float32 operation order: scales = log(clamp_min(min edge length * circle radius, 1e-7)) on
+    both in-plane axes of the face's n Gaussians; the complex numbers (1, 0); densities logit(0.1); sh_dc =
+    RGB2SH(the barycentric mix of the face's vertex colours); sh_rest zeros [P,(sh_degree+1)^2-1,3]."""
+    from . import meshbind
+    from .checkpoint import mesh_namespace
+    n = n_gaussians_per_surface_triangle
+    if n not in CIRCLE_RADIUS:
+        raise ValueError(f"n_gaussians_per_surface_triangle must be 1, 3, 4 or 6, got {n!r}")
+    points = torch.as_tensor(verts).float()
+    dev = points.device
+    faces = torch.as_tensor(faces).to(dev)
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point:
+        raise ValueError(f"faces must be an integer [F,3] tensor, got {faces.dtype} {tuple(faces.shape)}")
+    colors_v = torch.as_tensor(vertex_colors).float().to(dev)
+    F, P = faces.shape[0], faces.shape[0] * n
+    bary = meshbind.bary_coords(n, dev)[..., None]                     # [n,3,1]
+    colors = (colors_v[faces][:, None] * bary[None]).sum(dim=-2).reshape(-1, 3)
+    fv = points[faces]
+    scales = (fv - fv[:, [1, 2, 0]]).norm(dim=-1).min(dim=-1)[0] * CIRCLE_RADIUS[n]
+    scales = scales.clamp_min(0.0000001).reshape(F, -1, 1).expand(-1, n, 2).clone().reshape(-1, 2)
+    complex_numbers = torch.zeros(P, 2, device=dev)
+    complex_numbers[:, 0] = 1.0
+    opacity = 0.1 * torch.ones((P, 1), dtype=torch.float, device=dev)
+    leaf = lambda t: t.contiguous().requires_grad_(True)
+    raw = dict(verts=leaf(points.detach().clone()), densities=leaf(torch.log(opacity / (1 - opacity))),
+               scales=leaf(torch.log(scales)), quaternions=leaf(complex_numbers),
+               sh_dc=leaf(((colors - 0.5) / SH_C0).unsqueeze(dim=1)),
+               sh_rest=leaf(torch.zeros(P, (sh_degree + 1) ** 2 - 1, 3, device=dev)))
+    return raw, mesh_namespace(faces, n, thickness, points.shape[0])
 
 
 def train_3dgs(raw, views, spatial_extent, num_iterations=30_000, sh_degree=3, sh_every=1000,
