@@ -822,6 +822,41 @@ SGR_API int sgr_image_prepare(int32_t H_in, int32_t W_in, int32_t C, int32_t mod
                               const int32_t *y_bounds, const int32_t *y_coeffs, const uint8_t *src, uint8_t *tmp,
                               float *out, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * LPIPS, VGG16 v0.1 (the metric of metrics.py, gaussian_splatting/lpipsPyTorch; sugar_b200/lpips.py sequences the
+ * passes).  The N renders x and N ground truths y run through the network as one batch of 2N images, x first.
+ * Activations are NHWC float32 [2N, H, W, C].  conv3x3 runs on the tensor cores: it rounds its input to TF32 and
+ * reads its weights as TF32, so pass them rounded (to nearest, ties away: sugar_b200/lpips.py: tf32_round);
+ * accumulation is float32.  conv1 is float32 throughout.
+ *   weights   the packed blob, sgr_lpips_weight_floats() floats: for each of the 13 convs its weights KRSC
+ *             [Cout, 3, 3, Cin] (TF32-rounded but conv1_1's) then its bias [Cout]; then the five linear vectors
+ *             [64], [128], [256], [512], [512]
+ *   conv1     x, y f32[N, 3, H, W] (values in [0, 1]) -> out [2N, H, W, 64]: z-score (v - mean) / std in float32,
+ *             conv1_1 with zero padding of the z-scored image, bias, ReLU.  2 N H W 64 < 2^31.
+ *   conv3x3   in [B, H, W, Cin] -> out [B, H, W, Cout]: 3x3 conv, stride 1, zero padding 1, bias, ReLU;
+ *             Cin, Cout in {64, 128, 256, 512}; in, weight, out 16-byte aligned; B H W max(Cin, Cout) < 2^31.
+ *   tap       feat [2N, H, W, C], lin f32[C], C in {64, 128, 256, 512}: per pixel of pair n (images n, N + n)
+ *             sum_c lin[c] (fx_c / (|fx| + 1e-10) - fy_c / (|fy| + 1e-10))^2, summed per CTA in double into
+ *             partials (N x the tap's CTA count, from sgr_lpips_scratch_layout); pooled (may be NULL) <- the 2x2 max
+ *             pool [2N, H/2, W/2, C] (floored) of feat.
+ *   reduce    after the five taps of an H x W input: taps f32[N, 5] (may be NULL) <- each tap's mean over its own
+ *             (H >> t) x (W >> t) pixels, out f32[N] <- their sum; fixed summation order (run-to-run identical, and
+ *             the same for an image whatever batch it is in).  H, W >= 16.
+ * Scratch of an H x W input: sgr_lpips_scratch_layout walks its carve and writes offsets[8]: [0], [1] the two
+ * activation buffers (2 N H W 64 floats each), [2 + t] tap t's partials, as byte offsets from `scratch`, and [7] the
+ * bytes to allocate.  Call it with scratch = NULL for the size, then with the allocation for its offsets.
+ * ------------------------------------------------------------------------------------------ */
+SGR_API size_t sgr_lpips_weight_floats(void);
+SGR_API int sgr_lpips_scratch_layout(int32_t N, int32_t H, int32_t W, const void *scratch, size_t *offsets);
+SGR_API int sgr_lpips_conv1(int32_t N, int32_t H, int32_t W, const float *x, const float *y, const float *weight,
+                            const float *bias, float *out, void *stream);
+SGR_API int sgr_lpips_conv3x3(int32_t B, int32_t H, int32_t W, int32_t Cin, int32_t Cout, const float *in,
+                              const float *weight, const float *bias, float *out, void *stream);
+SGR_API int sgr_lpips_tap(int32_t N, int32_t H, int32_t W, int32_t C, const float *feat, const float *lin,
+                          float *pooled, double *partials, void *stream);
+SGR_API int sgr_lpips_reduce(int32_t N, int32_t H, int32_t W, const double *partials, float *taps, float *out,
+                             void *stream);
+
 /* Measurement hooks (bench.py): number of kernels this library has launched in this process;
  * optional CUDA-event bracketing of every launch on its own stream.  sgr_profile_read fills
  * total_ms[kind] / counts[kind] for kind < sgr_num_kernel_kinds() and resets the log. */

@@ -15,7 +15,7 @@ LIB = os.environ.get("SGR_LIB_OUT", os.path.join(HERE, "lib", "libsugar_b200.so"
 SOURCES = ["sgr_api.cu", "sgr_forward.cu", "sgr_backward.cu", "sgr_exchange.cu", "sgr_field.cu", "sgr_normal.cu", "sgr_knn.cu", "sgr_scan.cu", "sgr_meshbind.cu",
            "sgr_peer.cu", "sgr_loss.cu", "sgr_meshloss.cu", "sgr_meshlap.cu", "sgr_splatmesh.cu",
            "sgr_texture.cu", "sgr_mcubes.cu", "sgr_decimate.cu", "sgr_densify.cu", "sgr_poisson.cu", "sgr_compose.cu",
-           "sgr_postprocess.cu", "sgr_adam.cu", "sgr_image.cu"]
+           "sgr_postprocess.cu", "sgr_adam.cu", "sgr_image.cu", "sgr_lpips.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--shared",
